@@ -2,15 +2,16 @@
 """bench.py - images/sec of the IR-SDE reverse-diffusion sampler (BASELINE.json metric).
 
 A "step" is ONE complete chain x_T -> x_0 (T network forwards + T fused updates) over one batch of synthetic LQ images.
-Default workload (the driver's line) = BASELINE config 2: IR-SDE deraining, 8x3x256x256 per GPU, T=100, ConditionalUNet
-nf=64 depth=4, bf16 tcgen05 path, CUDA-graph step replay; weak scaling, every rank owns its own 8 images, no data-path
+Default workload = BASELINE config 2: IR-SDE deraining, 8x3x256x256 per GPU, T=100, ConditionalUNet
+nf=64 depth=4, bf16 wgmma path, CUDA-graph step replay; weak scaling, every rank owns its own 8 images, no data-path
 collective (one weight broadcast before, one gather of x0 after).  The other BASELINE configs are --workload c3 / c4 / c5
 (see WORKLOADS); --precision fp32x3 runs the fp32-accurate tensor-core mode (3 x tf32 split MMA) that meets the 1e-3 bound.
 
   python bench.py --gpus 1 --steps 3 --warmup 3
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
-  python bench.py --impl reference                 # the UNMODIFIED reference (baseline/_ref) on the host cores
-  python bench.py --impl reference --device cuda   # context number: the reference in PyTorch eager on the B200
+  python bench.py --gpus 1 --steps 3 --warmup 3 --dump-outputs DIR   # + DIR/x0.npy: the last timed step's x0 (float32)
+  python bench.py --impl reference                 # the UNMODIFIED reference (oracle/_ref) on the host cores
+  python bench.py --impl reference --device cuda   # context number: the reference in PyTorch eager on the GPU
 """
 import argparse
 import ctypes
@@ -52,7 +53,7 @@ def synth(B, H, W, seed=1234):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -105,40 +106,6 @@ def build_info():
     return d
 
 
-def ncu_traffic_per_launch():
-    """(mean DRAM bytes (read + write) per tcgen05 conv launch, source description) from the newest committed
-    `ncu --set full` capture of this workload (profiles/rNN_conv_tc_ncu_full_one_step.csv + .meta.json), or (None, why).
-    Not measured live: ncu cannot run inside a timed bench.  The description carries the commit / source hash the capture
-    was taken from and whether that equals the build being timed."""
-    import csv
-    import glob
-    files = sorted(glob.glob(os.path.join(ROOT, "profiles", "r*_conv_tc_ncu_full_one_step.csv")))
-    files = [f for f in files if "_v1_" not in f]
-    if not files:
-        return None, "no profiles/r*_conv_tc_ncu_full_one_step.csv"
-    path = files[-1]
-    try:
-        rows = list(csv.DictReader(open(path)))[1:]   # first row holds the units (Mbyte)
-        tot = sum(float(r["dram__bytes_read.sum"]) + float(r["dram__bytes_write.sum"]) for r in rows)
-        meta = {}
-        try:
-            meta = json.load(open(path[:-4] + ".meta.json"))
-        except Exception:
-            pass
-        bi = build_info()
-        same = bool(meta.get("csrc_sha256")) and meta.get("csrc_sha256") == bi.get("csrc_sha256")
-        same_conv = bool(meta.get("conv_tc_sha256")) and meta.get("conv_tc_sha256") == bi.get("conv_tc_sha256")
-        src = ("%s: mean dram read+write bytes per launch over %d launches of one step, ncu --set full; captured from commit %s "
-               "(csrc %s, conv_tc %s); this build: commit %s (csrc %s, conv_tc %s) -> %s" % (
-                   os.path.relpath(path, ROOT), len(rows), meta.get("commit", "?"), meta.get("csrc_sha256", "?"),
-                   meta.get("conv_tc_sha256", "?"), bi.get("commit", "?"), bi.get("csrc_sha256", "?"), bi.get("conv_tc_sha256", "?"),
-                   "same sources" if same else ("same conv kernel sources (conv_tc.cu + common.cuh), other kernels changed" if same_conv
-                                                else "DIFFERENT sources")))
-        return tot * 1e6 / len(rows), src
-    except Exception as e:
-        return None, "unreadable %s: %s" % (path, e)
-
-
 def usable_cores():
     """Host cores this process may actually use: affinity mask capped by the cgroup CPU quota."""
     n = len(os.sched_getaffinity(0)) if hasattr(os, "sched_getaffinity") else (os.cpu_count() or 1)
@@ -148,7 +115,7 @@ def usable_cores():
             n = min(n, max(1, int(float(q) / float(p))))
     except Exception:
         pass
-    # PyTorch's CPU conv stops scaling (and on this pool's 128-thread hosts gets slower) beyond ~32 threads
+    # PyTorch's CPU conv stops scaling (and on 128-thread hosts gets slower) beyond ~32 threads
     return max(1, min(n, 32))
 
 
@@ -171,13 +138,13 @@ def metric_name(wl):
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# reference arm: the UNMODIFIED reference (baseline/_ref, staged by baseline/make_ref.py) - its own IRSDE and
+# reference arm: the UNMODIFIED reference (oracle/_ref, staged by oracle/make_ref.py) - its own IRSDE and
 # ConditionalUNet classes, its own reverse_sde loop.  Falls back to the oracle port only when the staging is absent.
 # ------------------------------------------------------------------------------------------------------------------
 def _reference_objects(wl, device):
-    """(sde, net, kind): the reference's own classes when baseline/_ref is staged, else None (oracle port)."""
+    """(sde, net, kind): the reference's own classes when oracle/_ref is staged, else None (oracle port)."""
     import torch
-    sys.path.insert(0, os.path.join(ROOT, "baseline"))
+    sys.path.insert(0, os.path.join(ROOT, "oracle"))
     try:
         import ref_loader
     except Exception:
@@ -215,7 +182,7 @@ def cpu_reference_sample(wl, steps_per_sample=3, threads=None, objs=None, prewar
             t0 = time.perf_counter()
             getattr(sde, "reverse_" + w["mode"])(xT, T=steps_per_sample)
             dt = time.perf_counter() - t0
-        kind, what = "reference", "the reference's own IRSDE.reverse_%s + ConditionalUNet (baseline/_ref)" % w["mode"]
+        kind, what = "reference", "the reference's own IRSDE.reverse_%s + ConditionalUNet (oracle/_ref)" % w["mode"]
     else:
         from oracle import irsde_oracle as O
         P = O.make_weights(3, 3, nf, depth, seed=0)
@@ -227,7 +194,7 @@ def cpu_reference_sample(wl, steps_per_sample=3, threads=None, objs=None, prewar
             t0 = time.perf_counter()
             O.reverse_chain(sc, net, xT, lq, zs, w["mode"], T=steps_per_sample)
             dt = time.perf_counter() - t0
-        kind, what = "port", "oracle port of the reference (baseline/_ref not staged)"
+        kind, what = "port", "oracle port of the reference (oracle/_ref not staged)"
     s_per_step = dt / steps_per_sample
     return 1.0 / (T * s_per_step), dt, ("%s: %d steps of 1x3x%dx%d (nf=%d depth=%d) on %d threads; img/s extrapolated as "
                                         "1/(T*s_per_step), T=%d" % (what, steps_per_sample, H, W, nf, depth, threads, T)), kind
@@ -264,7 +231,7 @@ def run_reference(args):
 
 
 def run_reference_cuda(args):
-    """Context number (BASELINE.md 3): the reference unchanged in PyTorch eager on one B200 - cuDNN / cuBLAS library kernels,
+    """Context number (BASELINE.md 3): the reference unchanged in PyTorch eager on one GPU - cuDNN / cuBLAS library kernels,
     stock settings (cudnn.allow_tf32 stays at torch's default True, as the reference never touches it) unless --no-tf32."""
     import torch
     wl = args.workload
@@ -275,7 +242,7 @@ def run_reference_cuda(args):
         torch.backends.cuda.matmul.allow_tf32 = False
     objs = _reference_objects(wl, dev)
     if objs is None:
-        print(json.dumps({"impl": "reference", "unavailable": "baseline/_ref not staged"}))
+        print(json.dumps({"impl": "reference", "unavailable": "oracle/_ref not staged"}))
         return
     sde, net = objs
     B = w["B"] if w["scaling"] == "weak" else min(w["B"], w.get("chunk", w["B"]))
@@ -297,15 +264,24 @@ def run_reference_cuda(args):
     line = {"impl": "reference", "device": "cuda", "metric": metric_name(wl), "value": value, "unit": "images/s", "n_gpus": 1,
             "steps": args.steps, "warmup": 1, "ms_per_step": ms, "higher_is_better": True, "scaling": w["scaling"], "vs_baseline": None,
             "dtype": "f32 (cudnn tf32 %s)" % ("off" if args.no_tf32 else "on: torch default"), "data": "synthetic",
-            "config": {"workload": workload_name(wl), "batch": B, "note": "UNMODIFIED reference (baseline/_ref), PyTorch eager on "
-                       "the B200: library kernels only; context, not the CPU baseline"},
+            "config": {"workload": workload_name(wl), "batch": B, "note": "UNMODIFIED reference (oracle/_ref), PyTorch eager on "
+                       "the GPU: library kernels only; context, not the CPU baseline"},
             "finite": bool(torch.isfinite(x0).all())}
     print(json.dumps(line), flush=True)
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# B200 arm
+# native arm (the project's own CUDA kernels)
 # ------------------------------------------------------------------------------------------------------------------
+def dump_outputs(d, outs, rank, world):
+    """The images the timed path returned in its last step (x0, NCHW), float32; one file per rank when sharded."""
+    import numpy as np
+    import torch
+    os.makedirs(d, exist_ok=True)
+    x0 = torch.cat([o.float() for o in outs]).cpu().numpy() if outs else np.zeros((0,), np.float32)
+    np.save(os.path.join(d, "x0.npy" if world == 1 else "x0_rank%d.npy" % rank), x0.astype(np.float32))
+
+
 def _peaks():
     try:
         return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
@@ -321,7 +297,7 @@ def _profile(ctx, _lib, run, nsteps):
     _lib.check(ctx.L.irsde_profile_begin(ctx.h), ctx.h)
     run()
     _lib.check(ctx.L.irsde_profile_end_bytes(ctx.h, ms_a, fl_a, n_a, by_a, ncat), ctx.h)
-    names = ["tcgen05_conv", "simt_conv", "layernorm", "attention", "misc", "update"]
+    names = ["wgmma_conv", "simt_conv", "layernorm", "attention", "misc", "update"]
     bd = {names[i]: {"ms_per_step": ms_a[i] / nsteps, "ops_per_step": n_a[i] / nsteps,
                      "tflops": (fl_a[i] / (ms_a[i] * 1e-3) / 1e12) if ms_a[i] > 0 and fl_a[i] > 0 else None,
                      "algorithmic_gbs": (by_a[i] / (ms_a[i] * 1e-3) / 1e9) if ms_a[i] > 0 and by_a[i] > 0 else None}
@@ -339,7 +315,7 @@ def run_b200(args):
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device; the B200 arm has no CPU fallback (use --impl reference)")
+        raise SystemExit("bench.py: no CUDA device; the native arm has no CPU fallback (use --impl reference)")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     if world > 1:
@@ -482,6 +458,8 @@ def run_b200(args):
     launches = launch_total() - l0
     value = B_glob * args.steps / (ms_total / 1000.0)
     assert all(torch.isfinite(o).all() for o in outs)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, outs, rank, world)
 
     # ---- (2) end to end through the public API with HOST buffers (pinned): H2D of the inputs, the sampler exactly as
     #          test.py drives it (UNet workloads: torch RNG, one randn_like per step), D2H of x0, the final gather
@@ -507,30 +485,29 @@ def run_b200(args):
         ms_a, fl_a, n_a, by_a, breakdown = _profile(ctx, _lib, lambda: chain_resident(prof_steps), prof_steps)
         tot_ms = sum(ms_a)
         if w["kind"] == "unet" and prec in ("bf16", "fp32x3") and ms_a[0] > 0:
-            peak_tf = float(peaks.get("bf16_tflops_sustained", 1400.0))
+            peak_tf = float(peaks.get("bf16_tflops_sustained", 989.0))
             if prec == "fp32x3":
-                peak_tf *= 0.5   # kind::tf32 MMA runs at half the bf16 rate; no measured tf32 GEMM peak on this pool
+                peak_tf *= 0.5   # tf32 wgmma runs at half the bf16 rate
             ach = fl_a[0] / (ms_a[0] * 1e-3) / 1e12
-            traffic, traffic_src = ncu_traffic_per_launch() if (wl == "c2" and prec == "bf16") else (None, "no ncu capture of this workload")
-            roof = {"kernel": "conv_tc_persist_kernel (tcgen05 tap-GEMM conv%s)" % (", 3 x kind::tf32 split MMA" if prec == "fp32x3" else ""),
+            roof = {"kernel": "conv_tc_persist_kernel (wgmma tap-GEMM conv%s)" % (", 3 x tf32 split MMA" if prec == "fp32x3" else ""),
                     "bound": "tensor", "achieved": ach, "peak": peak_tf, "unit": "TFLOP/s", "frac": ach / peak_tf,
-                    "peak_source": ("measured (MEASURED_PEAKS.json bf16_tflops_sustained)" if peaks else "fallback 1.4 PF sustained "
-                                    "(B200_PROFILING.md)") + (" x 0.5 for tf32" if prec == "fp32x3" else ""),
+                    "peak_source": ("measured (MEASURED_PEAKS.json bf16_tflops_sustained)" if peaks else "H100 SXM data sheet, "
+                                    "989 TFLOP/s dense bf16 at 700 W") + (" x 0.5 for tf32" if prec == "fp32x3" else ""),
                     "flops_per_launch": fl_a[0] / n_a[0], "avg_launch_ms": ms_a[0] / n_a[0], "launches": int(n_a[0]),
-                    "share_of_step": ms_a[0] / tot_ms, "traffic": traffic, "traffic_source": traffic_src,
+                    "share_of_step": ms_a[0] / tot_ms,
                     "how": "executed conv FLOPs (x3 MMA passes NOT counted for fp32x3) / summed launch durations; CUDA events "
                            "around each launch, %d sampler steps, non-graph pass after the timed region" % prof_steps}
         elif w["kind"] == "unet" and ms_a[1] > 0:
             ach = fl_a[1] / (ms_a[1] * 1e-3) / 1e12
-            roof = {"kernel": "conv_simt_kernel (fp32 FMA)", "bound": "tensor", "achieved": ach, "peak": 75.0, "unit": "TFLOP/s",
-                    "frac": ach / 75.0, "peak_source": "nominal fp32 FMA peak (no tensor cores on this path)", "traffic": None,
+            roof = {"kernel": "conv_simt_kernel (fp32 FMA)", "bound": "tensor", "achieved": ach, "peak": 67.0, "unit": "TFLOP/s",
+                    "frac": ach / 67.0, "peak_source": "H100 SXM data sheet fp32 FMA peak (no tensor cores on this path)", "traffic": None,
                     "share_of_step": ms_a[1] / tot_ms}
         elif tot_ms > 0:
-            peak_bw = float(peaks.get("hbm_gbs", 6650.0))
+            peak_bw = float(peaks.get("hbm_gbs", 3350.0))
             ach = sum(by_a) / (tot_ms * 1e-3) / 1e9
             roof = {"kernel": "whole NAFNet sampler step (1x1-conv GEMMs, depthwise+gate, LayerNorm: HBM-bound, SURVEY 8 d)",
                     "bound": "hbm", "achieved": ach, "peak": peak_bw, "unit": "GB/s", "frac": ach / peak_bw,
-                    "peak_source": "measured (MEASURED_PEAKS.json hbm_gbs)" if peaks else "fallback 6.65 TB/s", "traffic": None,
+                    "peak_source": "measured (MEASURED_PEAKS.json hbm_gbs)" if peaks else "H100 SXM data sheet, 3.35 TB/s", "traffic": None,
                     "bytes_per_step": sum(by_a) / prof_steps, "ms_per_step": tot_ms / prof_steps,
                     "how": "algorithmic bytes (every op's inputs + outputs + weights once) / summed op durations, CUDA events, "
                            "%d steps on one tile batch" % prof_steps}
@@ -548,7 +525,7 @@ def run_b200(args):
                 "vs_baseline": None, "dtype": {"bf16": "bf16", "fp32": "f32", "fp32x3": "f32 (3 x tf32 split tensor-core MMA)"}[prec],
                 "data": "synthetic",
                 "config": {"workload": workload_name(wl), "global_batch": B_glob, "parallelism": par, "graph": sde.use_graph,
-                           "l2": "per-step activation working set (>4 GB) exceeds the 126 MB L2; no flush needed",
+                           "l2": "per-step activation working set (>1 GB) exceeds the 50 MB L2; no flush needed",
                            "noise": "in-kernel Philox for `value`; torch.randn_like per step (reference RNG order) for e2e"},
                 "clocks": clocks,
                 "e2e": {"value": e2e_value, "unit": "images/s", "h2d_bytes_per_step": nbytes_in, "d2h_bytes_per_step": nbytes_out},
@@ -571,6 +548,7 @@ def main():
     ap.add_argument("--no-tf32", action="store_true", help="reference arm on cuda: disable cuDNN/cuBLAS TF32")
     ap.add_argument("--no-graph", action="store_true")
     ap.add_argument("--no-cpu", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs as DIR/<name>.npy (float32)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

@@ -1,4 +1,4 @@
-"""irsde_b200: B200-native (sm_100a) IR-SDE / Denoising-SDE reverse-diffusion sampler.
+"""irsde_b200: H100-native (sm_90a) IR-SDE / Denoising-SDE reverse-diffusion sampler.
 
 Public surface mirrors the reference (Algolzw/image-restoration-sde):
   * ``IRSDE`` / ``DenoisingSDE``            <- codes/utils/sde_utils.py

@@ -1,6 +1,6 @@
 """ctypes binding of libirsde_b200.so (the C ABI in include/irsde_b200.h).
 
-There is no CPU or PyTorch fallback: if the library is missing, or there is no sm_100 device, calls
+There is no CPU or PyTorch fallback: if the library is missing, or there is no sm_90 device, calls
 raise.  ``load()`` only dlopens (works without a GPU, used by the symbol-export test).
 """
 import ctypes
@@ -10,8 +10,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("IRSDE_B200_LIB") or os.path.join(HERE, "libirsde_b200.so")  # override: A/B of builds
 
 PREC_FP32, PREC_BF16, PREC_FP32X3 = 0, 1, 2
-# name -> irsde_config.precision.  fp32: fp32 storage + SIMT FMA; bf16: tcgen05 bf16 (perf mode); fp32x3: fp32 storage,
-# every conv = 3 x tcgen05.mma.kind::tf32 on hi/lo split operands (tensor cores at the fp32 mode's accuracy)
+# name -> irsde_config.precision.  fp32: fp32 storage + SIMT FMA; bf16: wgmma bf16 (perf mode); fp32x3: fp32 storage,
+# every conv = 3 x tf32 wgmma on hi/lo split operands (tensor cores at the fp32 mode's accuracy)
 PRECISIONS = {"fp32": PREC_FP32, "bf16": PREC_BF16, "fp32x3": PREC_FP32X3}
 NET_CONDITIONAL, NET_DENOISING = 0, 1
 MODE_SDE, MODE_ODE, MODE_POSTERIOR, MODE_DSDE_SDE, MODE_DSDE_ODE = range(5)
@@ -43,7 +43,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             "irsde_b200: %s not found. Build it with `python image-restoration-sde_b200/build.py` "
-            "(needs nvcc with sm_100a support). There is no CPU / PyTorch fallback." % LIB_PATH)
+            "(needs nvcc with sm_90a support). There is no CPU / PyTorch fallback." % LIB_PATH)
     L = ctypes.CDLL(LIB_PATH)
     vp, i32, i64, u64, fp = ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_uint64, ctypes.POINTER(ctypes.c_float)
     L.irsde_create.argtypes = [ctypes.POINTER(Config), ctypes.POINTER(vp)]

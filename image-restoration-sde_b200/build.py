@@ -1,4 +1,4 @@
-"""Build libirsde_b200.so in-tree with nvcc for sm_100a (no JIT cache: the .so travels with the repo)."""
+"""Build libirsde_b200.so in-tree with nvcc for sm_90a (H100; no JIT cache)."""
 import os
 import subprocess
 import sys
@@ -8,7 +8,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libirsde_b200.so")
 SOURCES = ["engine.cu", "conv_simt.cu", "conv_tc.cu", "elementwise.cu", "attention.cu", "nafnet.cu", "imaging.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
          "-cudart", "static"]
 
 
@@ -21,7 +21,7 @@ def _stale():
 
 
 def csrc_sha256():
-    """Hash of the CUDA sources + the C header: names the build a profile was captured from (profiles/*.meta.json)."""
+    """Hash of the CUDA sources + the C header: names the build a bench line was measured on (BUILD_INFO)."""
     import hashlib
     h = hashlib.sha256()
     for f in sorted(os.listdir(CSRC)):
@@ -33,8 +33,8 @@ def csrc_sha256():
 
 
 def conv_tc_sha256(read=None):
-    """Hash of the sources the tcgen05 conv kernel compiles from (conv_tc.cu + common.cuh): a conv capture stays valid across
-    builds that only touch the other kernels."""
+    """Hash of the sources the tensor-core conv kernel compiles from (conv_tc.cu + common.cuh): tells whether two builds run
+    the same conv kernel when only the other kernels changed."""
     import hashlib
     read = read or (lambda f: open(os.path.join(CSRC, f), "rb").read())
     h = hashlib.sha256()
@@ -82,7 +82,7 @@ def build(force=False, verbose=False):
         failed |= p.returncode != 0
     if failed:
         raise RuntimeError("nvcc failed building libirsde_b200.so")
-    cmd = [NVCC, "-shared", "-cudart", "static", "-o", LIB] + objs + ["-ldl", "-lpthread", "-lrt"]
+    cmd = [NVCC, "-shared"] + FLAGS[:2] + ["-cudart", "static", "-o", LIB] + objs + ["-ldl", "-lpthread", "-lrt"]
     subprocess.check_call(cmd)
     _write_build_info()
     return LIB

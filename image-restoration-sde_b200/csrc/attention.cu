@@ -9,8 +9,8 @@
 
 namespace irsde {
 
-// Round-2b kernels of this file, one bit each (IRSDE_HBM_NEW; 0 = the round-2a kernels, kept for same-box A/B runs and as
-// the reference scripts/hbm_probe.py compares against).  IRSDE_HBM_DEFAULT is the setting validated on the GPU.
+// Newer kernels of this file, one bit each (IRSDE_HBM_NEW; 0 = the previous kernels, kept for A/B runs and as the reference
+// the newer ones are compared against).  IRSDE_HBM_DEFAULT is the default setting.
 //   1 = LayerNorm with compile-time lane geometry     2 = la_combine with 128-bit record loads
 //   4 = la_fold with 16 output rows per block          8 = k/v pass with warp-shuffle, branch-free softmax statistics
 //  16 = la_combine with the records spread over 8 warps (takes precedence over 2)
@@ -153,8 +153,7 @@ __global__ void __launch_bounds__(256) layernorm_vec_kernel(const T* __restrict_
   }
 }
 
-// Round-2b LayerNorm.  ncu on the kernel above (profiles/r02_hbm_kernels_ncu_full.csv): 2.9-4.1 TB/s at SM throughput 82-84 % -
-// it is bound by the instructions it ISSUES per 16-byte vector (run-time lane geometry: integer divisions, shuffle loops
+// LayerNorm with compile-time geometry.  The kernel above is bound by the instructions it ISSUES per 16-byte vector (run-time lane geometry: integer divisions, shuffle loops
 // with branches, per-vector bounds checks, IEEE divide / sqrt slow-path scaffolding), not by bytes in flight.  Here the
 // geometry is a template parameter (C == N * LPP * MAXV exactly, lane / LPP are shifts, shuffle trees unrolled), a lane
 // group owns PP pixels so the gain row and the address set-up are shared, the residual row is requested together with x,
@@ -451,8 +450,7 @@ __global__ void __launch_bounds__(256) la_kv_kernel(const T* __restrict__ qkv, i
 }
 
 // One block = 256 ctx entries (8 d-rows x 32 e) of one (image, head); the loops over the <= 64 partial records are fully
-// unrolled so that all their loads are in flight at once: the kernel is pure dependent-load latency (round 1/2 ncu: 17.5 us
-// for 5 MB with 8-deep batches).  Same arithmetic and summation order per entry as before (bit-identical ctx).
+// unrolled so that all their loads are in flight at once: the kernel is pure dependent-load latency.  Same arithmetic and summation order per entry as before (bit-identical ctx).
 __global__ void __launch_bounds__(256) la_combine_kernel(const float* __restrict__ part, float* __restrict__ ctx,
                                                          int N, int nblk) {
   PDL_ENTRY();
@@ -487,8 +485,8 @@ __global__ void __launch_bounds__(256) la_combine_kernel(const float* __restrict
   ctx[(long long)bh * 1024 + tid] = acc / S / (float)N;
 }
 
-// Round-2b merge.  la_combine_kernel above issues 192 scalar requests per thread (1 536 per block / SM): the time (19 us for
-// 5 MB under ncu) is the SM's outstanding-request limit, not latency of a single chain.  Here one WARP owns 4 d-rows of one
+// Wide-load merge.  la_combine_kernel above issues 192 scalar requests per thread (1 536 per block / SM): its time is the
+// SM's outstanding-request limit, not latency of a single chain.  Here one WARP owns 4 d-rows of one
 // (image, head) = 128 ctx entries as one float4 per lane: the 64 records' (m, s) for those rows come in as two float4 loads
 // per lane and are shared through shared memory, and each record's ctx slice is ONE 128-bit request per lane, 32 records
 // in flight.  Per entry the arithmetic and its order are those of la_combine_kernel (bit-identical ctx).
@@ -538,8 +536,8 @@ __global__ void __launch_bounds__(32) la_combine4_kernel(const float* __restrict
       make_float4(acc.x / S / fN, acc.y / S / fN, acc.z / S / fN, acc.w / S / fN);
 }
 
-// Merge with the records spread over warps.  la_combine4_kernel turned the request storm into 40 wide loads per lane but
-// ncu still shows 21.6 us: what remains is ONE warp walking the <= 64 records in sequence (expf + 5 dependent FMAs each).
+// Merge with the records spread over warps.  la_combine4_kernel turned the request storm into 40 wide loads per lane, but
+// what remains is ONE warp walking the <= 64 records in sequence (expf + 5 dependent FMAs each).
 // Here the 8 warps of a block take records w, w + 8, ... (<= 8 each, all loads in flight at once), and warp 0 adds the 8
 // partial (S, ctx) pairs in a fixed order.  The record partition does not depend on the batch, so batch-sharded runs stay
 // bit-identical; the summation order differs from la_combine_kernel (fp32 rounding only).
@@ -674,12 +672,11 @@ __device__ __forceinline__ void mma_bf16_16816(float* c, uint32_t a0, uint32_t a
                : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
 }
 
-// SHFL (round 2b): the softmax statistics of a chunk stay inside a warp.  Lane (qtr = lane / 4, cpl = lane % 4) of warp w
+// SHFL: the softmax statistics of a chunk stay inside a warp.  Lane (qtr = lane / 4, cpl = lane % 4) of warp w
 // owns channel pairs w*4+cpl and 32+w*4+cpl on the 8 pixels px == qtr (mod 8): the running max / sum live in registers
 // (replicated over the 8 qtr lanes), the cross-pixel max and sum are three xor-shuffles each, and the bf16x2 accesses
 // (word = 4*px + pair mod 32) are bank-conflict free.  One chunk then needs TWO block barriers (tile landed / P and alpha
-// visible to the MMA warps) instead of five; ncu on the <false> form: 99 us for 268 MB with SM throughput 58 % - the
-// per-chunk barrier chain, not memory, was the bound.
+// visible to the MMA warps) instead of five: in the <false> form the per-chunk barrier chain, not memory, is the bound.
 template <bool SHFL>
 __global__ void __launch_bounds__(256) la_kv_mma_kernel(const bf16* __restrict__ qkv, int pitch, float* __restrict__ part,
                                                         int N, int nchunks, int nblk) {
@@ -981,7 +978,7 @@ __global__ void la_fold_kernel(const float* __restrict__ ctx, const float* __res
   for (int e = 0; e < 32; ++e) acc += w[e] * cs[h][d][e];
   Mb[((long long)b * C + c) * 128 + k] = __float2bfloat16_rn(acc);
 }
-// Round-2b fold: la_fold_kernel stages the image's whole 16 KB context in shared memory for TWO output rows (2 048 blocks x
+// 16-row fold: la_fold_kernel stages the image's whole 16 KB context in shared memory for TWO output rows (2 048 blocks x
 // 16 KB of L2 reads at C = 512).  Here a block owns 16 output rows: a thread keeps ITS context row (h, d, 0..31) in
 // registers (eight 128-bit loads, no staging), the 16 weight rows go through shared memory once, and all loads of the block
 // are one round trip.  Same per-entry sum order as above (bit-identical Mb).
@@ -1098,9 +1095,8 @@ __global__ void __launch_bounds__(128) fullattn_kernel(const T* __restrict__ qkv
 // online softmax on the accumulator fragments (row max / sum across the 4 lanes of a quad by shuffles), P re-packed in
 // registers as the bf16 A operand of the second product (the FlashAttention-2 register reuse, no smem round trip),
 // O += P V with V fragments from ldmatrix.trans.  K and V tiles stream through a double-buffered cp.async ring.
-// Measured (profiles/r02_fullattn_ncu_full.csv, 1 024 keys, 8 images): 38 us per launch, HMMA pipe 26 %, issue slots
-// 60 % busy at 20 % occupancy: with d = 32 every mma.sync is surrounded by ~6 softmax / re-pack instructions, so the issue
-// slots fill first (MUFU is at ~20 %).  It stays on mma.sync, whose operands come straight from registers.
+// With d = 32 every mma.sync is surrounded by ~6 softmax / re-pack instructions, so the issue slots fill before the tensor
+// pipe does.  It stays on mma.sync, whose operands come straight from registers.
 // ---------------------------------------------------------------------------------------------
 static const int FA_Q = 64, FA_K = 64, FA_P = 40;  // queries / keys per block; smem row pitch (32 + 8 pad, bf16)
 __device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {

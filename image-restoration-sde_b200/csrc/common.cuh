@@ -1,4 +1,4 @@
-// Shared declarations for the irsde_b200 native library (sm_100a only).
+// Shared declarations for the irsde_b200 native library (sm_90a only).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -28,9 +28,9 @@ __device__ __forceinline__ float silu_f(float v) { return v / (1.0f + expf(-v));
 // right away (its CTAs become resident and run their own prologue as SM resources free up) and then blocks until
 // the PREVIOUS kernel has completed and flushed - so all global-memory accesses keep plain stream-order semantics,
 // but the launch latency and the tail of one kernel overlap the ramp of the next.  pdl_launch() attaches the launch
-// attribute (also inside stream capture: the step graph gets programmatic edges).  OPT-IN (IRSDE_PDL=1): on B200 the
-// captured step graph with plain edges measured faster (UNet step 701 vs 706 ms per chain, NAFNet step 2.62 vs
-// 2.70 ms, same box) - early-resident CTAs parked in griddepcontrol.wait cost more than the launch gap they hide.
+// attribute (also inside stream capture: the step graph gets programmatic edges).  OPT-IN (IRSDE_PDL=1): the
+// captured step graph uses plain edges by default; early-resident CTAs parked in griddepcontrol.wait can cost more
+// than the launch gap they hide.
 // Without the attribute the device instructions are no-ops.
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
@@ -174,7 +174,7 @@ void launch_random_states(const float* x0, const float* mu, const float* noise, 
 template <typename T>
 void launch_space_to_depth(const T* in, int in_pitch, T* out, int B, int H, int W, int C, cudaStream_t st);
 
-// ---- tcgen05 tap-GEMM conv (conv_tc.cu) ---------------------------------------------------------
+// ---- tensor-core (wgmma) tap-GEMM conv (conv_tc.cu) ---------------------------------------------------------
 struct TcTap {
   int dh, dw;   // pixel offset of this tap in the A tensor
   int plane;    // 5th coordinate of the A tensor map (space-to-depth plane), 0 otherwise
@@ -185,7 +185,7 @@ TcConvDesc* tc_conv_create(const bf16* in, int in_pitch, int B, int Hin, int Win
                            int nphases /*1 or 4 (upsample phases)*/, const Epilogue& ep, bf16* out, int out_pitch,
                            int Hout, int Wout, std::string* err, int flags = 0);
 enum { TC_FLAG_QSOFTMAX = 1, TC_FLAG_W_PER_IMAGE = 2 };
-// fp32x3 mode (3 x tcgen05.mma.kind::tf32 on hi/lo split fp32 operands, fp32 output); see conv_tc.cu MODE 3
+// fp32x3 mode (3 x tf32 wgmma on hi/lo split fp32 operands, fp32 output); see conv_tc.cu MODE 3
 TcConvDesc* tc_conv_create_f32x3(const float* in_split /*[2][planes][B][H][W][Cin]*/, int B, int Hin, int Win, int Cin, int planes,
                                  const float* wsplit /*[phase*tap][2][Cout_w][Cin]*/, int Cout, int ntaps, const TcTap* taps,
                                  int nphases, const Epilogue& ep, float* out, int out_pitch, int Hout, int Wout, std::string* err);

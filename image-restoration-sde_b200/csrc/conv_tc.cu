@@ -1,5 +1,4 @@
-// tcgen05 "tap-GEMM" convolution for sm_100a: bf16 NHWC activations, bf16 weights, fp32 accumulate in
-// TMEM.
+// Hopper (sm_90a) "tap-GEMM" convolution: bf16 NHWC activations, bf16 weights, fp32 accumulate in registers (wgmma).
 //
 //   D[pixel, n] = sum_{tap} sum_{c} A[pixel + (dh,dw)_tap, c] * Wt[phase][tap][n][c]
 //
@@ -7,17 +6,17 @@
 // (BW*BH = 128), so that for every tap the A operand is ONE TMA box {64 ch, BW, BH} of the NHWC
 // tensor shifted by (dw,dh): zero padding is the TMA out-of-bounds fill, im2col never exists in
 // memory.  The box lands in shared memory as 128 rows x 128 B with the 128B swizzle, which is exactly
-// the canonical K-major UMMA operand layout; the weights tile ({64 ch, BN} of [tap][Cout][Cin]) likewise.
+// the canonical K-major wgmma operand layout; the weights tile ({64 ch, BN} of [tap][Cout][Cin]) likewise.
 // This one kernel serves: 3x3 (9 taps), 1x1 (1 tap), 4x4/s2 (16 taps over 4 space-to-depth planes),
 // nearest-x2-upsample + 3x3 (4 output phases x 4 taps with pre-summed weights).
 //
-// One persistent kernel (conv_tc_persist_kernel<BN, MODE, CG, EKT>), 320 threads: warp 0 = TMEM alloc + TMA producer, warp 1 =
-// MMA issuer (one elected lane), warps 2..9 = epilogue (tcgen05.ld -> bias / (scale+1)*x+shift / SiLU / q-softmax /
-// +residual -> bf16 -> swizzled staging -> TMA bulk store at the channel offset of the destination concat buffer).
-// Pipeline: STAGES-deep smem ring with full/empty mbarriers (tcgen05.commit releases slots), double-buffered TMEM
-// accumulators so the epilogue of tile i overlaps the main loop of tile i+1.  Variants: MODE 0 per-tap boxes, MODE 2 ROWS
-// (3x3, row-window reuse), MODE 3 fp32x3 (3 x kind::tf32 on split fp32 operands), CG = 2 CTA pairs (cta_group::2), EKT =
-// epilogue features compiled in.
+// One persistent kernel (conv_tc_persist_kernel<BN, MODE, EKT>), 288 threads: warps 0..7 = two consumer warpgroups (each
+// issues wgmma.m64nBNk16 for 64 of the 128 pixel rows into its registers, then runs the epilogue: registers -> fp32 staging
+// in shared memory -> bias / (scale+1)*x+shift / SiLU / q-softmax / +residual -> bf16 -> swizzled staging -> TMA bulk store
+// at the channel offset of the destination concat buffer), warp 8 = TMA producer.  Pipeline: STAGES-deep smem ring with
+// full/empty mbarriers (each warpgroup releases a slot once wgmma.wait_group shows its MMAs on it are done); the producer
+// runs ahead into the next tile while the consumers run the epilogue.  Variants: MODE 0 per-tap boxes, MODE 2 ROWS (3x3,
+// row-window reuse), MODE 3 fp32x3 (3 x tf32 wgmma on split fp32 operands), EKT = epilogue features compiled in.
 #include <cuda.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -54,8 +53,8 @@ struct TcParams {
   const float* res_f32; // MODE 3: fp32 residual view
   int lo_plane_off;     // MODE 3: plane offset of the "lo" split of the A tensor ([hi planes][lo planes])
   // tile decode without integer divisions (they cost ~25 instructions + a MUFU.RCP each, five per tile and warp: on layers
-  // with one k-iteration per tile the kernel was ISSUE-bound on them, ncu r02): q = umulhi(x, mg) with mg = ceil(2^32 / d)
-  unsigned mg_tiles_m, mg_tiles_n, mg_tilesW, mg_tilesH, mg_B, mg_pairs_m;  // 0: divisor is 1 (or fast path not provable): see fdiv
+  // with one k-iteration per tile the kernel is ISSUE-bound on them): q = umulhi(x, mg) with mg = ceil(2^32 / d)
+  unsigned mg_tiles_m, mg_tiles_n, mg_tilesW, mg_tilesH, mg_B;  // 0: divisor is 1 (or fast path not provable): see fdiv
   int epi_kind;         // EK_* combination the epilogue is specialised for (EK_GENERIC: every feature checked at run time)
   int n_fast;           // tile order: N tiles of one M tile are consecutive (1x1 convs with several N tiles, see tc_conv_create)
   int tiles_n;
@@ -108,8 +107,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 __device__ __forceinline__ void tma_load_5d(void* smem, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2,
                                             int c3, int c4) {
@@ -128,178 +125,123 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
 
-// SM100 shared-memory matrix descriptor: K-major operand, 128B swizzle, rows of 128 bytes,
-// 8-row core groups 1024 B apart (SBO), descriptor version 1.
-__device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr, uint32_t sbo_bytes = 1024) {
+// sm_90 wgmma shared-memory matrix descriptor: K-major operand, 128B swizzle, rows of 128 bytes, 8-row core groups
+// 1024 B apart (SBO).  Stepping K by 16 bf16 (or 8 tf32) inside the swizzle atom = +32 B on the start address (+2).
+__device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr) {
   uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);        // start address
-  d |= (uint64_t)(0) << 16;                           // leading byte offset (unused for swizzled K-major)
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;   // stride byte offset between 8-row groups
-  d |= (uint64_t)1 << 46;                             // version = 1 (sm_100)
-  d |= (uint64_t)2 << 61;                             // SWIZZLE_128B
+  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);  // start address
+  d |= (uint64_t)1 << 16;                       // leading byte offset (unused for swizzled K-major)
+  d |= (uint64_t)(1024 >> 4) << 32;             // stride byte offset between 8-row groups
+  d |= (uint64_t)1 << 62;                       // SWIZZLE_128B
   return d;
 }
-// kind::f16 instruction descriptor: D=f32, A=B=bf16, both K-major, M x N.
-__device__ __forceinline__ uint32_t make_idesc_bf16(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// Pins the accumulator registers: no read of them is scheduled above a preceding wgmma.wait_group.
+template <int N>
+__device__ __forceinline__ void acc_fence(float* d) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
+// D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, both K-major in shared memory, fp32 accumulator in registers; tf32: K = 8.
+template <int N>
+__device__ void wgmma_bf16(float* d, uint64_t a, uint64_t b);
+template <int N>
+__device__ void wgmma_tf32(float* d, uint64_t a, uint64_t b);
+template <> __device__ __forceinline__ void wgmma_bf16<32>(float* d, uint64_t a, uint64_t b) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(a), "l"(b), "r"(1));
 }
-// kind::tf32 instruction descriptor: D=f32, A=B=tf32 (32-bit containers, 10-bit mantissa), both K-major, M x N; K = 8.
-__device__ __forceinline__ uint32_t make_idesc_tf32(int M, int N) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
+template <> __device__ __forceinline__ void wgmma_bf16<64>(float* d, uint64_t a, uint64_t b) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a), "l"(b), "r"(1));
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t v[32]) {
+template <> __device__ __forceinline__ void wgmma_bf16<128>(float* d, uint64_t a, uint64_t b) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a), "l"(b), "r"(1));
 }
-
-__device__ __forceinline__ void tmem_ld32_async(uint32_t taddr, uint32_t v[32]) {
+template <> __device__ __forceinline__ void wgmma_bf16<256>(float* d, uint64_t a, uint64_t b) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr));
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(a), "l"(b), "r"(1));
 }
-// The registers are tied to the wait ("+r") so the compiler cannot schedule their consumers above it.
-__device__ __forceinline__ void tmem_ld_wait(uint32_t v[32]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(v[0]), "+r"(v[1]), "+r"(v[2]), "+r"(v[3]), "+r"(v[4]), "+r"(v[5]), "+r"(v[6]), "+r"(v[7]), "+r"(v[8]),
-                 "+r"(v[9]), "+r"(v[10]), "+r"(v[11]), "+r"(v[12]), "+r"(v[13]), "+r"(v[14]), "+r"(v[15]), "+r"(v[16]),
-                 "+r"(v[17]), "+r"(v[18]), "+r"(v[19]), "+r"(v[20]), "+r"(v[21]), "+r"(v[22]), "+r"(v[23]), "+r"(v[24]),
-                 "+r"(v[25]), "+r"(v[26]), "+r"(v[27]), "+r"(v[28]), "+r"(v[29]), "+r"(v[30]), "+r"(v[31])
-               :
-               : "memory");
-}
-
-// ---- CTA-pair (cta_group::2) variants: per-tap BN = 256 layers, opt-in / auto (g_pair) ----------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// Executed by both CTAs of the pair: the data lands in the issuing CTA's shared memory, the transaction bytes are
-// counted on the LEADER's barrier (clearing the CTA-rank bit of the shared::cluster address selects the even CTA).
-constexpr uint32_t PAIR_PEER_MASK = 0xFEFFFFFFu;
-__device__ __forceinline__ void tma_load_5d_pair(void* smem, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2,
-                                                 int c3, int c4) {
+template <> __device__ __forceinline__ void wgmma_tf32<32>(float* d, uint64_t a, uint64_t b) {
   asm volatile(
-      "cp.async.bulk.tensor.5d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
-      ::"r"(smem_u32(smem)), "l"(map), "r"(smem_u32(bar) & PAIR_PEER_MASK), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(a), "l"(b), "r"(1));
 }
-__device__ __forceinline__ void tma_load_3d_pair(void* smem, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2) {
+template <> __device__ __forceinline__ void wgmma_tf32<64>(float* d, uint64_t a, uint64_t b) {
   asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(smem_u32(smem)), "l"(map), "r"(smem_u32(bar) & PAIR_PEER_MASK), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a), "l"(b), "r"(1));
 }
-__device__ __forceinline__ void umma_bf16_pair(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
+template <> __device__ __forceinline__ void wgmma_tf32<128>(float* d, uint64_t a, uint64_t b) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
-      : "memory");
-}
-// one commit arrives on the barrier at this offset in BOTH CTAs of the pair
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(smem_u32(bar)), "h"((uint16_t)3)
-               : "memory");
-}
-// arrive on the LEADER's copy of a barrier from either CTA of the pair
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t* bar) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, 0;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}"
-      ::"r"(smem_u32(bar))
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a), "l"(b), "r"(1));
 }
 
 constexpr int A_STAGE_BYTES = 128 * 128;  // 128 pixel rows x 64 bf16
 
 // =====================================================================================================
-// Persistent kernel: one CTA per SM loops over output tiles.  The TMEM accumulator is
-// double buffered (2 x BN columns) so the epilogue of tile i overlaps the MMA main loop of tile i+1,
-// the smem ring is as deep as 192 KB allows (BN=256: 4, BN=128: 6, BN<=64: 8 stages) to cover TMA
-// latency, and the prologue (barrier init, TMEM alloc, descriptor prefetch) is paid once per SM.
+// Persistent kernel: one CTA per SM loops over output tiles.  The smem ring is as deep as the 227 KB of shared memory
+// allows (at most 8 stages) to cover TMA latency, and the prologue (barrier init, descriptor prefetch) is paid once per SM.
 // =====================================================================================================
 //
 // ROWS mode (default for 3x3 stride-1 convs with BN <= 128): a stage is ONE TMA box of (BH+2) image rows x BW pixels
 // for a given horizontal shift dw, plus the three weight tiles of the taps (dh=-1,0,1; dw).  The three vertical taps
 // read 1024-byte-ALIGNED row windows of the same box (window dh starts (dh+1)*BW pixel rows in), so the A operand
-// is fetched 3x instead of 9x per 64-channel chunk with ordinary aligned UMMA descriptors, and one full/empty
-// barrier round covers 12 MMAs.
-constexpr int TF3_SEG = 2;  // fp32x3: k-iterations (of 32 channels, 12 MMAs each) accumulated in TMEM before a flush to registers
+// is fetched 3x instead of 9x per 64-channel chunk with ordinary aligned wgmma descriptors, and one full/empty
+// barrier round covers 12 MMAs per warpgroup.
+constexpr int TF3_SEG = 2;  // fp32x3: k-iterations (of 32 channels, 12 MMAs each) accumulated from zero before a fp32 sum
 constexpr int ROWS_A_SLOT = 20 * 1024;  // (8+2) rows x 16 px x 128 B (or 18 x 8 px for narrow images)
+constexpr int ACC_PITCH = 68;           // fp32 accumulator staging row: 64 columns + 4 (conflict-free 16-byte row reads)
+constexpr int SMEM_LIMIT = 232448;      // 227 KB: the opt-in shared memory per block of sm_90
 
 // MODE 3 "fp32x3" (the fp32-accurate tensor-core mode, SURVEY 7 "Parity vs precision"): operands are fp32 tensors that were
 // split into hi = rn_tf32(x) and lo = rn_tf32(x - hi) (|x - hi - lo| <= 2^-22 |x|); a K chunk is 32 fp32 channels = the same
-// 128-byte swizzled row as 64 bf16 channels; per chunk the MMA warp issues A_hi*W_hi + A_lo*W_hi + A_hi*W_lo as three
-// groups of four tcgen05.mma.kind::tf32 (K=8) into the SAME fp32 TMEM accumulator (the dropped lo*lo term is 2^-22 relative).
+// 128-byte swizzled row as 64 bf16 channels; per chunk each warpgroup issues A_hi*W_hi + A_lo*W_hi + A_hi*W_lo as three
+// groups of four tf32 wgmma (K=8) into the SAME fp32 accumulator (the dropped lo*lo term is 2^-22 relative).
 // The epilogue keeps everything in fp32 (IEEE SiLU, fp32 residual, fp32 NHWC / NCHW stores).
-// CG = 2: CTA pair (cta_group::2) - a cluster of two CTAs computes a 256-pixel x 256-channel tile with M = 256 MMAs issued by
-// the leader; each CTA stages its own 128 pixels of A and HALF of the weight tile (32 KB instead of 48 KB per k-iteration
-// and SM: the BN = 256 layers were L2->smem feed bound, MMA warp ~40 % of the time on the `full` barrier).
-template <int BN, int MODE, int CG = 1>
+template <int BN, int MODE>
 struct TcCfgP {
   static constexpr bool ROWS = MODE == 2;
   static constexpr bool TF3 = MODE == 3;
-  static constexpr int B_STAGE_BYTES = BN * 128 / CG;
-  // G consecutive k-iterations (64-channel chunks) share one full/empty barrier round, which amortises the
-  // mbarrier wait + tcgen05.commit of the single MMA-issuing thread over 4*G MMAs (matters for narrow N tiles)
-  static constexpr int G = 1;  // measured: G=2 trades issue overhead for coarser prefetch granularity; no net gain
-  // Epilogue staging for the TMA stores: one 2 KB tile per epilogue warp.  (Two tiles per warp - so that a warp need not
-  // wait for its previous bulk store to finish reading the tile - were measured in round 2, same-box ABAB: no change;
-  // the store-heavy 1x1 convs are bound by L2 traffic (A re-read per N tile + weight tile re-fetched per output tile),
-  // not by the store latency.  STG_BUFS = 2 still works where shared memory allows it.)
+  static constexpr int B_STAGE_BYTES = BN * 128;
+  // Epilogue staging for the TMA stores: one 2 KB tile per consumer warp (STG_BUFS = 2 alternates two tiles per warp).
   static constexpr int STG_BUFS = TF3 ? 0 : 1;
-  static constexpr int STAGES = CG == 2 ? 6 : TF3 ? (BN == 128 ? 3 : (BN == 64 ? 4 : 5))
-                                : ROWS ? (BN == 128 ? 3 : (BN == 64 ? 4 : 5))
-                                       : (BN == 256 ? 4 : (BN == 128 ? 6 : 8));
   static constexpr int BSUB = ROWS ? 3 : (TF3 ? 2 : 1);  // weight tiles per stage
-  static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;  // per k-iteration (mode 0)
-  static constexpr int A_BYTES = TF3 ? STAGES * 2 * A_STAGE_BYTES
-                                     : (ROWS ? STAGES * ROWS_A_SLOT : STAGES * G * A_STAGE_BYTES);
-  static constexpr int EPI_FLOATS = 3 * BN;
-  static constexpr int STG_BYTES = STG_BUFS * 8 * 2048;  // per epilogue warp: STG_BUFS 32 rows x 64 B staging tiles for TMA stores
-  static constexpr int SMEM_BYTES = 1024 + A_BYTES + STAGES * G * BSUB * B_STAGE_BYTES + STG_BYTES + EPI_FLOATS * 4 + 512;
-  static_assert(SMEM_BYTES <= 232448, "over the 227 KB per-CTA shared memory limit");
-  static constexpr int TMEM_COLS = 2 * BN < 32 ? 32 : 2 * BN;
+  static constexpr int A_SLOT = TF3 ? 2 * A_STAGE_BYTES : (ROWS ? ROWS_A_SLOT : A_STAGE_BYTES);
+  static constexpr int STAGE_BYTES = A_SLOT + BSUB * B_STAGE_BYTES;
+  static constexpr int EPI_FLOATS = 2 * BN;
+  static constexpr int STG_BYTES = STG_BUFS * 8 * 2048;  // per consumer warp: STG_BUFS 32 rows x 64 B staging tiles
+  static constexpr int ACC_BYTES = 2 * 64 * ACC_PITCH * 4;  // fp32 staging: 64 rows x 64 columns per warpgroup
+  static constexpr int FIXED_BYTES = 1024 + STG_BYTES + ACC_BYTES + EPI_FLOATS * 4 + 256;
+  static constexpr int STAGES_FIT = (SMEM_LIMIT - FIXED_BYTES) / STAGE_BYTES;
+  static constexpr int STAGES = STAGES_FIT > 8 ? 8 : STAGES_FIT;
+  static constexpr int A_BYTES = STAGES * A_SLOT;
+  static constexpr int SMEM_BYTES = FIXED_BYTES + STAGES * STAGE_BYTES;
+  static_assert(STAGES >= 2, "shared memory holds fewer than two pipeline stages");
+  static_assert(SMEM_BYTES <= SMEM_LIMIT, "over the 227 KB per-CTA shared memory limit");
 };
 
 // One elected lane of a converged warp (the compiler recognises elect.sync and emits straight-line uniform
@@ -358,24 +300,6 @@ __device__ __forceinline__ TileCoord decode_tile(const TcParams& P, int tile, in
   return t;
 }
 
-// CTA pair: pair tile `pt` covers the m-tiles 2*mp and 2*mp+1 (one per CTA rank) of one N tile.  An odd tail leaves the
-// second CTA without pixels: it still runs the whole protocol on an out-of-range image index (TMA loads zero-fill,
-// TMA stores are clipped).
-__device__ __forceinline__ TileCoord decode_pair_tile(const TcParams& P, int pt, int rank, int tiles_m, int BN) {
-  const int pairs_m = (tiles_m + 1) >> 1;
-  const int q = fdiv(pt, pairs_m, P.mg_pairs_m);
-  const int mp = pt - q * pairs_m;
-  const int m_idx = 2 * mp + rank;
-  TileCoord t;
-  t.n0 = q * BN;
-  if (m_idx >= tiles_m) {
-    t.b = P.B; t.phase = 0; t.py = 0; t.px = 0; t.h0 = 0; t.w0 = 0;
-    return t;
-  }
-  decode_m(P, m_idx, t);
-  return t;
-}
-
 #define DBG_WAIT(ctr, bar, par)                 \
   do {                                          \
     if (P.dbg) {                                \
@@ -387,323 +311,240 @@ __device__ __forceinline__ TileCoord decode_pair_tile(const TcParams& P, int pt,
     }                                           \
   } while (0)
 
-// EKT: EK_* features the epilogue is compiled for.  Only the per-tap BN <= 128 instantiations that serve the 1x1 convs with one
-// or two k-iterations per tile (res_conv: 0, to_qkv: EK_QSM, to_out: EK_AFF) are specialised - there the kernel is issue-bound
-// on epilogue instructions; everything else runs EK_GENERIC (an in-kernel switch over all kinds made ptxas spill 3-4 KB).
-template <int BN, int MODE, int CG = 1, int EKT = 16 /* EK_GENERIC */>
-__global__ void __launch_bounds__(320, 1) conv_tc_persist_kernel(const __grid_constant__ CUtensorMap map_a,
+
+// EKT: EK_* features the epilogue is compiled for.  Only the per-tap and ROWS instantiations that serve the common layer kinds
+// (res_conv: 0, to_qkv: EK_QSM, to_out: EK_AFF, ResBlock convs: EK_AFF|EK_SILU, EK_SILU|EK_RES) are specialised - there the
+// kernel is issue-bound on epilogue instructions; everything else runs EK_GENERIC (every feature checked at run time).
+template <int BN, int MODE, int EKT = 16 /* EK_GENERIC */>
+__global__ void __launch_bounds__(288, 1) conv_tc_persist_kernel(const __grid_constant__ CUtensorMap map_a,
                                                                  const __grid_constant__ CUtensorMap map_b,
                                                                  const __grid_constant__ OutMaps map_o,
                                                                  const __grid_constant__ TcParams P, int tiles_m,
                                                                  int num_tiles) {
-  using Cfg = TcCfgP<BN, MODE, CG>;
+  using Cfg = TcCfgP<BN, MODE>;
   constexpr bool ROWS = Cfg::ROWS;
   constexpr bool TF3 = Cfg::TF3;
   constexpr int STAGES = Cfg::STAGES;
-  static_assert(CG == 1 || (CG == 2 && MODE == 0 && BN == 256), "the CTA-pair variant exists for per-tap mode, BN = 256");
+  constexpr int NACC = BN / 2;  // accumulator registers per thread: m64 x BN per warpgroup
   pdl_trigger();  // the next kernel may be scheduled; this one's prologue below touches no global memory
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* smem_a = smem;                       // A ring
   uint8_t* smem_b = smem + Cfg::A_BYTES;
-  uint8_t* smem_stg = smem_b + STAGES * Cfg::G * Cfg::BSUB * Cfg::B_STAGE_BYTES;  // 1024-aligned
-  float* s_epi = reinterpret_cast<float*>(smem_stg + Cfg::STG_BYTES);
+  uint8_t* smem_stg = smem_b + STAGES * Cfg::BSUB * Cfg::B_STAGE_BYTES;  // 1024-aligned
+  float* s_acc = reinterpret_cast<float*>(smem_stg + Cfg::STG_BYTES);
+  float* s_epi = s_acc + Cfg::ACC_BYTES / 4;
   uint64_t* bars = reinterpret_cast<uint64_t*>(s_epi + Cfg::EPI_FLOATS);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + STAGES;
-  uint64_t* tfull_bar = bars + 2 * STAGES;       // [2] accumulator ready
-  uint64_t* tempty_bar = bars + 2 * STAGES + 2;  // [2] accumulator drained
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 8);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int KI = P.ntaps * P.kchunks;
-  // CTA pair (CG == 2): blockIdx.x = 2 * cluster + rank; `num_tiles` counts pair tiles; both CTAs walk the same pair tiles
-  const int crank = CG == 2 ? (int)cluster_ctarank() : 0;
-  const int tile_first = CG == 2 ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-  const int tile_step = CG == 2 ? (int)(gridDim.x >> 1) : (int)gridDim.x;
-  auto tile_coord = [&](int tile) -> TileCoord {
-    if constexpr (CG == 2) return decode_pair_tile(P, tile, crank, tiles_m, BN);
-    else return decode_tile(P, tile, tiles_m, BN);
-  };
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tfull_bar[a], 1);
-      mbar_init(&tempty_bar[a], 8 * CG);  // one arrive per epilogue warp (of both CTAs of a pair, on the leader)
+      mbar_init(&empty_bar[s], 2);  // one arrive per consumer warpgroup
     }
     fence_barrier_init();
   }
-  if (warp == 0) {
-    if (lane == 0) {
-      tma_prefetch_desc(&map_a);
-      tma_prefetch_desc(&map_b);
-    }
-    __syncwarp();
-    if constexpr (CG == 2) {  // collective over the pair: the same warp of both CTAs, same destination offset
-      asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                   "n"(Cfg::TMEM_COLS)
-                   : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    } else {
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                   "n"(Cfg::TMEM_COLS)
-                   : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
+  if (warp == 8 && lane == 0) {
+    tma_prefetch_desc(&map_a);
+    tma_prefetch_desc(&map_b);
   }
-  tc_fence_before();
   __syncthreads();
-  if constexpr (CG == 2) cluster_sync_all();  // both CTAs' barriers are initialised before any remote arrive / TMA signal
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // barriers, TMEM and descriptors are ready: from here on global memory written by the previous kernel is read
+  // barriers and descriptors are ready: from here on global memory written by the previous kernel is read
   // (activations, the device step counter behind P.t_ptr) and buffers it may still be reading are overwritten
   pdl_wait();
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ================= TMA producer (whole warp loops; one elected lane issues) =================
-    {
-      int it = 0;
-      long long w_prod = 0, t_start = clock64();
-      for (int tile = tile_first; tile < num_tiles; tile += tile_step) {
-        const TileCoord t = tile_coord(tile);
-        if constexpr (TF3) {
-          for (int ki = 0; ki < KI; ++ki, ++it) {
-            const int s = it % STAGES;
-            if (it >= STAGES) DBG_WAIT(w_prod, &empty_bar[s], ((it / STAGES) - 1) & 1);
-            if (elect_one()) {
-              const int tap = ki / P.kchunks, kc = ki - tap * P.kchunks;
-              const int dh = P.taps[tap].dh + (P.nphases == 4 ? t.py : 0);
-              const int dw = P.taps[tap].dw + (P.nphases == 4 ? t.px : 0);
-              const int wt = (t.phase * P.ntaps + tap) * 2;
-              mbar_expect_tx(&full_bar[s], 2 * A_STAGE_BYTES + 2 * Cfg::B_STAGE_BYTES);
-              tma_load_5d(smem_a + (s * 2 + 0) * A_STAGE_BYTES, &map_a, &full_bar[s], kc * 32, t.w0 + dw, t.h0 + dh, t.b, P.taps[tap].plane);
-              tma_load_5d(smem_a + (s * 2 + 1) * A_STAGE_BYTES, &map_a, &full_bar[s], kc * 32, t.w0 + dw, t.h0 + dh, t.b,
-                          P.taps[tap].plane + P.lo_plane_off);
-              tma_load_3d(smem_b + (s * 2 + 0) * Cfg::B_STAGE_BYTES, &map_b, &full_bar[s], kc * 32, t.n0, wt);
-              tma_load_3d(smem_b + (s * 2 + 1) * Cfg::B_STAGE_BYTES, &map_b, &full_bar[s], kc * 32, t.n0, wt + 1);
-            }
-            __syncwarp();
-          }
-        } else if constexpr (ROWS) {
-          for (int kc = 0; kc < P.kchunks; ++kc) {
-            for (int dwi = 0; dwi < 3; ++dwi, ++it) {
-              const int s = it % STAGES;
-              if (it >= STAGES) DBG_WAIT(w_prod, &empty_bar[s], ((it / STAGES) - 1) & 1);
-              if (elect_one()) {
-                mbar_expect_tx(&full_bar[s], P.rows_a_bytes + 3 * Cfg::B_STAGE_BYTES);
-                tma_load_5d(smem_a + s * ROWS_A_SLOT, &map_a, &full_bar[s], kc * 64, t.w0 + dwi - 1, t.h0 - 1, t.b, 0);
-#pragma unroll
-                for (int j = 0; j < 3; ++j)  // taps (dh = j-1, dw = dwi-1): index (dh+1)*3 + (dw+1)
-                  tma_load_3d(smem_b + (s * 3 + j) * Cfg::B_STAGE_BYTES, &map_b, &full_bar[s], kc * 64, t.n0, j * 3 + dwi);
-              }
-              __syncwarp();
-            }
-          }
-        } else {
-          constexpr int G = Cfg::G;
-          for (int g0 = 0; g0 < KI; g0 += G, ++it) {
-            const int s = it % STAGES;
-            if (it >= STAGES) DBG_WAIT(w_prod, &empty_bar[s], ((it / STAGES) - 1) & 1);
-            if (elect_one()) {
-              const int n = (KI - g0) < G ? (KI - g0) : G;
-              if constexpr (CG == 2) {
-                // the leader's barrier collects both CTAs' bytes: own 128 pixels of A + own half (128 channels) of B, each
-                if (crank == 0) mbar_expect_tx(&full_bar[s], 2 * n * Cfg::STAGE_BYTES);
-#pragma unroll
-                for (int j = 0; j < G; ++j) {
-                  if (j < n) {
-                    const int ki = g0 + j, tap = ki / P.kchunks, kc = ki - tap * P.kchunks;
-                    const int dh = P.taps[tap].dh + (P.nphases == 4 ? t.py : 0);
-                    const int dw = P.taps[tap].dw + (P.nphases == 4 ? t.px : 0);
-                    tma_load_5d_pair(smem_a + (s * G + j) * A_STAGE_BYTES, &map_a, &full_bar[s], kc * 64, t.w0 + dw, t.h0 + dh,
-                                     t.b, P.taps[tap].plane);
-                    tma_load_3d_pair(smem_b + (s * G + j) * Cfg::B_STAGE_BYTES, &map_b, &full_bar[s], kc * 64,
-                                     t.n0 + crank * (BN / 2), t.phase * P.ntaps + tap);
-                  }
-                }
-              } else {
-                mbar_expect_tx(&full_bar[s], n * Cfg::STAGE_BYTES);
-#pragma unroll
-                for (int j = 0; j < G; ++j) {
-                  if (j < n) {
-                    const int ki = g0 + j, tap = ki / P.kchunks, kc = ki - tap * P.kchunks;
-                    const int dh = P.taps[tap].dh + (P.nphases == 4 ? t.py : 0);
-                    const int dw = P.taps[tap].dw + (P.nphases == 4 ? t.px : 0);
-                    tma_load_5d(smem_a + (s * G + j) * A_STAGE_BYTES, &map_a, &full_bar[s], kc * 64, t.w0 + dw, t.h0 + dh, t.b,
-                                P.taps[tap].plane);
-                    tma_load_3d(smem_b + (s * G + j) * Cfg::B_STAGE_BYTES, &map_b, &full_bar[s], kc * 64, t.n0,
-                                t.phase * P.ntaps + tap + (P.w_per_image ? t.b : 0));
-                  }
-                }
-              }
-            }
-            __syncwarp();
-          }
-        }
-      }
-      if (P.dbg && lane == 0) { P.dbg[blockIdx.x * 8 + 0] = (unsigned long long)w_prod; P.dbg[blockIdx.x * 8 + 1] = (unsigned long long)(clock64() - t_start); }
-    }
-  } else if (warp == 1) {
-    // ================= MMA issuer (whole warp loops; one elected lane issues) =================
-    {
-      const uint32_t idesc = TF3 ? make_idesc_tf32(128, BN) : make_idesc_bf16(128 * CG, BN);  // pair: M = 256 over both CTAs' lanes
-      int it = 0, lt = 0;
-      long long w_full = 0, w_tempty = 0, t_start = clock64();
+    int it = 0;
+    long long w_prod = 0, t_start = clock64();
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      const TileCoord t = decode_tile(P, tile, tiles_m, BN);
       if constexpr (TF3) {
-        // fp32x3: the K loop of a tile is cut into SEGMENTS of TF3_SEG k-iterations; each segment accumulates from zero in
-        // one of the two TMEM buffers and is handed to the epilogue warps, which sum the segments in fp32 registers with
-        // round-to-nearest adds.  Reason (measured, profiles/ + tests/test_gpu_fp32x3.py): the tensor core's accumulator
-        // update truncates, so a single TMEM accumulation over n MMAs drifts by ~n * 2^-26 relative - 3e-5 per layer at
-        // K = 13 824 (5 184 MMAs), 70x the error of the fp32 FMA path.  24 MMAs per segment (TF3_SEG = 2) keep it at the fp32 FMA path's own level;
-        // TF3_SEG = 8 measured 9x that level at nf=64 (2.3e-5 vs 2.6e-6 relative RMS at the last layer).
-        int st = 0;  // segments issued by this CTA (TMEM buffer = st & 1)
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-          for (int k0 = 0; k0 < KI; k0 += TF3_SEG, ++st) {
-            const int acc = st & 1;
-            if (st >= 2) DBG_WAIT(w_tempty, &tempty_bar[acc], ((st >> 1) - 1) & 1);  // epilogue drained this buffer
-            tc_fence_after();
-            const uint32_t tmem_d = tmem_base + (uint32_t)(acc * BN);
-            const int k1 = k0 + TF3_SEG < KI ? k0 + TF3_SEG : KI;
-            for (int ki = k0; ki < k1; ++ki, ++it) {
-              const int s = it % STAGES;
-              DBG_WAIT(w_full, &full_bar[s], (it / STAGES) & 1);
-              tc_fence_after();
-              if (elect_one()) {
-                const uint64_t a_hi = make_sw128_desc(smem_u32(smem_a + (s * 2 + 0) * A_STAGE_BYTES));
-                const uint64_t a_lo = make_sw128_desc(smem_u32(smem_a + (s * 2 + 1) * A_STAGE_BYTES));
-                const uint64_t b_hi = make_sw128_desc(smem_u32(smem_b + (s * 2 + 0) * Cfg::B_STAGE_BYTES));
-                const uint64_t b_lo = make_sw128_desc(smem_u32(smem_b + (s * 2 + 1) * Cfg::B_STAGE_BYTES));
-                // the two small cross terms first, the dominant hi*hi product last
-#pragma unroll
-                for (int k = 0; k < 4; ++k)  // 4 x (K=8 tf32) per 32-channel chunk: +32 B inside the swizzle atom
-                  umma_tf32(tmem_d, a_lo + (uint64_t)(k * 2), b_hi + (uint64_t)(k * 2), idesc, (ki > k0 || k > 0) ? 1u : 0u);
-#pragma unroll
-                for (int k = 0; k < 4; ++k) umma_tf32(tmem_d, a_hi + (uint64_t)(k * 2), b_lo + (uint64_t)(k * 2), idesc, 1u);
-#pragma unroll
-                for (int k = 0; k < 4; ++k) umma_tf32(tmem_d, a_hi + (uint64_t)(k * 2), b_hi + (uint64_t)(k * 2), idesc, 1u);
-                umma_commit(&empty_bar[s]);
-              }
-              __syncwarp();
-            }
-            if (elect_one()) umma_commit(&tfull_bar[acc]);
-            __syncwarp();
+        for (int ki = 0; ki < KI; ++ki, ++it) {
+          const int s = it % STAGES;
+          if (it >= STAGES) DBG_WAIT(w_prod, &empty_bar[s], ((it / STAGES) - 1) & 1);
+          if (elect_one()) {
+            const int tap = ki / P.kchunks, kc = ki - tap * P.kchunks;
+            const int dh = P.taps[tap].dh + (P.nphases == 4 ? t.py : 0);
+            const int dw = P.taps[tap].dw + (P.nphases == 4 ? t.px : 0);
+            const int wt = (t.phase * P.ntaps + tap) * 2;
+            mbar_expect_tx(&full_bar[s], 2 * A_STAGE_BYTES + 2 * Cfg::B_STAGE_BYTES);
+            tma_load_5d(smem_a + (s * 2 + 0) * A_STAGE_BYTES, &map_a, &full_bar[s], kc * 32, t.w0 + dw, t.h0 + dh, t.b, P.taps[tap].plane);
+            tma_load_5d(smem_a + (s * 2 + 1) * A_STAGE_BYTES, &map_a, &full_bar[s], kc * 32, t.w0 + dw, t.h0 + dh, t.b,
+                        P.taps[tap].plane + P.lo_plane_off);
+            tma_load_3d(smem_b + (s * 2 + 0) * Cfg::B_STAGE_BYTES, &map_b, &full_bar[s], kc * 32, t.n0, wt);
+            tma_load_3d(smem_b + (s * 2 + 1) * Cfg::B_STAGE_BYTES, &map_b, &full_bar[s], kc * 32, t.n0, wt + 1);
           }
+          __syncwarp();
         }
-      }
-      for (int tile = tile_first; tile < num_tiles && !TF3 && (CG == 1 || crank == 0); tile += tile_step, ++lt) {  // pair: leader only
-        const int acc = lt & 1;
-        if (lt >= 2) DBG_WAIT(w_tempty, &tempty_bar[acc], ((lt >> 1) - 1) & 1);  // epilogue drained this buffer
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + (uint32_t)(acc * BN);
-        if constexpr (ROWS) {
-          const int nst = 3 * P.kchunks;
-          for (int si = 0; si < nst; ++si, ++it) {
+      } else if constexpr (ROWS) {
+        for (int kc = 0; kc < P.kchunks; ++kc) {
+          for (int dwi = 0; dwi < 3; ++dwi, ++it) {
             const int s = it % STAGES;
-            DBG_WAIT(w_full, &full_bar[s], (it / STAGES) & 1);
-            tc_fence_after();
+            if (it >= STAGES) DBG_WAIT(w_prod, &empty_bar[s], ((it / STAGES) - 1) & 1);
             if (elect_one()) {
-              const uint32_t a0 = smem_u32(smem_a + s * ROWS_A_SLOT);
+              mbar_expect_tx(&full_bar[s], P.rows_a_bytes + 3 * Cfg::B_STAGE_BYTES);
+              tma_load_5d(smem_a + s * ROWS_A_SLOT, &map_a, &full_bar[s], kc * 64, t.w0 + dwi - 1, t.h0 - 1, t.b, 0);
 #pragma unroll
-              for (int j = 0; j < 3; ++j) {  // vertical tap dh = j-1: row window starting j*BW pixel rows into the box
-                const uint64_t adesc = make_sw128_desc(a0 + (uint32_t)(j * P.BW * 128));
-                const uint64_t bdesc = make_sw128_desc(smem_u32(smem_b + (s * 3 + j) * Cfg::B_STAGE_BYTES));
-#pragma unroll
-                for (int k = 0; k < 4; ++k)
-                  umma_bf16(tmem_d, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), idesc, (si > 0 || j > 0 || k > 0) ? 1u : 0u);
-              }
-              umma_commit(&empty_bar[s]);
-            }
-            __syncwarp();
-          }
-        } else {
-          constexpr int G = Cfg::G;
-          for (int g0 = 0; g0 < KI; g0 += G, ++it) {
-            const int s = it % STAGES;
-            DBG_WAIT(w_full, &full_bar[s], (it / STAGES) & 1);
-            tc_fence_after();
-            if (elect_one()) {
-              const int n = (KI - g0) < G ? (KI - g0) : G;
-#pragma unroll
-              for (int j = 0; j < G; ++j) {
-                if (j < n) {
-                  const uint64_t adesc = make_sw128_desc(smem_u32(smem_a + (s * G + j) * A_STAGE_BYTES));
-                  const uint64_t bdesc = make_sw128_desc(smem_u32(smem_b + (s * G + j) * Cfg::B_STAGE_BYTES));
-#pragma unroll
-                  for (int k = 0; k < 4; ++k) {
-                    if constexpr (CG == 2)
-                      umma_bf16_pair(tmem_d, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), idesc, (g0 + j > 0 || k > 0) ? 1u : 0u);
-                    else
-                      umma_bf16(tmem_d, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), idesc, (g0 + j > 0 || k > 0) ? 1u : 0u);
-                  }
-                }
-              }
-              if constexpr (CG == 2) umma_commit_pair(&empty_bar[s]);  // frees stage s in both CTAs
-              else umma_commit(&empty_bar[s]);
+              for (int j = 0; j < 3; ++j)  // taps (dh = j-1, dw = dwi-1): index (dh+1)*3 + (dw+1)
+                tma_load_3d(smem_b + (s * 3 + j) * Cfg::B_STAGE_BYTES, &map_b, &full_bar[s], kc * 64, t.n0, j * 3 + dwi);
             }
             __syncwarp();
           }
         }
-        if (elect_one()) {
-          if constexpr (CG == 2) umma_commit_pair(&tfull_bar[acc]);  // both epilogues
-          else umma_commit(&tfull_bar[acc]);
+      } else {
+        for (int ki = 0; ki < KI; ++ki, ++it) {
+          const int s = it % STAGES;
+          if (it >= STAGES) DBG_WAIT(w_prod, &empty_bar[s], ((it / STAGES) - 1) & 1);
+          if (elect_one()) {
+            const int tap = ki / P.kchunks, kc = ki - tap * P.kchunks;
+            const int dh = P.taps[tap].dh + (P.nphases == 4 ? t.py : 0);
+            const int dw = P.taps[tap].dw + (P.nphases == 4 ? t.px : 0);
+            mbar_expect_tx(&full_bar[s], Cfg::STAGE_BYTES);
+            tma_load_5d(smem_a + s * A_STAGE_BYTES, &map_a, &full_bar[s], kc * 64, t.w0 + dw, t.h0 + dh, t.b, P.taps[tap].plane);
+            tma_load_3d(smem_b + s * Cfg::B_STAGE_BYTES, &map_b, &full_bar[s], kc * 64, t.n0,
+                        t.phase * P.ntaps + tap + (P.w_per_image ? t.b : 0));
+          }
+          __syncwarp();
         }
-        __syncwarp();
-      }
-      if (P.dbg && lane == 0) {
-        P.dbg[blockIdx.x * 8 + 2] = (unsigned long long)w_full;
-        P.dbg[blockIdx.x * 8 + 3] = (unsigned long long)w_tempty;
-        P.dbg[blockIdx.x * 8 + 4] = (unsigned long long)(clock64() - t_start);
       }
     }
-  } else {
-    // ================= epilogue (warps 2..9) =================
-    // Two warps per TMEM lane quadrant (warp & 3), taking alternate 32-column chunks; the tcgen05.ld of the next
-    // chunk is in flight while the current one is converted, staged (64B-swizzled) and bulk-stored by TMA.
-    const int et = threadIdx.x - 64;  // 0..255
-    const int quad = warp & 3;
-    const int half = (warp - 2) >> 2;
-    const int m = quad * 32 + lane;
-    const int trow = P.t_ptr ? *P.t_ptr : 0;
-    const bool affine = (P.ss != nullptr) || (P.bias != nullptr) || (P.mult_vec != nullptr);
-    uint8_t* const stg_base = smem_stg + (warp - 2) * 2048 * (Cfg::STG_BUFS > 0 ? Cfg::STG_BUFS : 1);
-    int stg_i = 0;  // staging tile used by the next bulk store (alternates when STG_BUFS == 2)
-    long long w_tfull = 0, t_start = clock64();
-    int lt = 0, epi_n0 = -1, epi_b = -1;
-    int seg_st = 0;  // fp32x3: K segments consumed by this warp (TMEM buffer = seg_st & 1)
-    for (int tile = tile_first; tile < num_tiles; tile += tile_step, ++lt) {
-      const TileCoord t = tile_coord(tile);
-      const int acc = lt & 1;
-      // The per-channel (mult, add) table depends on the N tile (and on the image only with per-image timesteps):
-      // rebuild it - two barriers and a dependent global load on the epilogue's critical path - only when that changes.
-      const int key_b = P.ss_img_stride ? t.b : 0;
-      if (affine && (t.n0 != epi_n0 || key_b != epi_b)) {
-        epi_n0 = t.n0; epi_b = key_b;
-        asm volatile("bar.sync 1, 256;" ::: "memory");  // previous tile's reads of s_epi are done
-        const int tb = (CG == 2 && t.b >= P.B) ? 0 : t.b;  // pair tail: a CTA without pixels still needs a valid table row
-        const float* ssrow = P.ss ? P.ss + (long long)(trow + tb * P.ss_img_stride) * P.ss_S + P.ss_off : nullptr;
-        for (int j = et; j < BN; j += 256) {
-          const int n = t.n0 + j;
-          float mult = 1.f, add = 0.f, bias = 0.f;
-          if (n < P.Cout) {
-            if (ssrow) { mult = ssrow[n] + 1.0f; add = ssrow[P.Cout + n]; }
-            if (P.mult_vec) mult *= P.mult_vec[n];
-            if (P.bias) bias = P.bias[n];
-          }
-          s_epi[j] = mult; s_epi[BN + j] = bias * mult + add;  // (x + bias) * mult + add == x * mult + (bias * mult + add)
-        }
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-      }
-      const int hh = t.h0 + (m >> P.logBW), ww = t.w0 + (m & (P.BW - 1));
-      const bool pvalid = hh < P.H && ww < P.W && (CG == 1 || t.b < P.B);
-      const long long opix = ((long long)t.b * P.Hout + (hh * P.os + t.py)) * P.Wout + (ww * P.os + t.px);
-      bf16* orow = P.out + opix * P.out_pitch + t.n0;
-      const bf16* rrow = P.res ? P.res + opix * P.res_pitch + t.n0 : nullptr;
+    if (P.dbg && lane == 0) { P.dbg[blockIdx.x * 8 + 0] = (unsigned long long)w_prod; P.dbg[blockIdx.x * 8 + 1] = (unsigned long long)(clock64() - t_start); }
+    return;
+  }
 
+  // ================= consumers: warpgroup wg owns pixel rows 64*wg .. 64*wg+63 of every tile =================
+  const int wg = warp >> 2;
+  const int wq = warp & 3;               // wgmma layout: this warp holds accumulator rows 16*wq + lane/4 (+8)
+  const int quad = wg * 2 + (wq & 1);    // epilogue layout: pixel m = quad*32 + lane, 32-channel chunks alternate by `half`
+  const int half = wq >> 1;
+  const int m = quad * 32 + lane;
+  const int et = threadIdx.x;  // 0..255
+  const int trow = P.t_ptr ? *P.t_ptr : 0;
+  const bool affine = (P.ss != nullptr) || (P.bias != nullptr) || (P.mult_vec != nullptr);
+  uint8_t* const stg_base = smem_stg + warp * 2048 * (Cfg::STG_BUFS > 0 ? Cfg::STG_BUFS : 1);
+  float* const acc_stg = s_acc + wg * 64 * ACC_PITCH;
+  const uint32_t a_off = (uint32_t)(wg * 64 * 128);  // this warpgroup's 64 pixel rows inside every A box
+  const bool signaller = (threadIdx.x & 127) == 0;
+  int stg_i = 0;  // staging tile used by the next bulk store (alternates when STG_BUFS == 2)
+  long long w_full = 0, t_start = clock64();
+  int it = 0, lt = 0, epi_n0 = -1, epi_b = -1;
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++lt) {
+    const TileCoord t = decode_tile(P, tile, tiles_m, BN);
+    float acc[NACC];
+    float sum[TF3 ? NACC : 1];  // fp32x3: the tile's K segments summed with round-to-nearest adds
+#pragma unroll
+    for (int r = 0; r < NACC; ++r) acc[r] = 0.f;
+#pragma unroll
+    for (int r = 0; r < (TF3 ? NACC : 1); ++r) sum[r] = 0.f;
+    // one stage: wait for its bytes, issue this warpgroup's MMAs on it, then release the PREVIOUS stage once its MMAs have
+    // finished reading shared memory (one wgmma group stays in flight)
+    int prev_s = -1;
+    auto stage_begin = [&](int s) __attribute__((always_inline)) {
+      DBG_WAIT(w_full, &full_bar[s], (it / STAGES) & 1);
+      wgmma_fence();
+    };
+    auto stage_end = [&](int s) __attribute__((always_inline)) {
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (prev_s >= 0 && signaller) mbar_arrive(&empty_bar[prev_s]);
+      prev_s = s;
+      ++it;
+    };
+    auto drain = [&]() __attribute__((always_inline)) {
+      wgmma_wait<0>();
+      acc_fence<NACC>(acc);
+      if (prev_s >= 0 && signaller) mbar_arrive(&empty_bar[prev_s]);
+      prev_s = -1;
+    };
+    if constexpr (TF3) {
+      // fp32x3: the K loop of a tile is cut into SEGMENTS of TF3_SEG k-iterations; each segment accumulates from zero and is
+      // added to `sum` with round-to-nearest adds.  Reason: the tensor core's accumulator update truncates, so a single
+      // accumulation over n MMAs drifts by ~n * 2^-26 relative (3e-5 per layer at K = 13 824); 24 MMAs per segment keep
+      // it at the fp32 FMA path's own level.
+      for (int k0 = 0; k0 < KI; k0 += TF3_SEG) {
+        const int k1 = k0 + TF3_SEG < KI ? k0 + TF3_SEG : KI;
+        for (int ki = k0; ki < k1; ++ki) {
+          const int s = it % STAGES;
+          stage_begin(s);
+          const uint64_t a_hi = make_sw128_desc(smem_u32(smem_a + (s * 2 + 0) * A_STAGE_BYTES) + a_off);
+          const uint64_t a_lo = make_sw128_desc(smem_u32(smem_a + (s * 2 + 1) * A_STAGE_BYTES) + a_off);
+          const uint64_t b_hi = make_sw128_desc(smem_u32(smem_b + (s * 2 + 0) * Cfg::B_STAGE_BYTES));
+          const uint64_t b_lo = make_sw128_desc(smem_u32(smem_b + (s * 2 + 1) * Cfg::B_STAGE_BYTES));
+          // the two small cross terms first, the dominant hi*hi product last
+#pragma unroll
+          for (int k = 0; k < 4; ++k) wgmma_tf32<BN>(acc, a_lo + (uint64_t)(k * 2), b_hi + (uint64_t)(k * 2));
+#pragma unroll
+          for (int k = 0; k < 4; ++k) wgmma_tf32<BN>(acc, a_hi + (uint64_t)(k * 2), b_lo + (uint64_t)(k * 2));
+#pragma unroll
+          for (int k = 0; k < 4; ++k) wgmma_tf32<BN>(acc, a_hi + (uint64_t)(k * 2), b_hi + (uint64_t)(k * 2));
+          stage_end(s);
+        }
+        drain();
+#pragma unroll
+        for (int r = 0; r < NACC; ++r) {
+          sum[(TF3 ? r : 0)] = __fadd_rn(sum[(TF3 ? r : 0)], acc[r]);
+          acc[r] = 0.f;
+        }
+      }
+    } else if constexpr (ROWS) {
+      const int nst = 3 * P.kchunks;
+      for (int si = 0; si < nst; ++si) {
+        const int s = it % STAGES;
+        stage_begin(s);
+        const uint32_t a0 = smem_u32(smem_a + s * ROWS_A_SLOT) + a_off;
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {  // vertical tap dh = j-1: row window starting j*BW pixel rows into the box
+          const uint64_t adesc = make_sw128_desc(a0 + (uint32_t)(j * P.BW * 128));
+          const uint64_t bdesc = make_sw128_desc(smem_u32(smem_b + (s * 3 + j) * Cfg::B_STAGE_BYTES));
+#pragma unroll
+          for (int k = 0; k < 4; ++k) wgmma_bf16<BN>(acc, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2));
+        }
+        stage_end(s);
+      }
+      drain();
+    } else {
+      for (int ki = 0; ki < KI; ++ki) {
+        const int s = it % STAGES;
+        stage_begin(s);
+        const uint64_t adesc = make_sw128_desc(smem_u32(smem_a + s * A_STAGE_BYTES) + a_off);
+        const uint64_t bdesc = make_sw128_desc(smem_u32(smem_b + s * Cfg::B_STAGE_BYTES));
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wgmma_bf16<BN>(acc, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2));
+        stage_end(s);
+      }
+      drain();
+    }
+
+    // ---- epilogue
+    // The per-channel (mult, add) table depends on the N tile (and on the image only with per-image timesteps):
+    // rebuild it - two barriers and a dependent global load - only when that changes.
+    const int key_b = P.ss_img_stride ? t.b : 0;
+    if (affine && (t.n0 != epi_n0 || key_b != epi_b)) {
+      epi_n0 = t.n0; epi_b = key_b;
+      asm volatile("bar.sync 1, 256;" ::: "memory");  // previous tile's reads of s_epi are done
+      const float* ssrow = P.ss ? P.ss + (long long)(trow + t.b * P.ss_img_stride) * P.ss_S + P.ss_off : nullptr;
+      for (int j = et; j < BN; j += 256) {
+        const int n = t.n0 + j;
+        float mult = 1.f, add = 0.f, bias = 0.f;
+        if (n < P.Cout) {
+          if (ssrow) { mult = ssrow[n] + 1.0f; add = ssrow[P.Cout + n]; }
+          if (P.mult_vec) mult *= P.mult_vec[n];
+          if (P.bias) bias = P.bias[n];
+        }
+        s_epi[j] = mult; s_epi[BN + j] = bias * mult + add;  // (x + bias) * mult + add == x * mult + (bias * mult + add)
+      }
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+    }
+    const int hh = t.h0 + (m >> P.logBW), ww = t.w0 + (m & (P.BW - 1));
+    const bool pvalid = hh < P.H && ww < P.W;
+    const long long opix = ((long long)t.b * P.Hout + (hh * P.os + t.py)) * P.Wout + (ww * P.os + t.px);
+    bf16* orow = P.out + opix * P.out_pitch + t.n0;
+    const bf16* rrow = P.res ? P.res + opix * P.res_pitch + t.n0 : nullptr;
       // KC: std::integral_constant<int, KIND>.  KIND = the EK_* features this conv has, fixed per launch: feature blocks
       // outside KIND do not exist in the instantiation (the compiler had turned several of them into predicated code that
       // was issued for every chunk), EK_GENERIC keeps every run-time check (fp32 NCHW output, no-TMA-store fallback).
@@ -835,96 +676,53 @@ __global__ void __launch_bounds__(320, 1) conv_tc_persist_kernel(const __grid_co
             if (t.n0 + c0 + g * 8 < P.Cout) *reinterpret_cast<uint4*>(orow + c0 + g * 8) = ov[g];
         }
       };
-      typedef std::integral_constant<int, EK_GENERIC> KGen;
 
-      constexpr int NCH = (BN / 32 + 1) / 2;  // chunks per warp
-      if constexpr (TF3) {
-        // sum the tile's K segments in registers (IEEE round-to-nearest adds), then run the epilogue on the sums
-        float accf[NCH][32];
+    // registers (wgmma layout) -> fp32 staging rows (one pixel per row) in 64-column rounds -> per-pixel 32-channel chunks
+    auto fin = [&](int r) __attribute__((always_inline)) -> float {
+      if constexpr (TF3) return sum[r];
+      else return acc[r];
+    };
+    constexpr int NR = (BN + 63) / 64;
 #pragma unroll
-        for (int i = 0; i < NCH; ++i)
+    for (int i = 0; i < NR; ++i) {
+      asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");  // this warpgroup's previous reads of the staging rows are done
 #pragma unroll
-          for (int j = 0; j < 32; ++j) accf[i][j] = 0.f;
-        for (int k0 = 0; k0 < KI; k0 += TF3_SEG, ++seg_st) {
-          const int sacc = seg_st & 1;
-          DBG_WAIT(w_tfull, &tfull_bar[sacc], (seg_st >> 1) & 1);
-          tc_fence_after();
-          const uint32_t tmem_seg = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(sacc * BN);
-#pragma unroll
-          for (int i = 0; i < NCH; ++i) {
-            const int c0 = (2 * i + half) * 32;
-            if (c0 < BN) {
-              uint32_t v1[32];
-              tmem_ld32(tmem_seg + (uint32_t)c0, v1);
-#pragma unroll
-              for (int j = 0; j < 32; ++j) accf[i][j] = __fadd_rn(accf[i][j], __uint_as_float(v1[j]));
-            }
-          }
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&tempty_bar[sacc]);
+      for (int jj = 0; jj < 8; ++jj) {
+        const int j = i * 8 + jj;  // n8 block of the accumulator: registers 4j .. 4j+3
+        if (j * 8 < BN) {
+          const int row = wq * 16 + (lane >> 2), col = jj * 8 + 2 * (lane & 3);
+          *reinterpret_cast<float2*>(acc_stg + row * ACC_PITCH + col) = make_float2(fin(4 * j), fin(4 * j + 1));
+          *reinterpret_cast<float2*>(acc_stg + (row + 8) * ACC_PITCH + col) = make_float2(fin(4 * j + 2), fin(4 * j + 3));
         }
-#pragma unroll
-        for (int i = 0; i < NCH; ++i) {
-          const int c0 = (2 * i + half) * 32;
-          if (c0 < BN && t.n0 + c0 < P.Cout) process(KGen{}, reinterpret_cast<uint32_t*>(accf[i]), c0);
-        }
-        continue;
       }
-      DBG_WAIT(w_tfull, &tfull_bar[acc], (lt >> 1) & 1);
-      tc_fence_after();
-      const uint32_t tmem_acc = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(acc * BN);
-      auto run_chunks = [&](auto KC) __attribute__((always_inline)) {
-        uint32_t v[2][32];
-        if (half * 32 < BN) tmem_ld32_async(tmem_acc + (uint32_t)(half * 32), v[0]);
+      asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
+      const int c0 = i * 64 + half * 32;
+      if (c0 < BN && t.n0 + c0 < P.Cout) {  // chunks entirely past Cout carry no output
+        uint32_t v[32];
+        const float* src = acc_stg + ((wq & 1) * 32 + lane) * ACC_PITCH + half * 32;
 #pragma unroll
-        for (int i = 0; i < NCH; ++i) {
-          const int c0 = (2 * i + half) * 32;
-          if (c0 < BN) {
-            tmem_ld_wait(v[i & 1]);
-            const int c1 = (2 * (i + 1) + half) * 32;
-            if (i + 1 < NCH && c1 < BN) tmem_ld32_async(tmem_acc + (uint32_t)c1, v[(i + 1) & 1]);
-            if (t.n0 + c0 < P.Cout) process(KC, v[i & 1], c0);  // chunks entirely past Cout carry no output
-          }
+        for (int g = 0; g < 8; ++g) {
+          const float4 f = *reinterpret_cast<const float4*>(src + 4 * g);
+          v[4 * g] = __float_as_uint(f.x); v[4 * g + 1] = __float_as_uint(f.y);
+          v[4 * g + 2] = __float_as_uint(f.z); v[4 * g + 3] = __float_as_uint(f.w);
         }
-      };
-      run_chunks(std::integral_constant<int, EKT>{});  // EKT: the kernel instantiation's epilogue specialisation (tc_conv_launch)
-      // every tcgen05.ld of this warp has completed: hand the accumulator buffer back to the MMA warp
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if constexpr (CG == 2) mbar_arrive_leader(&tempty_bar[acc]);  // the leader's MMA warp owns both accumulators' reuse
-        else mbar_arrive(&tempty_bar[acc]);
+        process(std::integral_constant<int, EKT>{}, v, c0);  // EKT: the instantiation's epilogue specialisation
       }
     }
-    if (lane == 0) bulk_wait_all();  // staging smem must stay valid until the last bulk store has read it
-    if (P.dbg && threadIdx.x == 64) {
-      P.dbg[blockIdx.x * 8 + 5] = (unsigned long long)w_tfull;
-      P.dbg[blockIdx.x * 8 + 6] = (unsigned long long)(clock64() - t_start);
-      P.dbg[blockIdx.x * 8 + 7] = (unsigned long long)lt;
-    }
   }
-  tc_fence_before();
-  __syncthreads();
-  if constexpr (CG == 2) {
-    cluster_sync_all();  // the leader's MMAs read the peer's shared memory and write its TMEM: nobody leaves early
-    if (warp == 0)
-      asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(Cfg::TMEM_COLS) : "memory");
-    return;
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(Cfg::TMEM_COLS) : "memory");
+  if (lane == 0) bulk_wait_all();  // staging smem must stay valid until the last bulk store has read it
+  if (P.dbg && threadIdx.x == 0) {
+    P.dbg[blockIdx.x * 8 + 2] = (unsigned long long)w_full;
+    P.dbg[blockIdx.x * 8 + 4] = (unsigned long long)(clock64() - t_start);
+    P.dbg[blockIdx.x * 8 + 7] = (unsigned long long)lt;
   }
 }
 
-int g_num_sms = 148;
+int g_num_sms = 132;
 bool g_tma_store = true;
 bool g_rows = true;
 int g_epi_spec = 3;  // specialised epilogues: 1 = the per-tap 1x1 layers, 2 = + the ROWS 3x3 ResBlock convs, 3 = + the BN = 256
-                     // CTA-pair ResBlock convs and biased per-tap convs; IRSDE_TC_EPI_SPEC=0: generic only
-bool g_pair = true;    // cta_group::2 tiles (CTA pairs, M = 256) for the per-tap BN = 256 3x3 layers; IRSDE_TC_PAIR=0 disables.
-                       // Same-box ABAB (round 2, config 2): 720.0 / 719.5 -> 710.4 / 710.5 ms per chain; the Cout >= 256 3x3
-                       // layers go from 1.18-1.30 to 1.23-1.36 PFLOP/s (84-93 % of the sustained bf16 peak)
+                     // biased / plain per-tap convs; IRSDE_TC_EPI_SPEC=0: generic only
 
 }  // namespace
 
@@ -936,9 +734,12 @@ struct TcConvDesc {
   dim3 grid;
   int tiles_m, num_tiles;
   int mode;  // 0 per-tap boxes, 2 ROWS (row-window reuse), 3 fp32x3
-  bool pair = false;   // CTA-pair (cta_group::2) variant
-  int pair_tiles = 0;  // ceil(tiles_m / 2) * N tiles
 };
+
+template <int BN, int MODE, int EKT = EK_GENERIC>
+static void tc_set_smem() {
+  cudaFuncSetAttribute(conv_tc_persist_kernel<BN, MODE, EKT>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfgP<BN, MODE>::SMEM_BYTES);
+}
 
 bool tc_init(std::string* err) {
   if (g_encode) return true;
@@ -950,25 +751,27 @@ bool tc_init(std::string* err) {
     return false;
   }
   g_encode = (EncodeTiledFn)fn;
-  cudaFuncSetAttribute(conv_tc_persist_kernel<32, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfgP<32, 0>::SMEM_BYTES);
-  cudaFuncSetAttribute(conv_tc_persist_kernel<32, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfgP<32, 2>::SMEM_BYTES);
-  cudaFuncSetAttribute(conv_tc_persist_kernel<64, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfgP<64, 0>::SMEM_BYTES);
-  cudaFuncSetAttribute(conv_tc_persist_kernel<64, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfgP<64, 2>::SMEM_BYTES);
-  cudaFuncSetAttribute(conv_tc_persist_kernel<128, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfgP<128, 0>::SMEM_BYTES);
-  cudaFuncSetAttribute(conv_tc_persist_kernel<128, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfgP<128, 2>::SMEM_BYTES);
-  cudaFuncSetAttribute(conv_tc_persist_kernel<256, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfgP<256, 0>::SMEM_BYTES);
-  cudaFuncSetAttribute(conv_tc_persist_kernel<64, 2, 1, EK_AFF | EK_SILU>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfgP<64, 2>::SMEM_BYTES);
-  cudaFuncSetAttribute(conv_tc_persist_kernel<64, 2, 1, EK_SILU | EK_RES>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfgP<64, 2>::SMEM_BYTES);
-  cudaFuncSetAttribute(conv_tc_persist_kernel<128, 2, 1, EK_AFF | EK_SILU>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfgP<128, 2>::SMEM_BYTES);
-  cudaFuncSetAttribute(conv_tc_persist_kernel<128, 2, 1, EK_SILU | EK_RES>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfgP<128, 2>::SMEM_BYTES);
-  cudaFuncSetAttribute(conv_tc_persist_kernel<64, 0, 1, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfgP<64, 0>::SMEM_BYTES);
-  cudaFuncSetAttribute(conv_tc_persist_kernel<64, 0, 1, EK_AFF>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfgP<64, 0>::SMEM_BYTES);
-  cudaFuncSetAttribute(conv_tc_persist_kernel<128, 0, 1, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfgP<128, 0>::SMEM_BYTES);
-  cudaFuncSetAttribute(conv_tc_persist_kernel<128, 0, 1, EK_AFF>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfgP<128, 0>::SMEM_BYTES);
-  cudaFuncSetAttribute(conv_tc_persist_kernel<128, 0, 1, EK_QSM>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfgP<128, 0>::SMEM_BYTES);
-  cudaFuncSetAttribute(conv_tc_persist_kernel<32, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfgP<32, 3>::SMEM_BYTES);
-  cudaFuncSetAttribute(conv_tc_persist_kernel<64, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfgP<64, 3>::SMEM_BYTES);
-  cudaFuncSetAttribute(conv_tc_persist_kernel<128, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfgP<128, 3>::SMEM_BYTES);
+  tc_set_smem<32, 0>();
+  tc_set_smem<32, 2>();
+  tc_set_smem<64, 0>();
+  tc_set_smem<64, 2>();
+  tc_set_smem<128, 0>();
+  tc_set_smem<128, 2>();
+  tc_set_smem<256, 0>();
+  tc_set_smem<64, 2, EK_AFF | EK_SILU>();
+  tc_set_smem<64, 2, EK_SILU | EK_RES>();
+  tc_set_smem<128, 2, EK_AFF | EK_SILU>();
+  tc_set_smem<128, 2, EK_SILU | EK_RES>();
+  tc_set_smem<64, 0, 0>();
+  tc_set_smem<64, 0, EK_AFF>();
+  tc_set_smem<128, 0, 0>();
+  tc_set_smem<128, 0, EK_AFF>();
+  tc_set_smem<128, 0, EK_QSM>();
+  tc_set_smem<256, 0, EK_AFF>();
+  tc_set_smem<256, 0, 0>();
+  tc_set_smem<32, 3>();
+  tc_set_smem<64, 3>();
+  tc_set_smem<128, 3>();
   {
     int dev = 0, n = 0;
     cudaGetDevice(&dev);
@@ -977,20 +780,10 @@ bool tc_init(std::string* err) {
     g_tma_store = !(e && e[0] == '0');
     e = getenv("IRSDE_TC_ROWS");
     g_rows = !(e && e[0] == '0');
-    e = getenv("IRSDE_TC_PAIR");
-    g_pair = !(e && e[0] == '0');
     e = getenv("IRSDE_TC_EPI_SPEC");
     if (e && e[0] >= '0' && e[0] <= '3') g_epi_spec = e[0] - '0';
-    cudaFuncSetAttribute(conv_tc_persist_kernel<256, 0, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfgP<256, 0, 2>::SMEM_BYTES);
-    cudaFuncSetAttribute(conv_tc_persist_kernel<256, 0, 2, EK_AFF | EK_SILU>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfgP<256, 0, 2>::SMEM_BYTES);
-    cudaFuncSetAttribute(conv_tc_persist_kernel<256, 0, 2, EK_SILU | EK_RES>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfgP<256, 0, 2>::SMEM_BYTES);
-    cudaFuncSetAttribute(conv_tc_persist_kernel<256, 0, 1, EK_AFF>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfgP<256, 0>::SMEM_BYTES);
-    cudaFuncSetAttribute(conv_tc_persist_kernel<256, 0, 1, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfgP<256, 0>::SMEM_BYTES);
-    cudaFuncSetAttribute(conv_tc_persist_kernel<256, 0, 2, EK_AFF>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfgP<256, 0, 2>::SMEM_BYTES);
-    cudaFuncSetAttribute(conv_tc_persist_kernel<256, 0, 2, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfgP<256, 0, 2>::SMEM_BYTES);
-    cudaFuncSetAttribute(conv_tc_persist_kernel<256, 0, 2>, cudaFuncAttributeNonPortableClusterSizeAllowed, 0);
     e = getenv("IRSDE_PDL");
-    g_pdl = (e && e[0] == '1');  // opt-in: measured 0.7 % (UNet step) to 3 % (NAFNet step) slower than plain graph edges
+    g_pdl = (e && e[0] == '1');  // opt-in (see common.cuh)
   }
   cudaError_t le = cudaGetLastError();
   if (le != cudaSuccess) {
@@ -1015,7 +808,6 @@ static void tc_fill_magic(TcConvDesc* d) {
   P.mg_tilesW = mg(P.tilesW);
   P.mg_tilesH = mg(P.tilesH);
   P.mg_B = mg(P.B);
-  P.mg_pairs_m = mg((d->tiles_m + 1) >> 1);
   int k = 0;
   if (P.qsm) k |= EK_QSM;
   if (P.ss || P.bias || P.mult_vec) k |= EK_AFF;
@@ -1085,13 +877,8 @@ TcConvDesc* tc_conv_create(const bf16* in, int in_pitch, int B, int Hin, int Win
   // K order for every BN, so results do not depend on this choice (and hence not on the batch size).
   if (!rows && !P.qsm && !nchw_out) {
     const int tm = P.tilesW * P.tilesH * B * nphases;
-    while (BN > 64 && Cout % (BN / 2) == 0 && (long long)tm * ((Cout + BN - 1) / BN) < 74) BN >>= 1;
+    while (BN > 64 && Cout % (BN / 2) == 0 && (long long)tm * ((Cout + BN - 1) / BN) < g_num_sms / 2) BN >>= 1;
   }
-  // CTA-pair variant: per-tap mode, full 256-channel N tiles, plain bf16 NHWC output through TMA stores
-  // (not the stride-2 space-to-depth layers: 16 taps over 4 planes measured 10 % slower as pairs)
-  d->pair = g_pair && g_tma_store && !rows && BN == 256 && Cout % 256 == 0 && !P.qsm && !P.w_per_image &&
-            !nchw_out && planes == 1 && ntaps > 1;
-  d->pair_tiles = ((P.tilesW * P.tilesH * B * nphases + 1) / 2) * (Cout / 256);
   d->BN = BN;
   d->grid = dim3((unsigned)(P.tilesW * P.tilesH * B * nphases), (unsigned)((Cout + BN - 1) / BN));
   d->tiles_m = P.tilesW * P.tilesH * B * nphases;
@@ -1099,7 +886,7 @@ TcConvDesc* tc_conv_create(const bf16* in, int in_pitch, int B, int Hin, int Win
   // Tile order.  Default: M fastest - the CTAs of a wave share one N tile, i.e. one set of weight tiles (3x3 layers: the
   // weights of an N tile are MBs, the A tensor of the deep levels fits in L2).  1x1 convs with several N tiles (to_qkv:
   // 384 outputs = 3 tiles) invert that: their weights are a few KB but the A tensor of the 256^2 / 128^2 levels is larger
-  // than L2, and M-fastest re-read it from DRAM once per N tile (ncu r02: 403 MB read for a 134 MB input).  N fastest
+  // than L2, and M-fastest re-read it from DRAM once per N tile (about 3x the input's bytes for to_qkv).  N fastest
   // makes the N tiles of one pixel tile run back to back in the same wave, so the second and third read hit L2.
   P.tiles_n = (Cout + BN - 1) / BN;
   // (only where the input is too large to stay in L2 anyway; small inputs keep M-fastest and its once-per-N-tile epilogue table)
@@ -1134,7 +921,7 @@ TcConvDesc* tc_conv_create(const bf16* in, int in_pitch, int B, int Hin, int Win
   {
     cuuint64_t dims[3] = {(cuuint64_t)Cin, (cuuint64_t)Cout_w, (cuuint64_t)(P.w_per_image ? B : nphases * ntaps)};
     cuuint64_t strides[2] = {(cuuint64_t)Cin * 2, (cuuint64_t)Cout_w * Cin * 2};
-    cuuint32_t box[3] = {64, (cuuint32_t)(d->pair ? BN / 2 : BN), 1};  // pair: each CTA loads its half of the channels
+    cuuint32_t box[3] = {64, (cuuint32_t)BN, 1};
     cuuint32_t es[3] = {1, 1, 1};
     CUresult r = g_encode(&d->map_b, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, (void*)wpacked, dims, strides, box, es,
                           CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -1216,7 +1003,7 @@ TcConvDesc* tc_conv_create_f32x3(const float* in_split, int B, int Hin, int Win,
   P.tilesH = (Hin + P.BH - 1) / P.BH;
   {
     const int tm = P.tilesW * P.tilesH * B * nphases;
-    while (BN > 32 && Cout % (BN / 2) == 0 && (long long)tm * ((Cout + BN - 1) / BN) < 74) BN >>= 1;
+    while (BN > 32 && Cout % (BN / 2) == 0 && (long long)tm * ((Cout + BN - 1) / BN) < g_num_sms / 2) BN >>= 1;
   }
   d->BN = BN;
   d->grid = dim3((unsigned)(P.tilesW * P.tilesH * B * nphases), (unsigned)((Cout + BN - 1) / BN));
@@ -1290,37 +1077,8 @@ int tc_conv_launch(TcConvDesc* d, cudaStream_t st) {
       cudaMemsetAsync(dbg_dev, 0, 256 * 8 * sizeof(unsigned long long), st);
     }
     d->P.dbg = dbg ? dbg_dev : nullptr;
-    if (d->pair) {
-      const int ncl = d->pair_tiles < g_num_sms / 2 ? d->pair_tiles : g_num_sms / 2;
-      cudaLaunchConfig_t cfg;
-      memset(&cfg, 0, sizeof cfg);
-      cfg.gridDim = dim3(2 * ncl);
-      cfg.blockDim = dim3(320);
-      cfg.dynamicSmemBytes = TcCfgP<256, 0, 2>::SMEM_BYTES;
-      cfg.stream = st;
-      cudaLaunchAttribute attr[1];
-      attr[0].id = cudaLaunchAttributeClusterDimension;
-      attr[0].val.clusterDim.x = 2;
-      attr[0].val.clusterDim.y = 1;
-      attr[0].val.clusterDim.z = 1;
-      cfg.attrs = attr;
-      cfg.numAttrs = 1;
-      const int ekp = g_epi_spec >= 3 ? d->P.epi_kind : EK_GENERIC;
-      cudaError_t le;
-      if (ekp == (EK_AFF | EK_SILU))
-        le = cudaLaunchKernelEx(&cfg, conv_tc_persist_kernel<256, 0, 2, EK_AFF | EK_SILU>, d->map_a, d->map_b, d->map_o, d->P, d->tiles_m, d->pair_tiles);
-      else if (ekp == (EK_SILU | EK_RES))
-        le = cudaLaunchKernelEx(&cfg, conv_tc_persist_kernel<256, 0, 2, EK_SILU | EK_RES>, d->map_a, d->map_b, d->map_o, d->P, d->tiles_m, d->pair_tiles);
-      else if (ekp == EK_AFF)
-        le = cudaLaunchKernelEx(&cfg, conv_tc_persist_kernel<256, 0, 2, EK_AFF>, d->map_a, d->map_b, d->map_o, d->P, d->tiles_m, d->pair_tiles);
-      else if (ekp == 0)
-        le = cudaLaunchKernelEx(&cfg, conv_tc_persist_kernel<256, 0, 2, 0>, d->map_a, d->map_b, d->map_o, d->P, d->tiles_m, d->pair_tiles);
-      else
-        le = cudaLaunchKernelEx(&cfg, conv_tc_persist_kernel<256, 0, 2>, d->map_a, d->map_b, d->map_o, d->P, d->tiles_m, d->pair_tiles);
-      return le == cudaSuccess ? 1 : -1;
-    }
 #define TC_LAUNCH(BNV, PV) \
-  pdl_launch(conv_tc_persist_kernel<BNV, PV>, g, 320, TcCfgP<BNV, PV>::SMEM_BYTES, st, d->map_a, d->map_b, d->map_o, d->P, d->tiles_m, d->num_tiles)
+  pdl_launch(conv_tc_persist_kernel<BNV, PV>, g, 288, TcCfgP<BNV, PV>::SMEM_BYTES, st, d->map_a, d->map_b, d->map_o, d->P, d->tiles_m, d->num_tiles)
     if (d->mode == 3) {
       switch (d->BN) {
         case 32: TC_LAUNCH(32, 3); break;
@@ -1329,7 +1087,7 @@ int tc_conv_launch(TcConvDesc* d, cudaStream_t st) {
       }
     } else if (d->mode == 2) {
 #define TC_LAUNCH_EK2(BNV, EKV) \
-  pdl_launch(conv_tc_persist_kernel<BNV, 2, 1, EKV>, g, 320, TcCfgP<BNV, 2>::SMEM_BYTES, st, d->map_a, d->map_b, d->map_o, d->P, d->tiles_m, d->num_tiles)
+  pdl_launch(conv_tc_persist_kernel<BNV, 2, EKV>, g, 288, TcCfgP<BNV, 2>::SMEM_BYTES, st, d->map_a, d->map_b, d->map_o, d->P, d->tiles_m, d->num_tiles)
       const int ek2 = g_epi_spec >= 2 ? d->P.epi_kind : EK_GENERIC;
       switch (d->BN) {
         case 32: TC_LAUNCH(32, 2); break;
@@ -1347,7 +1105,7 @@ int tc_conv_launch(TcConvDesc* d, cudaStream_t st) {
 #undef TC_LAUNCH_EK2
     } else {
 #define TC_LAUNCH_EK(BNV, EKV) \
-  pdl_launch(conv_tc_persist_kernel<BNV, 0, 1, EKV>, g, 320, TcCfgP<BNV, 0>::SMEM_BYTES, st, d->map_a, d->map_b, d->map_o, d->P, d->tiles_m, d->num_tiles)
+  pdl_launch(conv_tc_persist_kernel<BNV, 0, EKV>, g, 288, TcCfgP<BNV, 0>::SMEM_BYTES, st, d->map_a, d->map_b, d->map_o, d->P, d->tiles_m, d->num_tiles)
       const int ek = g_epi_spec >= 1 ? d->P.epi_kind : EK_GENERIC;
       switch (d->BN) {
         case 32: TC_LAUNCH(32, 0); break;
@@ -1377,8 +1135,8 @@ int tc_conv_launch(TcConvDesc* d, cudaStream_t st) {
       cudaMemcpy(h, dbg_dev, sizeof h, cudaMemcpyDeviceToHost);
       double a[8] = {0};
       for (unsigned i = 0; i < g; ++i) for (int k = 0; k < 8; ++k) a[k] += (double)h[i * 8 + k] / g;
-      fprintf(stderr, "TCDBG BN=%d mode=%d grid=%u tiles=%d ntaps=%d kch=%d | prod wait %.0f / %.0f | mma wait full %.0f tempty %.0f / %.0f | epi wait tfull %.0f / %.0f (tiles/cta %.1f)\n",
-              d->BN, d->mode, g, d->num_tiles, d->P.ntaps, d->P.kchunks, a[0], a[1], a[2], a[3], a[4], a[5], a[6], a[7]);
+      fprintf(stderr, "TCDBG BN=%d mode=%d grid=%u tiles=%d ntaps=%d kch=%d | prod wait %.0f / %.0f | consumer wait full %.0f / %.0f (tiles/cta %.1f)\n",
+              d->BN, d->mode, g, d->num_tiles, d->P.ntaps, d->P.kchunks, a[0], a[1], a[2], a[4], a[7]);
     }
     return 1;
   }

@@ -106,7 +106,7 @@ struct irsde_ctx {
   std::map<std::string, float*> w_simt;  // [KH*KW][Cin][Cout] fp32
   std::map<std::string, bf16*> w_tc;     // [phase][tap][Cout][Cin] bf16
   std::map<std::string, float*> w_tc3;   // fp32x3: [phase][tap][2 (hi,lo)][Cout_pad][Cin] fp32 (tf32-rounded parts)
-  bool use_tc3 = false;                  // fp32x3 mode: fp32 storage, convs through 3 x tcgen05.mma.kind::tf32
+  bool use_tc3 = false;                  // fp32x3 mode: fp32 storage, convs through 3 x tf32 wgmma
   std::map<std::string, int> ss_off;
   float *wall = nullptr, *ball = nullptr;
   int S = 0;
@@ -131,7 +131,7 @@ struct irsde_ctx {
   bool prof = false;
   struct ProfEv { int cat; double flops; cudaEvent_t e0, e1; const OpRec* op; };
   std::vector<ProfEv> prof_events;
-  bool use_tc = false;  // bf16 mode: route eligible convs through the tcgen05 engine
+  bool use_tc = false;  // bf16 mode: route eligible convs through the wgmma tap-GEMM engine
   std::vector<int> udim;  // UNet channels per level: nf * [1, ch_mult...] (DenoisingUNet_arch.py:51-56)
 };
 
@@ -504,7 +504,7 @@ struct Builder {
   std::map<void*, size_t> tmp_size;
   const float* pending_mult = nullptr;  // per-output-channel multiplier for the NEXT conv() (NAFBlock beta / gamma)
   int nchw_H = 0, nchw_W = 0;           // crop size of fp32 NCHW outputs (0 = the image size)
-  bool stem_padded = false;  // X0 lives in the zero-bordered [B][Hp+6][Wp+8][8] layout of the tcgen05 stem
+  bool stem_padded = false;  // X0 lives in the zero-bordered [B][Hp+6][Wp+8][8] layout of the tensor-core stem
 
   T* alloc(long long elems) {
     void* p = dev_alloc(ctx, (size_t)elems * sizeof(T), &plan->allocs);
@@ -771,8 +771,7 @@ struct Builder {
         plan->ops.back().bytes = (double)npix * 256 * sizeof(T);
         bf16* Mb = tmp((long long)B * C * 128);
         float* wout = fw(pre + "fn.fn.to_out.0.weight");
-        // (combine + fold in ONE kernel was tried in round 2: 8-64 blocks of latency-bound work instead of 32 + 256..4096
-        //  measured 0.62 vs 0.55 ms of attention time per step, same box ABAB - kept as two launches)
+        // (combine + fold in ONE kernel gives 8-64 blocks of latency-bound work instead of 32 + 256..4096: kept as two launches)
         plan->ops.push_back(OpRec{CAT_ATTN, 0.0, [=](Plan*, cudaStream_t st) {
           launch_la_fold(la_ctx, wout, Mb, B, C, st);
           c->launches++;
@@ -1414,7 +1413,7 @@ int ensure_chain_table(irsde_ctx* ctx, Plan* p, int T, cudaStream_t st) {
 // =====================================================================================================
 extern "C" {
 
-const char* irsde_version(void) { return "irsde_b200 0.1 sm_100a"; }
+const char* irsde_version(void) { return "irsde_b200 0.1 sm_90a"; }
 
 const char* irsde_last_error(const irsde_ctx* ctx) { return ctx ? ctx->err.c_str() : g_last_error.c_str(); }
 
@@ -1432,7 +1431,8 @@ int irsde_create(const irsde_config* cfg, irsde_ctx** out) {
   if (cfg->device < 0 || cfg->device >= ndev) return fail(nullptr, IRSDE_ERR_INVALID, "bad device ordinal");
   cudaDeviceProp prop;
   cudaGetDeviceProperties(&prop, cfg->device);
-  if (prop.major != 10) return fail(nullptr, IRSDE_ERR_UNSUPPORTED, "irsde_b200 is built for sm_100a (B200) only");
+  if (prop.major != 9 || prop.minor != 0)
+    return fail(nullptr, IRSDE_ERR_UNSUPPORTED, "irsde_b200 is built for sm_90a (H100) only");
   irsde_ctx* c = new irsde_ctx();
   c->cfg = *cfg;
   if (cudaSetDevice(cfg->device) != cudaSuccess) { delete c; return fail(nullptr, IRSDE_ERR_CUDA, "cudaSetDevice failed"); }
@@ -2075,7 +2075,7 @@ int irsde_conv2d_ex(irsde_ctx* ctx, int32_t engine, const float* x, const float*
   cudaStream_t st = (cudaStream_t)stream;
   int up = upsample ? 2 : 1;
   if (engine == 1) {
-    // tcgen05 engine: same taps/weight packing as the plan builder
+    // tensor-core engine: same taps/weight packing as the plan builder
     std::string terr;
     if (!tc_init(&terr)) return fail(ctx, IRSDE_ERR_CUDA, "tc_init: " + terr);
     bool k3 = KH == 3 && KW == 3 && stride == 1 && pad == 1, k1 = KH == 1 && KW == 1 && stride == 1 && pad == 0 && up == 1,
@@ -2154,7 +2154,7 @@ int irsde_conv2d_ex(irsde_ctx* ctx, int32_t engine, const float* x, const float*
     return rc;
   }
   if (engine == 2) {
-    // fp32x3 engine: fp32 NHWC, hi/lo split, 3 x tcgen05.mma.kind::tf32 (conv_tc.cu MODE 3)
+    // fp32x3 engine: fp32 NHWC, hi/lo split, 3 x tf32 wgmma (conv_tc.cu MODE 3)
     std::string terr;
     if (!tc_init(&terr)) return fail(ctx, IRSDE_ERR_CUDA, "tc_init: " + terr);
     bool k3 = KH == 3 && KW == 3 && stride == 1 && pad == 1, k1 = KH == 1 && KW == 1 && stride == 1 && pad == 0 && up == 1,

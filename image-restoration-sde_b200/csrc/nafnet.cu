@@ -12,8 +12,7 @@ namespace irsde {
 //   gate[b,p,ch] = dw(x)[ch] * dw(x)[ch + c]                   (DenoisingNAFNet_arch.py:65-66)
 //   partial[b][chunk][ch] = sum over the chunk's pixels of gate (AdaptiveAvgPool2d numerator, :29-30)
 // block = 64 channels x 4 pixel lanes, chunk = 64 pixels of one image - 16 for images of <= 1024 pixels, where 64-pixel
-// chunks leave a handful of blocks each walking 16 pixels x 9 taps serially (30 us for 512 KB of data at c=512,
-// 16x16) - (deterministic reduction order, fixed by the image shape)
+// chunks leave a handful of blocks each walking 16 pixels x 9 taps serially (c=512, 16x16) - (deterministic reduction order, fixed by the image shape)
 // =============================================================================================
 static inline int dw_pix(int N) { return N <= 1024 ? 16 : 64; }
 

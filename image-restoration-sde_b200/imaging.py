@@ -31,7 +31,7 @@ def _bind():
 
 def _cuda(t):
     if not torch.cuda.is_available():
-        raise RuntimeError("irsde_b200.imaging runs on CUDA (sm_100a) only; there is no CPU path")
+        raise RuntimeError("irsde_b200.imaging runs on CUDA (sm_90a) only; there is no CPU path")
     return t if t.is_cuda else t.cuda(non_blocking=True)
 
 

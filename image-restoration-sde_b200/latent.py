@@ -126,7 +126,7 @@ class UNet(ConditionalUNet):
 
     def _context(self, device):
         if device.type != "cuda":
-            raise RuntimeError("irsde_b200.UNet runs on CUDA (sm_100a) only; there is no CPU path")
+            raise RuntimeError("irsde_b200.UNet runs on CUDA (sm_90a) only; there is no CPU path")
         idx = device.index if device.index is not None else torch.cuda.current_device()
         if self._ctx is None or self._ctx_dev != idx:
             if self._ctx is not None:
@@ -141,7 +141,7 @@ class UNet(ConditionalUNet):
     @torch.no_grad()
     def encode(self, x):
         if not x.is_cuda:
-            raise RuntimeError("irsde_b200.UNet runs on CUDA (sm_100a) only; there is no CPU path")
+            raise RuntimeError("irsde_b200.UNet runs on CUDA (sm_90a) only; there is no CPU path")
         x = x.contiguous().float()
         B, C, H, W = x.shape
         ctx = self.sync_weights(x.device)
@@ -165,7 +165,7 @@ class UNet(ConditionalUNet):
                                "(one outstanding encode per module)")
         B, H, W = h.shape
         if not x.is_cuda:
-            raise RuntimeError("irsde_b200.UNet runs on CUDA (sm_100a) only; there is no CPU path")
+            raise RuntimeError("irsde_b200.UNet runs on CUDA (sm_90a) only; there is no CPU path")
         x = x.contiguous().float()
         ctx = self.sync_weights(x.device)
         if ctx is not h.ctx:

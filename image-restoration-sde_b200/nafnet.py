@@ -119,7 +119,7 @@ class ConditionalNAFNet(ConditionalUNet):
 
     def _context(self, device):
         if device.type != "cuda":
-            raise RuntimeError("irsde_b200.ConditionalNAFNet runs on CUDA (sm_100a) only; there is no CPU path")
+            raise RuntimeError("irsde_b200.ConditionalNAFNet runs on CUDA (sm_90a) only; there is no CPU path")
         idx = device.index if device.index is not None else torch.cuda.current_device()
         if self._ctx is None or self._ctx_dev != idx:
             if self._ctx is not None:

@@ -94,7 +94,7 @@ class Restorer:
             if not (isinstance(im, np.ndarray) and im.dtype == np.uint8 and im.ndim == 3):
                 raise TypeError("images must be uint8 numpy arrays [H,W,C]")
         if not torch.cuda.is_available():
-            raise RuntimeError("irsde_b200.Restorer runs on CUDA (sm_100a) only; there is no CPU path")
+            raise RuntimeError("irsde_b200.Restorer runs on CUDA (sm_90a) only; there is no CPU path")
         batches = plan_batches([im.shape for im in images], self.batch_size)
         out = [None] * len(images)
         with torch.cuda.device(self.device):

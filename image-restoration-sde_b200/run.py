@@ -1,5 +1,5 @@
 """Drop-in launcher: run an UNMODIFIED reference script (codes/config/<task>/test.py, inference.py, ...)
-on top of the B200-native sampler.
+on top of the H100-native sampler.
 
     python -m irsde_b200.run /path/to/codes/config/deraining/test.py -opt=options/test/ir-sde.yml
 

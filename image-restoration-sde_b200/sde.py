@@ -1,5 +1,5 @@
 """``IRSDE`` / ``DenoisingSDE`` with the reference's public surface (codes/utils/sde_utils.py:80-361,
-373-593) on top of the native sm_100a sampler.
+373-593) on top of the native sm_90a sampler.
 
 Host logic kept in Python: the theta/sigma schedules (a few hundred floats, computed once with the same
 torch ops as the reference so they are bit-identical) and the per-timestep scalar tables handed to the
@@ -139,7 +139,7 @@ class _SDEBase:
     def _ctx_for(self, x):
         """Native context used for the update kernel: the model's if it is ours, else a private one."""
         if not x.is_cuda:
-            raise RuntimeError("irsde_b200 samplers run on CUDA (sm_100a) only; there is no CPU path")
+            raise RuntimeError("irsde_b200 samplers run on CUDA (sm_90a) only; there is no CPU path")
         m = _unwrap(self.model) if self.model is not None else None
         if isinstance(m, ConditionalUNet):
             ctx = m.sync_weights(x.device)

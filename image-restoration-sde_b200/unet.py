@@ -1,6 +1,6 @@
 """``ConditionalUNet`` with the reference's constructor, ``forward(xt, cond, time)`` signature and
 state-dict names/shapes (codes/config/deraining/models/modules/DenoisingUNet_arch.py:19-134), executed
-by the native sm_100a library.  The ``nn.Module`` only holds the parameters (so ``load_state_dict``,
+by the native sm_90a library.  The ``nn.Module`` only holds the parameters (so ``load_state_dict``,
 ``.to(device)``, ``DataParallel(...)``, ``.eval()`` keep working, models/denoising_model.py:36-45,153);
 all arithmetic happens in hand-written CUDA kernels behind the C ABI.  No CPU path.
 """
@@ -84,7 +84,7 @@ class _Node(nn.Module):
 
 class ConditionalUNet(nn.Module):
     """Drop-in for the reference score network.  ``precision``: "fp32" (parity mode: fp32 storage and
-    FMA, matches the reference to ~1e-5 per forward) or "bf16" (perf mode: tcgen05 bf16 MMA with fp32
+    FMA, matches the reference to ~1e-5 per forward) or "bf16" (perf mode: wgmma bf16 MMA with fp32
     accumulation).  Default comes from ``IRSDE_B200_PRECISION`` (env) or "fp32"."""
 
     variant = "conditional"
@@ -133,7 +133,7 @@ class ConditionalUNet(nn.Module):
     # ---- native context management -------------------------------------------------------------
     def _context(self, device):
         if device.type != "cuda":
-            raise RuntimeError("irsde_b200.ConditionalUNet runs on CUDA (sm_100a) only; there is no CPU path")
+            raise RuntimeError("irsde_b200.ConditionalUNet runs on CUDA (sm_90a) only; there is no CPU path")
         idx = device.index if device.index is not None else torch.cuda.current_device()
         if self._ctx is None or self._ctx_dev != idx:
             if self._ctx is not None:
@@ -181,7 +181,7 @@ class ConditionalUNet(nn.Module):
     def _run(self, x, cond, time):
         import ctypes
         if not x.is_cuda:
-            raise RuntimeError("irsde_b200.ConditionalUNet runs on CUDA (sm_100a) only; there is no CPU path")
+            raise RuntimeError("irsde_b200.ConditionalUNet runs on CUDA (sm_90a) only; there is no CPU path")
         x = x.contiguous().float()
         if cond is not None:
             cond = cond.to(x.device).contiguous().float()

@@ -1,5 +1,5 @@
 /*
- * irsde_b200 - C ABI of the B200-native IR-SDE / Denoising-SDE reverse-diffusion sampler.
+ * irsde_b200 - C ABI of the H100-native IR-SDE / Denoising-SDE reverse-diffusion sampler.
  *
  * The reference (Algolzw/image-restoration-sde @ 2598d73) is pure Python and has no FFI; the
  * calls below are what a binding for its hot path would bind.  Each entry point cites the
@@ -39,11 +39,11 @@ typedef enum {
 
 /* numerics mode */
 #define IRSDE_PREC_FP32 0 /* parity mode: fp32 storage + fp32 FMA everywhere                     */
-#define IRSDE_PREC_BF16 1 /* perf mode: bf16 activations/weights, tcgen05 MMA, fp32 accumulate,  */
+#define IRSDE_PREC_BF16 1 /* perf mode: bf16 activations/weights, wgmma MMA, fp32 accumulate,  */
                           /* fp32 sampler state                                                   */
 #define IRSDE_PREC_FP32X3 2 /* fp32-accurate tensor-core mode: fp32 storage; every conv is three   */
-                            /* tcgen05.mma.kind::tf32 passes over hi/lo split operands            */
-                            /* (hi*hi + lo*hi + hi*lo, fp32 accumulate in TMEM): meets the 1e-3    */
+                            /* tf32 wgmma passes over hi/lo split operands            */
+                            /* (hi*hi + lo*hi + hi*lo, fp32 accumulate): meets the 1e-3    */
                             /* bound of the fp32 mode on the tensor cores                          */
 
 /* sampler */
@@ -65,7 +65,7 @@ typedef struct {
   int32_t device;    /* CUDA device ordinal                      */
   int32_t flags;     /* IRSDE_FLAG_* (0 = defaults)              */
 } irsde_config;
-/* flags (all three config structs): bf16 storage through the fp32-FMA SIMT conv engine instead of tcgen05 - a debugging
+/* flags (all three config structs): bf16 storage through the fp32-FMA SIMT conv engine instead of the tensor cores - a debugging
  * aid that separates storage rounding from tensor-core issues; never the product path. */
 #define IRSDE_FLAG_FORCE_SIMT 1
 
@@ -109,7 +109,7 @@ int irsde_create_ch_mult(const irsde_config* cfg, const int32_t* ch_mult, int32_
 int irsde_create_nafnet(const irsde_nafnet_config* cfg, irsde_ctx** out);
 void irsde_destroy(irsde_ctx* ctx);
 const char* irsde_last_error(const irsde_ctx* ctx);
-/* "irsde_b200 <version> sm_100a" */
+/* "irsde_b200 <version> sm_90a" */
 const char* irsde_version(void);
 
 /* Latent autoencoder context (same weight-loading entry points).  encode replaces `UNet.encode(x) -> (z, h)`
@@ -178,7 +178,7 @@ int irsde_set_image_uids(irsde_ctx* ctx, const uint64_t* uids, int32_t n, void* 
 
 /* Instrumented pass: between begin/end every op of the launch plan is bracketed by CUDA events on the
  * launching stream (graph replay is bypassed).  end() synchronises and returns, per op category
- * (0 tcgen05 conv, 1 SIMT conv, 2 LayerNorm, 3 attention, 4 misc, 5 update), the summed device time in
+ * (0 tensor-core conv, 1 SIMT conv, 2 LayerNorm, 3 attention, 4 misc, 5 update), the summed device time in
  * ms, the executed conv flops and the number of ops.  ncat must be >= 6. */
 int irsde_profile_begin(irsde_ctx* ctx);
 int irsde_profile_end(irsde_ctx* ctx, double* ms, double* flops, int64_t* launches, int32_t ncat);
@@ -193,7 +193,7 @@ int64_t irsde_device_bytes(const irsde_ctx* ctx);
 
 /* ---- standalone operator entry points (unit-test / micro-benchmark surface) -------------- */
 /* Generic NHWC convolution through the engine selected by `engine` (0 = fp32 SIMT implicit
- * GEMM, 1 = tcgen05 bf16 tap-GEMM, 2 = tcgen05 fp32x3 tap-GEMM: fp32 in/out, 3 x kind::tf32 MMA).  Input/weights/output are fp32 device buffers:
+ * GEMM, 1 = wgmma bf16 tap-GEMM, 2 = wgmma fp32x3 tap-GEMM: fp32 in/out, 3 x tf32 MMA).  Input/weights/output are fp32 device buffers:
  * x [B,Cin,H,W], w [Cout,Cin,KH,KW] (nn.Conv2d layout, module_util.py:96,101,105), y
  * [B,Cout,Ho,Wo]; the call repacks to the engine's layout, runs, and unpacks. */
 int irsde_conv2d(irsde_ctx* ctx, int32_t engine, const float* x, const float* w, const float* bias, float* y,

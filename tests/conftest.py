@@ -9,10 +9,10 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 @pytest.fixture(scope="session")
 def golden():
-    import torch
-    return torch.load(os.path.join(ROOT, "tests", "golden", "reference_golden.pt"), weights_only=True)
+    import _golden
+    return _golden.load("reference_golden.pt")

@@ -151,7 +151,9 @@ def main():
     gold["unet_dsde"] = dict(nf=8, depth=2, state=sd2, x=xd, t_int=9, y=yd, args=(75, 30, "cosine"), Tstar=Tstar,
                              zs=zs, x0_sde=xo_sde, x0_ode=xo_ode)
 
-    torch.save(gold, os.path.join(OUT, "reference_golden.pt"))
+    sys.path.insert(0, os.path.dirname(OUT))
+    import _golden
+    _golden.save(gold, "reference_golden.pt")
     n = os.path.getsize(os.path.join(OUT, "reference_golden.pt"))
     print("wrote reference_golden.pt", n, "bytes")
 

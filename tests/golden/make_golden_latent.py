@@ -1,6 +1,6 @@
 """Golden fixture for the Refusion latent autoencoder UNet.encode/decode, generated from the imported reference
 (random small configuration; the shipped checkpoint latent-dehazing.pth is exercised by a CPU test when the reference
-checkout is present).    python tests/golden/make_golden_latent.py"""
+is staged).    python tests/golden/make_golden_latent.py"""
 import importlib.util
 import os
 import sys
@@ -8,7 +8,8 @@ import types
 
 import torch
 
-REF = "/root/reference/codes"
+# the reference checkout as staged by oracle/make_ref.py (or IRSDE_REFERENCE = a checkout of it)
+REF = os.path.join(os.environ.get("IRSDE_REFERENCE") or os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "..", "oracle", "_ref"), "codes")
 OUT = os.path.dirname(os.path.abspath(__file__))
 
 

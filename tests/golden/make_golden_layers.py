@@ -103,6 +103,8 @@ x = torch.rand(2, 3, 16, 24, generator=g)
 layers, y = hooked_forward(net, lambda m: m(x, 5))
 out["denoising"] = {"cfg": cfg, "state": {k: v.detach().clone() for k, v in net.state_dict().items()}, "x": x, "t": 5, "y": y,
                     "layers": layers}
-torch.save(out, os.path.join(os.path.dirname(os.path.abspath(__file__)), "reference_golden_layers.pt"))
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
+import _golden  # noqa: E402
+_golden.save(out, "reference_golden_layers.pt")
 for k, v in out.items():
     print(k, len(v["layers"]), "layers", float(v["y"].abs().max()))

@@ -1,7 +1,7 @@
 """The BENCHMARKED kernels at BENCHMARK shapes against an independent reference (round-1 verdict, weak #1).
 
-`conv_tc_persist_kernel` runs min(tiles, 148) persistent CTAs; every case below has >= 2 x 148 output tiles per launch, so
-the multi-tile loop, the TMEM double-buffer hand-off and the mbarrier phase wrap are compared with an implementation that
+`conv_tc_persist_kernel` runs min(tiles, 132) persistent CTAs (one per H100 SM); every case below has >= 2 x 132 output tiles
+per launch, so the multi-tile loop, the producer running ahead into the next tile and the mbarrier phase wrap are compared with an implementation that
 shares nothing with them: torch's fp32 convolution (TF32 off) on the bf16-rounded operands, on the same GPU.  The only
 differences left are the fp32 summation order and the final rounding of the output to bf16, hence
 |y - ref| <= 2^-8 |ref| + 1e-3 * max|ref| elementwise.
@@ -21,7 +21,7 @@ pytestmark = pytest.mark.gpu
 
 from oracle import irsde_oracle as O
 
-NUM_SMS = 148
+NUM_SMS = 132
 
 
 def _dev():
@@ -183,8 +183,8 @@ def _layer_report(net, P, xt, cond, t, nf, depth, variant="conditional"):
 
 
 def test_unet_nf64_forward_bf16_vs_oracle_per_layer(lib, capsys):
-    """ConditionalUNet(nf=64, depth=4) on 2x3x256x256 - every layer shape of BASELINE config 2, >= 148 tiles on every
-    256^2/128^2 launch - bf16 tcgen05 path vs the fp32 CPU oracle: each checkpointed layer within 1.5 % relative RMS and
+    """ConditionalUNet(nf=64, depth=4) on 2x3x256x256 - every layer shape of BASELINE config 2, >= 132 tiles on every
+    256^2/128^2 launch - bf16 tensor-core path vs the fp32 CPU oracle: each checkpointed layer within 1.5 % relative RMS and
     3 % of the layer's max (a bf16 pipeline: 2^-9 per rounding, ~60 roundings deep; measured 0.2-0.95 % rel-rms growing
     with depth), output within 4 % of its scale (measured 2.1 %)."""
     dev = _dev()
@@ -200,7 +200,7 @@ def test_unet_nf64_forward_bf16_vs_oracle_per_layer(lib, capsys):
     yo, rows = _layer_report(net, P, xt, cond, t, nf, depth)
     y = net(xt.to(dev), cond.to(dev), t).cpu()
     with capsys.disabled():
-        print("\nper-layer bf16 (tcgen05) vs fp32 oracle, nf=64 depth=4, 2x3x256x256, t=%d" % t)
+        print("\nper-layer bf16 (tensor cores) vs fp32 oracle, nf=64 depth=4, 2x3x256x256, t=%d" % t)
         for key, dmax, rmax, rel in rows:
             print("  %-38s max|d| %.3e  max|ref| %.3e  rel-rms %.2e" % (key, dmax, rmax, rel))
         print("  %-38s max|d| %.3e  max|ref| %.3e" % ("output (eps-hat)", (y - yo).abs().max().item(), yo.abs().max().item()))

@@ -1,9 +1,9 @@
 """Drop-in proof (SURVEY 8 b): the reference's own `codes/config/deraining/test.py` (test.py:67-72,93-110), UNMODIFIED,
 run twice on three synthetic PNG pairs with a random-weight checkpoint -
-  (A) through `python -m irsde_b200.run` (IRSDE + ConditionalUNet swapped for the native sm_100a sampler, fp32 parity mode),
+  (A) through `python -m irsde_b200.run` (IRSDE + ConditionalUNet swapped for the native sm_90a sampler, fp32 parity mode),
   (B) through `python -m irsde_b200.run --reference` (nothing swapped: the reference on PyTorch eager, same GPU) -
 with the same seed.  The PNGs both runs write must agree to within one grey level (uint8 rounding of a <=1e-3 difference).
-Needs the reference staged under baseline/_ref (baseline/make_ref.py, done by __graft_entry__.build()); skipped without it."""
+Needs the reference staged under oracle/_ref (oracle/make_ref.py, done by __graft_entry__.build()); skipped without it."""
 import os
 import shutil
 import subprocess
@@ -13,7 +13,7 @@ import pytest
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.path.join(ROOT, "baseline", "_ref")
+REF = os.path.join(ROOT, "oracle", "_ref")
 
 YML = """name: dropin
 suffix: ~
@@ -68,7 +68,7 @@ def test_reference_test_py_runs_unchanged(tmp_path, mode):
     if not torch.cuda.is_available():
         pytest.skip("needs a CUDA device")
     if not os.path.exists(os.path.join(REF, ".staged")):
-        pytest.skip("baseline/_ref not staged (python baseline/make_ref.py in the build container)")
+        pytest.skip("oracle/_ref not staged (python oracle/make_ref.py next to the reference checkout)")
     trees = {}
     for arm in ("native", "reference"):
         tree = str(tmp_path / arm)
@@ -84,10 +84,10 @@ def test_reference_test_py_runs_unchanged(tmp_path, mode):
         open(os.path.join(tree, "opt.yml"), "w").write(YML.format(root=tree, mode=mode))
         trees[arm] = tree
     # checkpoint: the REFERENCE network's own state dict (default init, seed 0), saved the way save_network does
-    sys.path.insert(0, os.path.join(ROOT, "baseline"))
+    sys.path.insert(0, os.path.join(ROOT, "oracle"))
     code = ("import sys, torch; sys.path.insert(0, %r); import ref_loader; u, m = ref_loader.load('deraining'); torch.manual_seed(0); "
             "net = m.ConditionalUNet(3, 3, 16, 2); torch.save({k: v.cpu() for k, v in net.state_dict().items()}, sys.argv[1])"
-            % os.path.join(ROOT, "baseline"))
+            % os.path.join(ROOT, "oracle"))
     for tree in trees.values():
         subprocess.run([sys.executable, "-c", code, os.path.join(tree, "ckpt.pth")], check=True, timeout=300)
     out_native = _run(trees["native"], ["--seed", "123"], {"IRSDE_B200_PRECISION": "fp32"}, str(tmp_path / "native.log"))
@@ -120,8 +120,8 @@ def test_validation_sampling_adopts_reference_module_during_training():
     if not torch.cuda.is_available():
         pytest.skip("needs a CUDA device")
     if not os.path.exists(os.path.join(REF, ".staged")):
-        pytest.skip("baseline/_ref not staged")
-    sys.path.insert(0, os.path.join(ROOT, "baseline"))
+        pytest.skip("oracle/_ref not staged")
+    sys.path.insert(0, os.path.join(ROOT, "oracle"))
     sys.path.insert(0, ROOT)
     import ref_loader
     rutil, rmods = ref_loader.load("deraining")

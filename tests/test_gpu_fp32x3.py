@@ -1,4 +1,4 @@
-"""The fp32-accurate tensor-core mode (precision="fp32x3": fp32 storage; every conv = three tcgen05.mma.kind::tf32 passes
+"""The fp32-accurate tensor-core mode (precision="fp32x3": fp32 storage; every conv = three tf32 wgmma passes
 over hi/lo split operands, conv_tc.cu MODE 3) against the same references and the SAME bounds as the fp32 SIMT parity mode:
 convs 2e-5 (summation order + the 2^-21 split residue), network forwards 1e-4, full chains the north-star 1e-3 max-abs."""
 import ctypes
@@ -61,7 +61,7 @@ CASES = [
     ("nearest x2 + 3x3 phases", 2, 128, 8, 12, 64, 3, 1, 1, True, True, False, False),
     ("head Cout=3 fp32 NCHW epilogue", 2, 64, 16, 24, 3, 3, 1, 1, False, True, False, False),
     ("to_qkv-like tiny K", 1, 8, 20, 28, 384, 1, 1, 0, False, False, False, False),
-    # benchmark shapes, >= 2 x 148 tiles per launch: persistent multi-tile loop + TMEM double buffering in MODE 3
+    # benchmark shapes, >= 2 x 132 tiles per launch: persistent multi-tile loop + segmented accumulation in MODE 3
     ("ups.0 block1 3x3 1536->1024 @32^2", 5, 1536, 32, 32, 1024, 3, 1, 1, False, False, True, False),
     ("downs.0 block 3x3 64->64 @256^2", 1, 64, 256, 256, 64, 3, 1, 1, False, False, True, True),
     ("ups.3 block1 3x3 192->128 @256^2", 1, 192, 256, 256, 128, 3, 1, 1, False, False, True, False),

@@ -1,4 +1,4 @@
-"""GPU parity tests (B200): the CUDA path, called through the C ABI, against the CPU oracle and the
+"""GPU parity tests (H100): the CUDA path, called through the C ABI, against the CPU oracle and the
 golden outputs of the imported reference.  Tolerances are stated per test.
 
 fp32 "parity mode" is held to the north-star bound (1e-3 max-abs per pixel) with large margin;
@@ -254,7 +254,7 @@ TC_CASES = [
 
 @pytest.mark.parametrize("case", TC_CASES)
 def test_conv_tcgen05(lib, scratch_ctx, case):
-    """tcgen05 tap-GEMM vs fp32 conv on bf16-rounded operands (fp32 accumulation => only the output
+    """Tensor-core (wgmma) tap-GEMM vs fp32 conv on bf16-rounded operands (fp32 accumulation => only the output
     rounding to bf16 and summation order differ): tolerance 2^-8 relative to the output scale."""
     B, Cin, H, W, Cout, K, s, p, up, hb, silu = case
     g = torch.Generator().manual_seed(sum(case[:6]))
@@ -275,7 +275,7 @@ def test_conv_tcgen05(lib, scratch_ctx, case):
 
 @pytest.mark.parametrize("force_simt", [True, False])
 def test_unet_forward_bf16(lib, golden, force_simt):
-    """bf16 perf mode (force_simt=True: same bf16 storage through the SIMT engine; False: tcgen05)
+    """bf16 perf mode (force_simt=True: same bf16 storage through the SIMT engine; False: tensor cores)
     vs the fp32 oracle on one forward: relative error of a bf16 pipeline (~1e-2 of the output scale)."""
     dev = _dev()
     P = O.make_weights(3, 3, 16, 3, seed=5)
@@ -431,7 +431,7 @@ def test_latent_unet_fp32_vs_reference(lib):
 
 def test_latent_unet_bf16_and_real_architecture(lib):
     """The shipped checkpoint's architecture (ch=8, ch_mult=[4,8,8,16], embed 8) with random weights: fp32 vs oracle
-    <= 2e-4, bf16 (tcgen05 path) within 4 % of the output scale."""
+    <= 2e-4, bf16 (tensor-core path) within 4 % of the output scale."""
     dev = _dev()
     cfg = dict(in_ch=3, out_ch=3, ch=8, ch_mult=[4, 8, 8, 16], embed_dim=8)
     P = O.make_latent_unet_weights(3, 3, 8, [4, 8, 8, 16], 8, seed=2)

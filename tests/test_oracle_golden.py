@@ -125,13 +125,14 @@ def test_latent_unet_oracle_vs_reference():
 
 
 def test_latent_unet_oracle_real_checkpoint():
-    """The shipped latent-dehazing.pth (2.0 M params) through the reference module vs the oracle (needs the reference)."""
+    """The shipped latent-dehazing.pth (2.0 M params) through the reference module vs the oracle (staged under oracle/_ref by build())."""
     import os
     import sys
-    ck = "/root/reference/codes/config/latent-dehazing/pretrained_models/latent-dehazing.pth"
+    ref = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "_ref")
+    ck = os.path.join(ref, "codes", "config", "latent-dehazing", "pretrained_models", "latent-dehazing.pth")
     if not os.path.exists(ck):
         import pytest
-        pytest.skip("reference checkout not available")
+        pytest.skip("oracle/_ref not staged")
     sys.path.insert(0, os.path.join(os.path.dirname(__file__), "golden"))
     from make_golden_latent import load_unet_arch
     arch = load_unet_arch()
@@ -157,7 +158,7 @@ def test_latent_unet_oracle_real_checkpoint():
     # re-ordered fp32 implementation (the GPU kernels) can be held to.
     import cv2
     import numpy as np
-    img = cv2.imread("/root/reference/images/1.png")
+    img = cv2.imread(os.path.join(ref, "images", "1.png"))
     xi = torch.from_numpy(img[:, :, [2, 1, 0]].astype(np.float32) / 255.).permute(2, 0, 1)[None][:, :, :160, :224].contiguous()
     with torch.no_grad():
         zi, hi = net.encode(xi)
@@ -217,7 +218,8 @@ def test_oracle_per_layer_trace_vs_reference_hooks():
     """The oracle's `trace=` checkpoints (what the GPU per-layer parity reports compare with) against forward hooks on the
     reference's own modules (tests/golden/make_golden_layers.py): every layer's fingerprint - shape, fp64 sum / abs-sum,
     <= 512 strided elements - for the conditional UNet (ragged input) and the denoising-sde variant (full Attention)."""
-    G = torch.load(os.path.join(os.path.dirname(__file__), "golden", "reference_golden_layers.pt"), weights_only=True)
+    import _golden
+    G = _golden.load("reference_golden_layers.pt")
     for variant, g in (("conditional", G["cond"]), ("denoising", G["denoising"])):
         c = g["cfg"]
         tr = {}
