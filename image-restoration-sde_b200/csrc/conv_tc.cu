@@ -14,9 +14,14 @@
 // issues wgmma.m64nBNk16 for 64 of the 128 pixel rows into its registers, then runs the epilogue: registers -> fp32 staging
 // in shared memory -> bias / (scale+1)*x+shift / SiLU / q-softmax / +residual -> bf16 -> swizzled staging -> TMA bulk store
 // at the channel offset of the destination concat buffer), warp 8 = TMA producer.  Pipeline: STAGES-deep smem ring with
-// full/empty mbarriers (each warpgroup releases a slot once wgmma.wait_group shows its MMAs on it are done); the producer
-// runs ahead into the next tile while the consumers run the epilogue.  Variants: MODE 0 per-tap boxes, MODE 2 ROWS (3x3,
-// row-window reuse), MODE 3 fp32x3 (3 x tf32 wgmma on split fp32 operands), EKT = epilogue features compiled in.
+// full/empty mbarriers.  Each consumer warpgroup issues a stage's MMAs as one wgmma group and keeps it in flight while it
+// waits for the next stage's bytes and issues that stage's group; wgmma.wait_group 1 then shows the older group done and
+// the warpgroup releases its slot.  The producer runs ahead into the next tile while the consumers run the epilogue.
+// No function call may sit inside the wgmma window (see mbar_wait), or ptxas serializes every wgmma; the kernel makes no
+// external call at all.  (The fp32x3 epilogue keeps calls to the IEEE-division slow path, a subroutine of the kernel
+// itself that runs after the K loop's final wait.)
+// Variants: MODE 0 per-tap boxes, MODE 2 ROWS (3x3, row-window reuse), MODE 3 fp32x3 (3 x tf32 wgmma on split fp32
+// operands), EKT = epilogue features compiled in.
 #include <cuda.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -90,7 +95,10 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Bounded wait: a protocol bug traps (fails the launch) instead of hanging the GPU.
+// Bounded wait: a protocol bug traps (fails the launch) instead of hanging the GPU.  No message is printed: printf
+// compiles to a call of vprintf, and ptxas serializes every wgmma of a kernel whose wgmma window contains a function call
+// (warning C7510: each HGMMA is then followed by a wait for zero groups in flight).  The consumers wait here while their
+// previous stage's MMAs are still running, so the call must not exist; tests/test_conv_tc_sass.py checks that it does not.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   long long t0 = 0;
   uint32_t spins = 0;
@@ -98,10 +106,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     if ((++spins & 0xfffu) == 0) {
       long long now = clock64();
       if (t0 == 0) t0 = now;
-      else if (now - t0 > 4000000000LL) {  // ~2 s
-        printf("irsde conv_tc: mbarrier wait timeout (block %d,%d thread %d)\n", blockIdx.x, blockIdx.y, threadIdx.x);
-        __trap();
-      }
+      else if (now - t0 > 4000000000LL) __trap();  // ~2 s
     }
   }
 }
@@ -214,7 +219,6 @@ constexpr int A_STAGE_BYTES = 128 * 128;  // 128 pixel rows x 64 bf16
 // barrier round covers 12 MMAs per warpgroup.
 constexpr int TF3_SEG = 2;  // fp32x3: k-iterations (of 32 channels, 12 MMAs each) accumulated from zero before a fp32 sum
 constexpr int ROWS_A_SLOT = 20 * 1024;  // (8+2) rows x 16 px x 128 B (or 18 x 8 px for narrow images)
-constexpr int ACC_PITCH = 68;           // fp32 accumulator staging row: 64 columns + 4 (conflict-free 16-byte row reads)
 constexpr int SMEM_LIMIT = 232448;      // 227 KB: the opt-in shared memory per block of sm_90
 
 // MODE 3 "fp32x3" (the fp32-accurate tensor-core mode, SURVEY 7 "Parity vs precision"): operands are fp32 tensors that were
@@ -227,14 +231,24 @@ struct TcCfgP {
   static constexpr bool ROWS = MODE == 2;
   static constexpr bool TF3 = MODE == 3;
   static constexpr int B_STAGE_BYTES = BN * 128;
-  // Epilogue staging for the TMA stores: one 2 KB tile per consumer warp (STG_BUFS = 2 alternates two tiles per warp).
-  static constexpr int STG_BUFS = TF3 ? 0 : 1;
+  // COMPACT epilogue (the two classes whose consumers wait longest on full barriers): the fp32 staging is filled in two
+  // 32-column passes per 64-column round, and each warp's bf16 TMA-store tile lives inside its warpgroup's fp32 staging
+  // rows.  That cuts the shared memory outside the ring from 54 528 B to 21 760 B (BN=256) / 53 504 B to 20 736 B
+  // (ROWS BN=128), which buys each of them one more ring stage.  Cost: per 64-column round three more warpgroup
+  // barriers, and the next round waits for the bulk stores to have read their tiles.
+  static constexpr bool COMPACT = (BN == 256 && MODE == 0) || (BN == 128 && MODE == 2);
+  static constexpr int ACC_COLS = COMPACT ? 32 : 64;      // fp32 columns staged per pass
+  static constexpr int ACC_PITCH = ACC_COLS + 4;          // + 4: conflict-free 16-byte row reads
+  // Epilogue staging for the TMA stores: one 2 KB tile per consumer warp (STG_BUFS = 2 alternates two tiles per warp;
+  // 0: no TMA store (fp32x3) or the tile is inside the fp32 staging rows (COMPACT)).
+  static constexpr int STG_BUFS = (TF3 || COMPACT) ? 0 : 1;
   static constexpr int BSUB = ROWS ? 3 : (TF3 ? 2 : 1);  // weight tiles per stage
   static constexpr int A_SLOT = TF3 ? 2 * A_STAGE_BYTES : (ROWS ? ROWS_A_SLOT : A_STAGE_BYTES);
   static constexpr int STAGE_BYTES = A_SLOT + BSUB * B_STAGE_BYTES;
   static constexpr int EPI_FLOATS = 2 * BN;
   static constexpr int STG_BYTES = STG_BUFS * 8 * 2048;  // per consumer warp: STG_BUFS 32 rows x 64 B staging tiles
-  static constexpr int ACC_BYTES = 2 * 64 * ACC_PITCH * 4;  // fp32 staging: 64 rows x 64 columns per warpgroup
+  static constexpr int ACC_WG_BYTES = 64 * ACC_PITCH * 4;  // fp32 staging of one warpgroup: 64 rows x ACC_COLS columns
+  static constexpr int ACC_BYTES = 2 * ACC_WG_BYTES;
   static constexpr int FIXED_BYTES = 1024 + STG_BYTES + ACC_BYTES + EPI_FLOATS * 4 + 256;
   static constexpr int STAGES_FIT = (SMEM_LIMIT - FIXED_BYTES) / STAGE_BYTES;
   static constexpr int STAGES = STAGES_FIT > 8 ? 8 : STAGES_FIT;
@@ -242,6 +256,10 @@ struct TcCfgP {
   static constexpr int SMEM_BYTES = FIXED_BYTES + STAGES * STAGE_BYTES;
   static_assert(STAGES >= 2, "shared memory holds fewer than two pipeline stages");
   static_assert(SMEM_BYTES <= SMEM_LIMIT, "over the 227 KB per-CTA shared memory limit");
+  static_assert(!(BN == 256 && MODE == 0) || STAGES == 4, "per-tap BN=256 is meant to run a 4-stage ring");
+  static_assert(!(BN == 128 && MODE == 2) || STAGES == 3, "ROWS BN=128 is meant to run a 3-stage ring");
+  // COMPACT: four 2 KB store tiles per warpgroup inside its staging rows, 512-byte aligned for the 64B swizzle
+  static_assert(!COMPACT || (4 * 2048 <= ACC_WG_BYTES && ACC_WG_BYTES % 1024 == 0), "store tiles do not fit the staging rows");
 };
 
 // One elected lane of a converged warp (the compiler recognises elect.sync and emits straight-line uniform
@@ -426,8 +444,10 @@ __global__ void __launch_bounds__(288, 1) conv_tc_persist_kernel(const __grid_co
   const int et = threadIdx.x;  // 0..255
   const int trow = P.t_ptr ? *P.t_ptr : 0;
   const bool affine = (P.ss != nullptr) || (P.bias != nullptr) || (P.mult_vec != nullptr);
-  uint8_t* const stg_base = smem_stg + warp * 2048 * (Cfg::STG_BUFS > 0 ? Cfg::STG_BUFS : 1);
+  constexpr int ACC_PITCH = Cfg::ACC_PITCH;
   float* const acc_stg = s_acc + wg * 64 * ACC_PITCH;
+  uint8_t* const stg_base = Cfg::COMPACT ? reinterpret_cast<uint8_t*>(acc_stg) + wq * 2048
+                                         : smem_stg + warp * 2048 * (Cfg::STG_BUFS > 0 ? Cfg::STG_BUFS : 1);
   const uint32_t a_off = (uint32_t)(wg * 64 * 128);  // this warpgroup's 64 pixel rows inside every A box
   const bool signaller = (threadIdx.x & 127) == 0;
   int stg_i = 0;  // staging tile used by the next bulk store (alternates when STG_BUFS == 2)
@@ -683,30 +703,67 @@ __global__ void __launch_bounds__(288, 1) conv_tc_persist_kernel(const __grid_co
       else return acc[r];
     };
     constexpr int NR = (BN + 63) / 64;
+    if constexpr (!Cfg::COMPACT) {
 #pragma unroll
-    for (int i = 0; i < NR; ++i) {
-      asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");  // this warpgroup's previous reads of the staging rows are done
+      for (int i = 0; i < NR; ++i) {
+        asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");  // this warpgroup's previous reads of the staging rows are done
 #pragma unroll
-      for (int jj = 0; jj < 8; ++jj) {
-        const int j = i * 8 + jj;  // n8 block of the accumulator: registers 4j .. 4j+3
-        if (j * 8 < BN) {
-          const int row = wq * 16 + (lane >> 2), col = jj * 8 + 2 * (lane & 3);
-          *reinterpret_cast<float2*>(acc_stg + row * ACC_PITCH + col) = make_float2(fin(4 * j), fin(4 * j + 1));
-          *reinterpret_cast<float2*>(acc_stg + (row + 8) * ACC_PITCH + col) = make_float2(fin(4 * j + 2), fin(4 * j + 3));
+        for (int jj = 0; jj < 8; ++jj) {
+          const int j = i * 8 + jj;  // n8 block of the accumulator: registers 4j .. 4j+3
+          if (j * 8 < BN) {
+            const int row = wq * 16 + (lane >> 2), col = jj * 8 + 2 * (lane & 3);
+            *reinterpret_cast<float2*>(acc_stg + row * ACC_PITCH + col) = make_float2(fin(4 * j), fin(4 * j + 1));
+            *reinterpret_cast<float2*>(acc_stg + (row + 8) * ACC_PITCH + col) = make_float2(fin(4 * j + 2), fin(4 * j + 3));
+          }
+        }
+        asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
+        const int c0 = i * 64 + half * 32;
+        if (c0 < BN && t.n0 + c0 < P.Cout) {  // chunks entirely past Cout carry no output
+          uint32_t v[32];
+          const float* src = acc_stg + ((wq & 1) * 32 + lane) * ACC_PITCH + half * 32;
+#pragma unroll
+          for (int g = 0; g < 8; ++g) {
+            const float4 f = *reinterpret_cast<const float4*>(src + 4 * g);
+            v[4 * g] = __float_as_uint(f.x); v[4 * g + 1] = __float_as_uint(f.y);
+            v[4 * g + 2] = __float_as_uint(f.z); v[4 * g + 3] = __float_as_uint(f.w);
+          }
+          process(std::integral_constant<int, EKT>{}, v, c0);  // EKT: the instantiation's epilogue specialisation
         }
       }
-      asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
-      const int c0 = i * 64 + half * 32;
-      if (c0 < BN && t.n0 + c0 < P.Cout) {  // chunks entirely past Cout carry no output
-        uint32_t v[32];
-        const float* src = acc_stg + ((wq & 1) * 32 + lane) * ACC_PITCH + half * 32;
+    } else {
+      // COMPACT: a 64-column round is staged in two 32-column passes; pass p carries columns 16p .. 16p+15 of both
+      // 32-channel chunks of the round, so every thread gathers its chunk's 32 values over the two passes.  The bf16
+      // store tiles live in the staging rows: before a round writes them, each warp waits until its previous bulk store
+      // has read its tile, and process() (which writes the tile) starts only after every read of the round.
 #pragma unroll
-        for (int g = 0; g < 8; ++g) {
-          const float4 f = *reinterpret_cast<const float4*>(src + 4 * g);
-          v[4 * g] = __float_as_uint(f.x); v[4 * g + 1] = __float_as_uint(f.y);
-          v[4 * g + 2] = __float_as_uint(f.z); v[4 * g + 3] = __float_as_uint(f.w);
+      for (int i = 0; i < NR; ++i) {
+        const int c0 = i * 64 + half * 32;  // BN is a multiple of 64 here
+        uint32_t v[32];
+#pragma unroll
+        for (int p = 0; p < 2; ++p) {
+          if (p == 0 && lane == 0) bulk_wait_read0();
+          asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");  // the staging rows are free
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) {
+            const int j = i * 8 + jj;  // n8 block of the accumulator: registers 4j .. 4j+3
+            if (((jj >> 1) & 1) == p) {
+              const int row = wq * 16 + (lane >> 2), col = (jj >> 2) * 16 + (jj & 1) * 8 + 2 * (lane & 3);
+              *reinterpret_cast<float2*>(acc_stg + row * ACC_PITCH + col) = make_float2(fin(4 * j), fin(4 * j + 1));
+              *reinterpret_cast<float2*>(acc_stg + (row + 8) * ACC_PITCH + col) = make_float2(fin(4 * j + 2), fin(4 * j + 3));
+            }
+          }
+          asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
+          // read even when the chunk is past Cout: v then stays defined on every path (fewer live registers)
+          const float* src = acc_stg + ((wq & 1) * 32 + lane) * ACC_PITCH + half * 16;
+#pragma unroll
+          for (int g = 0; g < 4; ++g) {
+            const float4 f = *reinterpret_cast<const float4*>(src + 4 * g);
+            v[p * 16 + 4 * g] = __float_as_uint(f.x); v[p * 16 + 4 * g + 1] = __float_as_uint(f.y);
+            v[p * 16 + 4 * g + 2] = __float_as_uint(f.z); v[p * 16 + 4 * g + 3] = __float_as_uint(f.w);
+          }
         }
-        process(std::integral_constant<int, EKT>{}, v, c0);  // EKT: the instantiation's epilogue specialisation
+        asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");  // every read of the round is done
+        if (t.n0 + c0 < P.Cout) process(std::integral_constant<int, EKT>{}, v, c0);
       }
     }
   }
