@@ -71,7 +71,9 @@ struct Epilogue {
   int ss_S;               // row length of the table
   int ss_off;             // offset of this block's (scale[Cout], shift[Cout]) inside a row
   int ss_img_stride;      // rows per image (0 = shared time, 1 = per-image time)
-  const float* mult_vec;  // per-output-channel multiplier (NAFBlock beta / gamma) or null; overrides the table's scale
+  // per-output-channel multiplier (NAFBlock beta / gamma) or null: out = (acc + bias) * mult_vec.  Never combined with the
+  // time table (tc_conv_create* and the plan builder refuse it), so the engines need no common order for the two.
+  const float* mult_vec;
   int silu;               // apply SiLU after modulation
   const void* res;        // residual view (same dtype as output) or null
   int res_pitch;
@@ -196,6 +198,8 @@ void tc_conv_destroy(TcConvDesc*);
 void tc_conv_set_runtime(TcConvDesc*, const float* ss, const int* t_ptr, int ss_img_stride);
 void tc_conv_set_out_nchw(TcConvDesc*, float* out, int cropH, int cropW);  // out==nullptr at create => fp32 NCHW output
 int tc_conv_launch(TcConvDesc*, cudaStream_t st);  // returns number of launches (1), <0 on error
+// the kernel tc_conv_launch would run now (call after tc_conv_set_runtime): {BN, MODE, EKT, number of output tiles}
+void tc_conv_query(const TcConvDesc*, int info[4]);
 bool tc_init(std::string* err);                    // resolves cuTensorMapEncodeTiled
 
 // ---- image conversion / metrics (imaging.cu) ---------------------------------------------------

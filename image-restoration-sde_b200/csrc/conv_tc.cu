@@ -890,6 +890,7 @@ TcConvDesc* tc_conv_create(const bf16* in, int in_pitch, int B, int Hin, int Win
   if (!nchw_out && (Cout % 8 || out_pitch % 8)) return bad("output channel count / pitch must be multiples of 8");
   if (((uintptr_t)in & 15) || ((uintptr_t)wpacked & 15) || ((uintptr_t)out & 15)) return bad("operands must be 16-byte aligned");
   if (ep.res && (((uintptr_t)ep.res & 15) || ep.res_pitch % 8)) return bad("residual must be 16-byte aligned");
+  if (ep.ss && ep.mult_vec) return bad("the time-modulation table and mult_vec cannot be combined");
   TcConvDesc* d = new TcConvDesc();
   TcParams& P = d->P;
   memset(&P, 0, sizeof P);
@@ -1033,6 +1034,7 @@ TcConvDesc* tc_conv_create_f32x3(const float* in_split, int B, int Hin, int Win,
   if (!nchw_out && (Cout % 4 || out_pitch % 4)) return bad("fp32x3: output channels / pitch must be multiples of 4");
   if (((uintptr_t)in_split & 15) || ((uintptr_t)wsplit & 15) || ((uintptr_t)out & 15)) return bad("operands must be 16-byte aligned");
   if (ep.res && (((uintptr_t)ep.res & 15) || ep.res_pitch % 4)) return bad("residual must be 16-byte aligned");
+  if (ep.ss && ep.mult_vec) return bad("the time-modulation table and mult_vec cannot be combined");
   TcConvDesc* d = new TcConvDesc();
   TcParams& P = d->P;
   memset(&P, 0, sizeof P);
@@ -1123,6 +1125,31 @@ void tc_conv_set_runtime(TcConvDesc* d, const float* ss, const int* t_ptr, int s
   }
 }
 
+// EKT of the conv_tc_persist_kernel instantiation that runs this descriptor: its epilogue kind where an instantiation is
+// specialised for it (and the IRSDE_TC_EPI_SPEC level enables that class), EK_GENERIC otherwise.  tc_conv_launch and
+// tc_conv_query both read it, so what the query reports is what runs.
+static int tc_launch_ekt(const TcConvDesc* d) {
+  if (d->mode == 3) return EK_GENERIC;
+  if (d->mode == 2) {
+    const int ek = g_epi_spec >= 2 ? d->P.epi_kind : EK_GENERIC;
+    return d->BN != 32 && (ek == (EK_AFF | EK_SILU) || ek == (EK_SILU | EK_RES)) ? ek : EK_GENERIC;
+  }
+  const int ek = g_epi_spec >= 1 ? d->P.epi_kind : EK_GENERIC;
+  switch (d->BN) {
+    case 64: return ek == 0 || ek == EK_AFF ? ek : EK_GENERIC;
+    case 128: return ek == 0 || ek == EK_AFF || ek == EK_QSM ? ek : EK_GENERIC;
+    case 256: return g_epi_spec >= 3 && (ek == 0 || ek == EK_AFF) ? ek : EK_GENERIC;  // deep res_conv; downsample / to_out (bias)
+    default: return EK_GENERIC;
+  }
+}
+
+void tc_conv_query(const TcConvDesc* d, int info[4]) {
+  info[0] = d->BN;
+  info[1] = d->mode;
+  info[2] = tc_launch_ekt(d);
+  info[3] = d->num_tiles;
+}
+
 int tc_conv_launch(TcConvDesc* d, cudaStream_t st) {
   {
     const unsigned g = (unsigned)(d->num_tiles < g_num_sms ? d->num_tiles : g_num_sms);
@@ -1134,56 +1161,50 @@ int tc_conv_launch(TcConvDesc* d, cudaStream_t st) {
       cudaMemsetAsync(dbg_dev, 0, 256 * 8 * sizeof(unsigned long long), st);
     }
     d->P.dbg = dbg ? dbg_dev : nullptr;
-#define TC_LAUNCH(BNV, PV) \
-  pdl_launch(conv_tc_persist_kernel<BNV, PV>, g, 288, TcCfgP<BNV, PV>::SMEM_BYTES, st, d->map_a, d->map_b, d->map_o, d->P, d->tiles_m, d->num_tiles)
+#define TC_LAUNCH(BNV, PV, EKV)                                                                                            \
+  pdl_launch(conv_tc_persist_kernel<BNV, PV, EKV>, g, 288, TcCfgP<BNV, PV>::SMEM_BYTES, st, d->map_a, d->map_b, d->map_o, d->P, \
+             d->tiles_m, d->num_tiles)
+    const int ekt = tc_launch_ekt(d);
     if (d->mode == 3) {
       switch (d->BN) {
-        case 32: TC_LAUNCH(32, 3); break;
-        case 64: TC_LAUNCH(64, 3); break;
-        default: TC_LAUNCH(128, 3); break;
+        case 32: TC_LAUNCH(32, 3, EK_GENERIC); break;
+        case 64: TC_LAUNCH(64, 3, EK_GENERIC); break;
+        default: TC_LAUNCH(128, 3, EK_GENERIC); break;
       }
     } else if (d->mode == 2) {
-#define TC_LAUNCH_EK2(BNV, EKV) \
-  pdl_launch(conv_tc_persist_kernel<BNV, 2, EKV>, g, 288, TcCfgP<BNV, 2>::SMEM_BYTES, st, d->map_a, d->map_b, d->map_o, d->P, d->tiles_m, d->num_tiles)
-      const int ek2 = g_epi_spec >= 2 ? d->P.epi_kind : EK_GENERIC;
       switch (d->BN) {
-        case 32: TC_LAUNCH(32, 2); break;
+        case 32: TC_LAUNCH(32, 2, EK_GENERIC); break;
         case 64:
-          if (ek2 == (EK_AFF | EK_SILU)) TC_LAUNCH_EK2(64, EK_AFF | EK_SILU);
-          else if (ek2 == (EK_SILU | EK_RES)) TC_LAUNCH_EK2(64, EK_SILU | EK_RES);
-          else TC_LAUNCH(64, 2);
+          if (ekt == (EK_AFF | EK_SILU)) TC_LAUNCH(64, 2, EK_AFF | EK_SILU);
+          else if (ekt == (EK_SILU | EK_RES)) TC_LAUNCH(64, 2, EK_SILU | EK_RES);
+          else TC_LAUNCH(64, 2, EK_GENERIC);
           break;
         default:
-          if (ek2 == (EK_AFF | EK_SILU)) TC_LAUNCH_EK2(128, EK_AFF | EK_SILU);
-          else if (ek2 == (EK_SILU | EK_RES)) TC_LAUNCH_EK2(128, EK_SILU | EK_RES);
-          else TC_LAUNCH(128, 2);
+          if (ekt == (EK_AFF | EK_SILU)) TC_LAUNCH(128, 2, EK_AFF | EK_SILU);
+          else if (ekt == (EK_SILU | EK_RES)) TC_LAUNCH(128, 2, EK_SILU | EK_RES);
+          else TC_LAUNCH(128, 2, EK_GENERIC);
           break;
       }
-#undef TC_LAUNCH_EK2
     } else {
-#define TC_LAUNCH_EK(BNV, EKV) \
-  pdl_launch(conv_tc_persist_kernel<BNV, 0, EKV>, g, 288, TcCfgP<BNV, 0>::SMEM_BYTES, st, d->map_a, d->map_b, d->map_o, d->P, d->tiles_m, d->num_tiles)
-      const int ek = g_epi_spec >= 1 ? d->P.epi_kind : EK_GENERIC;
       switch (d->BN) {
-        case 32: TC_LAUNCH(32, 0); break;
+        case 32: TC_LAUNCH(32, 0, EK_GENERIC); break;
         case 64:
-          if (ek == 0) TC_LAUNCH_EK(64, 0);
-          else if (ek == EK_AFF) TC_LAUNCH_EK(64, EK_AFF);
-          else TC_LAUNCH(64, 0);
+          if (ekt == 0) TC_LAUNCH(64, 0, 0);
+          else if (ekt == EK_AFF) TC_LAUNCH(64, 0, EK_AFF);
+          else TC_LAUNCH(64, 0, EK_GENERIC);
           break;
         case 128:
-          if (ek == 0) TC_LAUNCH_EK(128, 0);
-          else if (ek == EK_AFF) TC_LAUNCH_EK(128, EK_AFF);
-          else if (ek == EK_QSM) TC_LAUNCH_EK(128, EK_QSM);
-          else TC_LAUNCH(128, 0);
+          if (ekt == 0) TC_LAUNCH(128, 0, 0);
+          else if (ekt == EK_AFF) TC_LAUNCH(128, 0, EK_AFF);
+          else if (ekt == EK_QSM) TC_LAUNCH(128, 0, EK_QSM);
+          else TC_LAUNCH(128, 0, EK_GENERIC);
           break;
         default:
-          if (g_epi_spec >= 3 && ek == EK_AFF) TC_LAUNCH_EK(256, EK_AFF);   // downsample convs / deep to_out (bias)
-          else if (g_epi_spec >= 3 && ek == 0) TC_LAUNCH_EK(256, 0);       // deep res_conv
-          else TC_LAUNCH(256, 0);
+          if (ekt == EK_AFF) TC_LAUNCH(256, 0, EK_AFF);
+          else if (ekt == 0) TC_LAUNCH(256, 0, 0);
+          else TC_LAUNCH(256, 0, EK_GENERIC);
           break;
       }
-#undef TC_LAUNCH_EK
     }
 #undef TC_LAUNCH
     if (dbg) {

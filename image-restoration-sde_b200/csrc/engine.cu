@@ -575,6 +575,7 @@ struct Builder {
     ep.silu = silu;
     ep.ss_S = ctx->S;
     bool use_ss = !ss_block.empty();
+    if (use_ss && ep.mult_vec) { ok = false; err = "time modulation and mult_vec cannot be combined: " + wname; return; }
     ep.ss_off = use_ss ? ctx->ss_off[ss_block] : 0;
     if (res) { ep.res = res->p; ep.res_pitch = res->pitch; }
     irsde_ctx* c = ctx;
@@ -2242,6 +2243,183 @@ int irsde_conv2d_ex(irsde_ctx* ctx, int32_t engine, const float* x, const float*
     if (cudaStreamSynchronize(st) != cudaSuccess || cudaGetLastError() != cudaSuccess) rc = fail(ctx, IRSDE_ERR_CUDA, "conv2d failed");
   }
   for (void* q : tmp) { cudaFree(q); }
+  return rc;
+}
+
+__global__ void cast_f32_bf16_kernel(const float* __restrict__ in, bf16* __restrict__ out, long long n) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    out[i] = __float2bfloat16_rn(in[i]);
+}
+__global__ void cast_bf16_f32_kernel(const bf16* __restrict__ in, float* __restrict__ out, long long n) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    out[i] = __bfloat162float(in[i]);
+}
+
+int irsde_conv2d_fused(irsde_ctx* ctx, int32_t engine, const float* x, const float* w, const irsde_conv_epilogue* epi, float* y,
+                       int32_t B, int32_t Cin, int32_t H, int32_t W, int32_t Cout, int32_t KH, int32_t KW, int32_t stride,
+                       int32_t pad, int32_t upsample, int32_t* info, void* stream) {
+  // ---- everything is validated here, before the first launch: no argument may make a kernel index out of bounds
+  if (!ctx || !x || !w || !y || !epi) return fail(ctx, IRSDE_ERR_INVALID, "null argument");
+  const irsde_conv_epilogue& e = *epi;
+  if (engine < 0 || engine > 2) return fail(ctx, IRSDE_ERR_INVALID, "unknown engine");
+  if (B < 1 || Cin < 1 || H < 1 || W < 1 || Cout < 1) return fail(ctx, IRSDE_ERR_INVALID, "bad shape");
+  const int up = upsample ? 2 : 1;
+  const bool k3 = KH == 3 && KW == 3 && stride == 1 && pad == 1, k1 = KH == 1 && KW == 1 && stride == 1 && pad == 0 && up == 1,
+             k4 = KH == 4 && KW == 4 && stride == 2 && pad == 1 && up == 1 && H % 2 == 0 && W % 2 == 0;
+  if (!(k3 || k1 || k4)) return fail(ctx, IRSDE_ERR_UNSUPPORTED, "fused conv: 3x3/1 (optionally after nearest x2), 1x1 or 4x4/2");
+  const int Ho = (H * up + 2 * pad - KH) / stride + 1, Wo = (W * up + 2 * pad - KW) / stride + 1;
+  const bool nchw = e.crop_h != 0 || e.crop_w != 0;
+  const bool qsm = (e.flags & IRSDE_CONV_QSOFTMAX) != 0;
+  if (e.flags & ~IRSDE_CONV_QSOFTMAX) return fail(ctx, IRSDE_ERR_UNSUPPORTED, "fused conv: flags other than IRSDE_CONV_QSOFTMAX");
+  if (qsm && (engine != 1 || !k1 || Cout < 128 || nchw))
+    return fail(ctx, IRSDE_ERR_INVALID, "q-softmax is the bf16 epilogue of a 1x1 conv with Cout >= 128");
+  const int al = engine == 1 ? 8 : 4;  // elements per 16 bytes of the engine's storage type
+  auto view_ok = [&](int pitch, int off, int C) {
+    return off >= 0 && (long long)off + C <= pitch && off % al == 0 && pitch % al == 0;
+  };
+  if (engine != 0 && (Cin % al || (!nchw && Cout % al)))
+    return fail(ctx, IRSDE_ERR_INVALID, "tensor-core engines: Cin and Cout must be multiples of 16 bytes");
+  if (!view_ok(e.in_pitch, e.in_off, Cin)) return fail(ctx, IRSDE_ERR_INVALID, "input view outside its pitch or not 16-byte aligned");
+  if (nchw) {
+    if (!k3 || up != 1) return fail(ctx, IRSDE_ERR_UNSUPPORTED, "the cropped fp32 NCHW output is the 3x3 head's epilogue");
+    if (e.crop_h < 1 || e.crop_w < 1 || e.crop_h > Ho || e.crop_w > Wo) return fail(ctx, IRSDE_ERR_INVALID, "crop larger than the output");
+    if (e.res) return fail(ctx, IRSDE_ERR_UNSUPPORTED, "no residual with the NCHW output");
+  } else if (!view_ok(e.out_pitch, e.out_off, Cout)) {
+    return fail(ctx, IRSDE_ERR_INVALID, "output view outside its pitch or not 16-byte aligned");
+  }
+  if (e.res && !view_ok(e.res_pitch, e.res_off, Cout))
+    return fail(ctx, IRSDE_ERR_INVALID, "residual view outside its pitch or not 16-byte aligned");
+  if (e.ss) {
+    if (e.mult_vec) return fail(ctx, IRSDE_ERR_INVALID, "the time-modulation table and mult_vec cannot be combined");
+    if (e.t_row < 0 || e.ss_img_stride < 0 || (long long)e.t_row + (long long)(B - 1) * e.ss_img_stride >= e.ss_rows)
+      return fail(ctx, IRSDE_ERR_INVALID, "time-modulation row outside the table");
+    if (e.ss_off < 0 || (long long)e.ss_off + 2LL * Cout > e.ss_S)
+      return fail(ctx, IRSDE_ERR_INVALID, "scale / shift columns outside the table row");
+  }
+  const float* ptrs[] = {x, y, e.res, e.bias, e.mult_vec, e.ss};
+  for (const float* q : ptrs)
+    if ((uintptr_t)q & 15) return fail(ctx, IRSDE_ERR_INVALID, "device buffers must be 16-byte aligned");
+  int32_t info_local[4];
+  if (!info) info = info_local;
+  info[0] = info[1] = info[2] = info[3] = 0;
+
+  cudaSetDevice(ctx->cfg.device);
+  cudaStream_t st = (cudaStream_t)stream;
+  std::string terr;
+  if (engine != 0 && !tc_init(&terr)) return fail(ctx, IRSDE_ERR_CUDA, "tc_init: " + terr);
+  const long long npix_in = (long long)B * H * W, npix_out = (long long)B * Ho * Wo;
+  const int Cout_pad = (Cout + 7) / 8 * 8;
+  std::vector<void*> tmp;
+  int rc = IRSDE_OK;
+  int* t_dev = (int*)dev_alloc(ctx, sizeof(int), &tmp);
+  if (!t_dev) rc = fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
+  if (!rc) cudaMemcpyAsync(t_dev, &e.t_row, sizeof(int), cudaMemcpyHostToDevice, st);
+  Epilogue ep;
+  memset(&ep, 0, sizeof ep);
+  ep.bias = e.bias;
+  ep.mult_vec = e.mult_vec;
+  ep.silu = e.silu;
+  ep.ss_S = e.ss_S;
+  ep.ss_off = e.ss_off;
+  ep.res_pitch = e.res_pitch;
+  // same taps as the plan builder (conv_impl)
+  TcTap taps[16];
+  int ntaps = 0, nph = 1, planes = 1, Ha = H, Wa = W;
+  if (k3 && up == 1) { for (int r = 0; r < 3; ++r) for (int q = 0; q < 3; ++q) taps[ntaps++] = TcTap{r - 1, q - 1, 0}; }
+  else if (k3) { nph = 4; for (int a = 0; a < 2; ++a) for (int q = 0; q < 2; ++q) taps[ntaps++] = TcTap{a - 1, q - 1, 0}; }
+  else if (k1) { taps[ntaps++] = TcTap{0, 0, 0}; }
+  else {
+    static const int PY[4] = {1, 0, 1, 0}, DH[4] = {-1, 0, 0, 1};
+    for (int r = 0; r < 4; ++r) for (int q = 0; q < 4; ++q) taps[ntaps++] = TcTap{DH[r], DH[q], PY[r] * 2 + PY[q]};
+    planes = 4; Ha = H / 2; Wa = W / 2;
+  }
+  auto blocks = [](long long n) { return (unsigned)std::min<long long>((n + 255) / 256, 65536); };
+  TcConvDesc* d = nullptr;
+  bf16* yb = nullptr;
+  if (!rc && engine == 0) {
+    ConvGeom g;
+    g.B = B; g.Hin = H; g.Win = W; g.Cin = Cin; g.up = up; g.KH = KH; g.KW = KW; g.stride = stride; g.pad = pad;
+    g.Hout = Ho; g.Wout = Wo; g.Cout = Cout;
+    const long long nw = (long long)Cout * Cin * KH * KW;
+    float* wp = (float*)dev_alloc(ctx, nw * 4, &tmp);
+    if (!wp) rc = fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
+    if (!rc) {
+      pack_simt_kernel<<<(unsigned)((nw + 255) / 256), 256, 0, st>>>(w, wp, Cout, Cin, KH, KW);
+      if (e.ss) { ep.ss = e.ss; ep.t_ptr = t_dev; ep.ss_img_stride = e.ss_img_stride; }
+      if (e.res) ep.res = e.res + e.res_off;
+      launch_conv_simt<float>(g, x + e.in_off, e.in_pitch, wp, ep, nchw ? nullptr : y + e.out_off, e.out_pitch, nchw ? y : nullptr,
+                              e.crop_h, e.crop_w, st);
+    }
+  } else if (!rc && engine == 1) {
+    const long long nin = npix_in * e.in_pitch;
+    const long long nwt = (k3 && up == 2) ? 16LL * Cout * Cin : (long long)Cout_pad * Cin * KH * KW;
+    bf16* xb = (bf16*)dev_alloc(ctx, nin * 2, &tmp);
+    bf16* s2d = k4 ? (bf16*)dev_alloc(ctx, npix_in * Cin * 2, &tmp) : nullptr;
+    bf16* wp = (bf16*)dev_alloc(ctx, nwt * 2, &tmp);
+    bf16* rb = e.res ? (bf16*)dev_alloc(ctx, npix_out * e.res_pitch * 2, &tmp) : nullptr;
+    yb = nchw ? nullptr : (bf16*)dev_alloc(ctx, npix_out * e.out_pitch * 2, &tmp);
+    if (!xb || (k4 && !s2d) || !wp || (e.res && !rb) || (!nchw && !yb)) rc = fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
+    if (!rc) {
+      cast_f32_bf16_kernel<<<blocks(nin), 256, 0, st>>>(x, xb, nin);
+      if (rb) cast_f32_bf16_kernel<<<blocks(npix_out * e.res_pitch), 256, 0, st>>>(e.res, rb, npix_out * e.res_pitch);
+      if (yb) cast_f32_bf16_kernel<<<blocks(npix_out * e.out_pitch), 256, 0, st>>>(y, yb, npix_out * e.out_pitch);
+      if (k3 && up == 2) pack_tc_up_kernel<<<(unsigned)((nwt + 255) / 256), 256, 0, st>>>(w, wp, Cout, Cin);
+      else pack_tc_padded_kernel<<<(unsigned)((nwt + 255) / 256), 256, 0, st>>>(w, wp, Cout, Cout_pad, Cin, KH, KW);
+      const bf16* a_ptr = xb + e.in_off;
+      int a_pitch = e.in_pitch;
+      if (k4) {
+        launch_space_to_depth<bf16>(a_ptr, a_pitch, s2d, B, H, W, Cin, st);
+        a_ptr = s2d;
+        a_pitch = Cin;
+      }
+      if (rb) ep.res = rb + e.res_off;
+      d = tc_conv_create(a_ptr, a_pitch, B, Ha, Wa, Cin, planes, wp, Cout, ntaps, taps, nph, ep, nchw ? nullptr : yb + e.out_off,
+                         e.out_pitch, Ho, Wo, &terr, qsm ? TC_FLAG_QSOFTMAX : 0);
+      if (!d) rc = fail(ctx, IRSDE_ERR_INVALID, "tc_conv_create: " + terr);
+    }
+  } else if (!rc) {
+    const long long nwt = (long long)((k3 && up == 2) ? 16 : KH * KW) * 2 * Cout_pad * Cin;
+    float* s2d = k4 ? (float*)dev_alloc(ctx, npix_in * Cin * 4, &tmp) : nullptr;
+    float* xsp = (float*)dev_alloc(ctx, 2 * npix_in * Cin * 4, &tmp);  // planes * Ha * Wa == H * W
+    float* wp = (float*)dev_alloc(ctx, nwt * 4, &tmp);
+    if ((k4 && !s2d) || !xsp || !wp) rc = fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
+    if (!rc) {
+      if (k3 && up == 2) pack_tc3_up_kernel<<<(unsigned)((nwt / 2 + 255) / 256), 256, 0, st>>>(w, wp, Cout, Cout_pad, Cin);
+      else pack_tc3_kernel<<<(unsigned)((nwt / 2 + 255) / 256), 256, 0, st>>>(w, wp, Cout, Cout_pad, Cin, KH, KW);
+      const float* a_src = x + e.in_off;
+      int a_pitch = e.in_pitch;
+      if (k4) {
+        launch_space_to_depth<float>(a_src, a_pitch, s2d, B, H, W, Cin, st);
+        a_src = s2d;
+        a_pitch = Cin;
+      }
+      launch_split_tf32(a_src, a_pitch, xsp, (long long)planes * B * Ha * Wa, Cin, st);
+      if (e.res) ep.res = e.res + e.res_off;
+      d = tc_conv_create_f32x3(xsp, B, Ha, Wa, Cin, planes, wp, Cout, ntaps, taps, nph, ep, nchw ? nullptr : y + e.out_off,
+                               e.out_pitch, Ho, Wo, &terr);
+      if (!d) rc = fail(ctx, IRSDE_ERR_INVALID, "tc_conv_create_f32x3: " + terr);
+    }
+  }
+  if (!rc && d) {
+    // as the plan's launch closures do: the table, its row pointer and the image stride arrive after the descriptor exists
+    if (e.ss) tc_conv_set_runtime(d, e.ss, t_dev, e.ss_img_stride);
+    if (nchw) tc_conv_set_out_nchw(d, y, e.crop_h, e.crop_w);
+    int q[4];
+    tc_conv_query(d, q);
+    for (int i = 0; i < 4; ++i) info[i] = q[i];
+    tc_conv_launch(d, st);
+    if (yb) cast_bf16_f32_kernel<<<blocks(npix_out * e.out_pitch), 256, 0, st>>>(yb, y, npix_out * e.out_pitch);
+  }
+  if (!rc) {
+    ctx->launches += 4;
+    cudaError_t ce = cudaStreamSynchronize(st);
+    if (ce == cudaSuccess) ce = cudaGetLastError();
+    if (ce != cudaSuccess) rc = fail(ctx, IRSDE_ERR_CUDA, std::string("fused conv2d failed: ") + cudaGetErrorString(ce));
+  } else {
+    cudaStreamSynchronize(st);  // conversions already queued read buffers freed below
+  }
+  if (d) tc_conv_destroy(d);
+  for (void* q : tmp) cudaFree(q);
   return rc;
 }
 

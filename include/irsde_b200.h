@@ -212,6 +212,35 @@ int irsde_conv2d_ex(irsde_ctx* ctx, int32_t engine, const float* x, const float*
                     float* y, int32_t B, int32_t Cin, int32_t H, int32_t W, int32_t Cout, int32_t KH, int32_t KW,
                     int32_t stride, int32_t pad, int32_t upsample, int32_t silu, int32_t flags, void* stream);
 
+/* The fused epilogue of one network conv, with the views the launch plan gives it.  All pointers are device pointers. */
+typedef struct {
+  const float* bias;     /* [Cout] or NULL */
+  const float* mult_vec; /* [Cout] or NULL: (acc + bias) * mult_vec (NAFBlock beta / gamma); not allowed together with ss */
+  const float* ss;       /* time-modulation table [ss_rows][ss_S] or NULL: image b uses row t_row + b * ss_img_stride, */
+                         /* scale = row[ss_off + n], shift = row[ss_off + Cout + n]: (acc + bias) * (scale + 1) + shift  */
+  const float* res;      /* residual added last, fp32 NHWC [B][Ho][Wo][res_pitch] read at channels res_off.., or NULL */
+  int32_t silu;          /* SiLU after the modulation, before the residual */
+  int32_t flags;         /* IRSDE_CONV_QSOFTMAX (engine 1, 1x1) */
+  int32_t ss_rows, ss_S, ss_off, ss_img_stride, t_row;
+  int32_t res_pitch, res_off;
+  int32_t in_pitch, in_off;   /* x is fp32 NHWC [B][H][W][in_pitch]; the conv reads channels in_off .. in_off+Cin-1 */
+  int32_t out_pitch, out_off; /* y is fp32 NHWC [B][Ho][Wo][out_pitch]; the conv writes channels out_off .. out_off+Cout-1 */
+  int32_t crop_h, crop_w;     /* > 0 (3x3 head only): y is fp32 NCHW [B][Cout][crop_h][crop_w] instead, the output's */
+                              /* top-left crop_h x crop_w pixels; out_pitch / out_off are then ignored */
+} irsde_conv_epilogue;
+
+/* One conv of the launch plan with its fused epilogue, through the same descriptor and launch calls the plan builder uses
+ * (engine 0 = fp32 SIMT, 1 = bf16 wgmma, 2 = fp32x3 wgmma; KxK/stride/pad/upsample as in irsde_conv2d, 3x3/1, 1x1 and 4x4/2).
+ * y is read and written: the whole buffer is converted to the engine's storage type (bf16 for engine 1), the conv writes its
+ * slice, and the whole buffer is converted back, so an element outside the slice comes back unchanged when it is
+ * representable in that type.  Every view, table row and crop is checked on the host before anything is launched; offsets
+ * and pitches must be multiples of 16 bytes of the engine's storage type.
+ * info (or NULL) receives {BN, MODE, EKT, number of output tiles} of the conv_tc_persist_kernel instantiation that ran
+ * (engines 1 and 2), or zeros (engine 0). */
+int irsde_conv2d_fused(irsde_ctx* ctx, int32_t engine, const float* x, const float* w, const irsde_conv_epilogue* ep, float* y,
+                       int32_t B, int32_t Cin, int32_t H, int32_t W, int32_t Cout, int32_t KH, int32_t KW, int32_t stride,
+                       int32_t pad, int32_t upsample, int32_t* info, void* stream);
+
 /* ---- launch-plan introspection (parity instrumentation: per-layer comparison with the oracle) ----
  * The network forward for a (B,H,W) input is a fixed list of ops.  irsde_plan_num_ops returns its length (or a negative
  * irsde_status); irsde_plan_op_info gives op `op`'s label (the state-dict name of the weight it applies, e.g.
