@@ -1,31 +1,14 @@
 // HBM-bound kernels around the attention sites of the UNet: channel LayerNorm, LinearAttention
 // (module_util.py:150-178) and the full softmax Attention of the denoising-sde variant (:182-204).
 // All loads/stores are 128-bit vectors over the NHWC channel dimension; math is fp32.
+// Where one operation has several kernels, the launcher picks by what the operands allow (channel geometry, pitch and
+// alignment): the general kernels serve the views the specialised ones cannot take.
 #include <math.h>
-#include <stdlib.h>
 #include <string.h>
 
 #include "common.cuh"
 
 namespace irsde {
-
-// Newer kernels of this file, one bit each (IRSDE_HBM_NEW; 0 = the previous kernels, kept for A/B runs and as the reference
-// the newer ones are compared against).  IRSDE_HBM_DEFAULT is the default setting.
-//   1 = LayerNorm with compile-time lane geometry     2 = la_combine with 128-bit record loads
-//   4 = la_fold with 16 output rows per block          8 = k/v pass with warp-shuffle, branch-free softmax statistics
-//  16 = la_combine with the records spread over 8 warps (takes precedence over 2)
-#define IRSDE_HBM_DEFAULT 31
-#define IRSDE_LN_PP_DEFAULT 2
-static int hbm_mask_from_env() {
-  const char* e = getenv("IRSDE_HBM_NEW");
-  return e && *e ? atoi(e) : IRSDE_HBM_DEFAULT;
-}
-static const int g_hbm_new = hbm_mask_from_env();
-static int ln_pp_from_env() {  // pixels per lane group of layernorm_geo_kernel (rows of <= 2 vectors per lane)
-  const char* e = getenv("IRSDE_LN_PP");
-  return e && *e ? (*e == '1' ? 1 : 2) : IRSDE_LN_PP_DEFAULT;
-}
-static const int g_ln_pp = ln_pp_from_env();
 
 // accurate exp in parity (fp32) mode, fast exp in perf (bf16) mode
 template <typename T>
@@ -297,24 +280,17 @@ void launch_layernorm(const T* x, int x_pitch, const float* g, const T* res, int
   }
   const int warps = 8;
   long long pix_per_block = (long long)warps * (32 / lpp);
-  if ((g_hbm_new & 1) && nvec == lpp * per_lane && (per_lane & (per_lane - 1)) == 0 && lpp >= 8 && npix > 0) {
-    // exact geometry: C == N * LPP * MAXV.  PP pixels per lane group (IRSDE_LN_PP, default 2) while the row fits 2 vectors per lane.
+  if (nvec == lpp * per_lane && (per_lane & (per_lane - 1)) == 0 && lpp >= 8 && npix > 0) {
+    // exact geometry: C == N * LPP * MAXV.  Two pixels per lane group while the row fits 2 vectors per lane.
 #define LN_GEO(MV, LP, PPX)                                                                                              \
   pdl_launch(layernorm_geo_kernel<T, MV, LP, PPX>, (unsigned)((npix + pix_per_block * PPX - 1) / (pix_per_block * PPX)),   \
              warps * 32, 0, st, x, x_pitch, g, res, res_pitch, out, out_pitch, npix, C, 1.0f / (float)C, mod)
-#define LN_GEO_PP(MV, LP)                \
-  do {                                   \
-    if (g_ln_pp == 2) LN_GEO(MV, LP, 2); \
-    else LN_GEO(MV, LP, 1);              \
-    return;                              \
-  } while (0)
-    if (lpp == 8 && per_lane == 1) LN_GEO_PP(1, 8);
-    if (lpp == 16 && per_lane == 1) LN_GEO_PP(1, 16);
-    if (lpp == 32 && per_lane == 1) LN_GEO_PP(1, 32);
-    if (lpp == 32 && per_lane == 2) LN_GEO_PP(2, 32);
+    if (lpp == 8 && per_lane == 1) { LN_GEO(1, 8, 2); return; }
+    if (lpp == 16 && per_lane == 1) { LN_GEO(1, 16, 2); return; }
+    if (lpp == 32 && per_lane == 1) { LN_GEO(1, 32, 2); return; }
+    if (lpp == 32 && per_lane == 2) { LN_GEO(2, 32, 2); return; }
     if (lpp == 32 && per_lane == 4) { LN_GEO(4, 32, 1); return; }
     if (lpp == 32 && per_lane == 8 && sizeof(T) == 4) { LN_GEO(8, 32, 1); return; }
-#undef LN_GEO_PP
 #undef LN_GEO
   }
   unsigned grid = (unsigned)((npix + pix_per_block - 1) / pix_per_block);
@@ -337,7 +313,7 @@ template void launch_layernorm<bf16>(const bf16*, int, const float*, const bf16*
 // qkv channel layout: [q(4x32) | k(4x32) | v(4x32)], head h = channels h*32..h*32+31 of each third.
 //   pass A (la_kv): each block streams chunks of 64 pixels of ONE image, all 4 heads, keeping running
 //           (max, sum, ctx[32x32]) per head with the online-softmax rescale; one partial per block
-//   pass B (la_combine): merge the per-block partials: ctx[d][e] = sum_n softmax_n(k)[d,n] v[e,n] / N
+//   pass B (la_combine8): merge the per-block partials: ctx[d][e] = sum_n softmax_n(k)[d,n] v[e,n] / N
 //   pass C (la_out): per pixel/head: q = softmax_d(q) * 32^-.5 ; out[e] = sum_d ctx[d][e] q[d]
 // =============================================================================================
 static const int LA_PIX = 64;               // pixels per chunk
@@ -449,98 +425,11 @@ __global__ void __launch_bounds__(256) la_kv_kernel(const T* __restrict__ qkv, i
   for (int j = 0; j < 16; j += 4) *reinterpret_cast<float4*>(cp + j) = make_float4(acc[j], acc[j + 1], acc[j + 2], acc[j + 3]);
 }
 
-// One block = 256 ctx entries (8 d-rows x 32 e) of one (image, head); the loops over the <= 64 partial records are fully
-// unrolled so that all their loads are in flight at once: the kernel is pure dependent-load latency.  Same arithmetic and summation order per entry as before (bit-identical ctx).
-__global__ void __launch_bounds__(256) la_combine_kernel(const float* __restrict__ part, float* __restrict__ ctx,
-                                                         int N, int nblk) {
-  PDL_ENTRY();
-  const int bh = blockIdx.x >> 2, b = bh >> 2, h = bh & 3, tid = (blockIdx.x & 3) * 256 + threadIdx.x;
-  const int d = tid >> 5;
-  const float* base = part + (long long)b * LA_MAXBLK * LA_REC + h * 1088;
-  float mk[LA_MAXBLK];
-#pragma unroll
-  for (int k = 0; k < LA_MAXBLK; ++k) mk[k] = k < nblk ? base[(long long)k * LA_REC + d] : -INFINITY;
-  float M = -INFINITY;
-#pragma unroll
-  for (int k = 0; k < LA_MAXBLK; ++k) M = fmaxf(M, mk[k]);
-  float S = 0.f, acc = 0.f;
-#pragma unroll
-  for (int k0 = 0; k0 < LA_MAXBLK; k0 += 16) {   // 16 records (32 loads) in flight per batch
-    float sk[16], ck[16];
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      const float* rec = base + (long long)(k0 + j) * LA_REC;
-      sk[j] = (k0 + j) < nblk ? rec[32 + d] : 0.f;
-      ck[j] = (k0 + j) < nblk ? rec[64 + tid] : 0.f;
-    }
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      if (k0 + j < nblk) {
-        const float w = expf(mk[k0 + j] - M);
-        S += sk[j] * w;
-        acc += ck[j] * w;
-      }
-    }
-  }
-  ctx[(long long)bh * 1024 + tid] = acc / S / (float)N;
-}
-
-// Wide-load merge.  la_combine_kernel above issues 192 scalar requests per thread (1 536 per block / SM): its time is the
-// SM's outstanding-request limit, not latency of a single chain.  Here one WARP owns 4 d-rows of one
-// (image, head) = 128 ctx entries as one float4 per lane: the 64 records' (m, s) for those rows come in as two float4 loads
-// per lane and are shared through shared memory, and each record's ctx slice is ONE 128-bit request per lane, 32 records
-// in flight.  Per entry the arithmetic and its order are those of la_combine_kernel (bit-identical ctx).
-__global__ void __launch_bounds__(32) la_combine4_kernel(const float* __restrict__ part, float* __restrict__ ctx, int N, int nblk) {
-  PDL_ENTRY();
-  __shared__ __align__(16) float ms[LA_MAXBLK][4], ss[LA_MAXBLK][4];
-  const int bh = blockIdx.x >> 3, b = bh >> 2, h = bh & 3, d0 = (blockIdx.x & 7) * 4;
-  const int lane = threadIdx.x, dd = lane >> 3, e4 = (lane & 7) * 4;
-  const float* base = part + (long long)b * LA_MAXBLK * LA_REC + h * 1088;
-#pragma unroll
-  for (int k = lane; k < LA_MAXBLK; k += 32) {
-    float4 m4 = make_float4(-INFINITY, -INFINITY, -INFINITY, -INFINITY), s4 = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (k < nblk) {
-      m4 = *reinterpret_cast<const float4*>(base + (long long)k * LA_REC + d0);
-      s4 = *reinterpret_cast<const float4*>(base + (long long)k * LA_REC + 32 + d0);
-    }
-    *reinterpret_cast<float4*>(ms[k]) = m4;
-    *reinterpret_cast<float4*>(ss[k]) = s4;
-  }
-  __syncwarp();
-  float M = -INFINITY;
-#pragma unroll
-  for (int k = 0; k < LA_MAXBLK; ++k) M = fmaxf(M, ms[k][dd]);
-  const float* cbase = base + 64 + (d0 + dd) * 32 + e4;
-  float S = 0.f;
-  float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-  for (int k0 = 0; k0 < LA_MAXBLK; k0 += 32) {
-    float4 ck[32];
-#pragma unroll
-    for (int j = 0; j < 32; ++j)
-      ck[j] = (k0 + j) < nblk ? *reinterpret_cast<const float4*>(cbase + (long long)(k0 + j) * LA_REC) : make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-    for (int j = 0; j < 32; ++j) {
-      if (k0 + j < nblk) {
-        const float w = expf(ms[k0 + j][dd] - M);
-        S += ss[k0 + j][dd] * w;
-        acc.x += ck[j].x * w;
-        acc.y += ck[j].y * w;
-        acc.z += ck[j].z * w;
-        acc.w += ck[j].w * w;
-      }
-    }
-  }
-  const float fN = (float)N;
-  *reinterpret_cast<float4*>(ctx + (long long)bh * 1024 + (d0 + dd) * 32 + e4) =
-      make_float4(acc.x / S / fN, acc.y / S / fN, acc.z / S / fN, acc.w / S / fN);
-}
-
-// Merge with the records spread over warps.  la_combine4_kernel turned the request storm into 40 wide loads per lane, but
-// what remains is ONE warp walking the <= 64 records in sequence (expf + 5 dependent FMAs each).
-// Here the 8 warps of a block take records w, w + 8, ... (<= 8 each, all loads in flight at once), and warp 0 adds the 8
-// partial (S, ctx) pairs in a fixed order.  The record partition does not depend on the batch, so batch-sharded runs stay
-// bit-identical; the summation order differs from la_combine_kernel (fp32 rounding only).
+// Merge of the per-block partial records of one image.  One WARP owns 4 d-rows of one (image, head) = 128 ctx entries as
+// one float4 per lane: the records' (m, s) for those rows come in as float4 loads and are shared through shared memory, and
+// each record's ctx slice is ONE 128-bit request per lane.  The 8 warps of a block take records w, w + 8, ... (<= 8 each,
+// all loads in flight at once), and warp 0 adds the 8 partial (S, ctx) pairs in a fixed order.  The record partition does
+// not depend on the batch, so the summation order, and with it the result, is the same for batch-sharded runs.
 __global__ void __launch_bounds__(256) la_combine8_kernel(const float* __restrict__ part, float* __restrict__ ctx, int N, int nblk) {
   PDL_ENTRY();
   __shared__ __align__(16) float ms[LA_MAXBLK][4], ss[LA_MAXBLK][4];
@@ -653,7 +542,7 @@ __global__ void __launch_bounds__(256) la_out_kernel(const T* __restrict__ qkv, 
 // ---------------------------------------------------------------------------------------------
 static const int LAM_TP = 264;  // tile row pitch (bf16): 256 + 8 pad -> conflict-free ldmatrix
 static const int LAM_PP = 136;  // P row pitch (bf16): 128 + 8 pad
-static const size_t LAM_SMEM = (size_t)2 * LA_PIX * LAM_TP * 2 + (size_t)LA_PIX * LAM_PP * 2 + (128 * 3 + 4 * 128) * 4;
+static const size_t LAM_SMEM = (size_t)2 * LA_PIX * LAM_TP * 2 + (size_t)LA_PIX * LAM_PP * 2 + 128 * 4;
 
 __device__ __forceinline__ void ldsm_x4_trans(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
   asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
@@ -672,25 +561,20 @@ __device__ __forceinline__ void mma_bf16_16816(float* c, uint32_t a0, uint32_t a
                : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
 }
 
-// SHFL: the softmax statistics of a chunk stay inside a warp.  Lane (qtr = lane / 4, cpl = lane % 4) of warp w
-// owns channel pairs w*4+cpl and 32+w*4+cpl on the 8 pixels px == qtr (mod 8): the running max / sum live in registers
-// (replicated over the 8 qtr lanes), the cross-pixel max and sum are three xor-shuffles each, and the bf16x2 accesses
-// (word = 4*px + pair mod 32) are bank-conflict free.  One chunk then needs TWO block barriers (tile landed / P and alpha
-// visible to the MMA warps) instead of five: in the <false> form the per-chunk barrier chain, not memory, is the bound.
-template <bool SHFL>
+// The softmax statistics of a chunk stay inside a warp.  Lane (qtr = lane / 4, cpl = lane % 4) of warp w owns channel
+// pairs w*4+cpl and 32+w*4+cpl on the 8 pixels px == qtr (mod 8): the running max / sum live in registers (replicated over
+// the 8 qtr lanes), the cross-pixel max and sum are three xor-shuffles each, and the bf16x2 accesses
+// (word = 4*px + pair mod 32) are bank-conflict free.  One chunk needs two block barriers: tile landed, and P and alpha
+// visible to the MMA warps.
 __global__ void __launch_bounds__(256) la_kv_mma_kernel(const bf16* __restrict__ qkv, int pitch, float* __restrict__ part,
                                                         int N, int nchunks, int nblk) {
   PDL_ENTRY();
   extern __shared__ __align__(16) uint8_t lam_sm[];
   bf16* tile = reinterpret_cast<bf16*>(lam_sm);                          // [2][64][LAM_TP]  (k | v)
   bf16* Ps = tile + 2 * LA_PIX * LAM_TP;                                 // [64][LAM_PP]
-  float* m_run = reinterpret_cast<float*>(Ps + LA_PIX * LAM_PP);         // [128]
-  float* s_run = m_run + 128;
-  float* alpha_s = s_run + 128;
-  float* red = alpha_s + 128;                                            // [4][128]
+  float* alpha_s = reinterpret_cast<float*>(Ps + LA_PIX * LAM_PP);       // [128]
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int b = blockIdx.y, blk = blockIdx.x;
-  if (tid < 128) { m_run[tid] = -INFINITY; s_run[tid] = 0.f; }
   const int c0 = (int)(((long long)nchunks * blk) / nblk), c1 = (int)(((long long)nchunks * (blk + 1)) / nblk);
   const int h = warp >> 1, dbase = h * 32 + (warp & 1) * 16;
   float acc[4][4];
@@ -699,33 +583,16 @@ __global__ void __launch_bounds__(256) la_kv_mma_kernel(const bf16* __restrict__
 #pragma unroll
     for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
 
-  auto issue_load = [&](int ch, int buf) {
-    const int n0 = ch * LA_PIX;
-    bf16* dst = tile + buf * LA_PIX * LAM_TP;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const int v = tid + i * 256;      // 2048 16-byte vectors: 32 per pixel
-      const int px = v >> 5, j = v & 31;
-      bf16* d = dst + px * LAM_TP + j * 8;
-      if (n0 + px < N) {
-        const bf16* src = qkv + ((long long)b * N + n0 + px) * pitch + 128 + j * 8;
-        asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(d)), "l"(src));
-      } else {
-        *reinterpret_cast<uint4*>(d) = make_uint4(0, 0, 0, 0);
-      }
-    }
-    asm volatile("cp.async.commit_group;" ::: "memory");
-  };
-  // SHFL loader: the same 8 vectors per thread, but the 64-bit source address and the shared-memory address are set up ONCE
-  // (vector i of a thread is pixel (tid / 32) + 8 i, channel vector tid % 32: a fixed pitch apart), and the k channels
-  // (vector index < 16) of a pixel past the image get -1e30 (bf16 0xF14A) instead of 0: their exp is 0 and the max is
-  // unaffected, so the statistics loops need no per-pixel bounds checks.  v rows past the image are zero as before.
+  // Loader: vector i of a thread is pixel (tid / 32) + 8 i, channel vector tid % 32, a fixed pitch apart, so the 64-bit
+  // source address and the shared-memory address are set up ONCE.  The k channels (vector index < 16) of a pixel past the
+  // image get -1e30 (bf16 0xF14A) instead of 0: their exp is 0 and the max is unaffected, so the statistics loops need no
+  // per-pixel bounds checks.  v rows past the image are zero.
   const int lpx0 = tid >> 5, lj = tid & 31;
   const bf16* const gsrc0 = qkv + ((long long)b * N + lpx0) * pitch + 128 + lj * 8;
   const long long gstep = (long long)8 * pitch;
   const uint32_t sdst0 = (uint32_t)__cvta_generic_to_shared(tile) + (uint32_t)((lpx0 * LAM_TP + lj * 8) * 2);
   const uint32_t kfill = lj < 16 ? 0xF14AF14Au : 0u;
-  auto issue_load_lean = [&](int ch, int buf) {
+  auto issue_load = [&](int ch, int buf) {
     const int n0 = ch * LA_PIX;
     const bf16* src = gsrc0 + (long long)n0 * pitch;
     const uint32_t dst = sdst0 + (uint32_t)(buf * LA_PIX * LAM_TP * 2);
@@ -747,13 +614,9 @@ __global__ void __launch_bounds__(256) la_kv_mma_kernel(const bf16* __restrict__
     asm volatile("cp.async.commit_group;" ::: "memory");
   };
 
-  if (c0 < c1) {
-    if constexpr (SHFL) issue_load_lean(c0, 0);
-    else issue_load(c0, 0);
-  }
-  const int cp2 = (tid & 63) * 2, qtr = tid >> 6;  // stats mapping: 2 channels x 16 pixels per thread
+  if (c0 < c1) issue_load(c0, 0);
   const float LOG2E = 1.4426950408889634f;
-  // SHFL mapping and register-resident running statistics: [0,1] = pair A (lo, hi channel), [2,3] = pair B
+  // statistics mapping and register-resident running statistics: [0,1] = pair A (lo, hi channel), [2,3] = pair B
   const int sq = lane >> 2, pA = warp * 4 + (lane & 3), pB = 32 + pA;
   float mr[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY}, sr[4] = {0.f, 0.f, 0.f, 0.f};
   for (int ch = c0; ch < c1; ++ch) {
@@ -761,102 +624,50 @@ __global__ void __launch_bounds__(256) la_kv_mma_kernel(const bf16* __restrict__
     const bf16* T0 = tile + buf * LA_PIX * LAM_TP;
     asm volatile("cp.async.wait_group 0;" ::: "memory");
     __syncthreads();  // tile[buf] landed; everyone is done with tile[buf^1] and Ps of the previous chunk
-    if (ch + 1 < c1) {
-      if constexpr (SHFL) issue_load_lean(ch + 1, buf ^ 1);
-      else issue_load(ch + 1, buf ^ 1);
+    if (ch + 1 < c1) issue_load(ch + 1, buf ^ 1);
+    // ---- softmax statistics, branch-free: rows past the image hold k = -1e30 (see issue_load); ~13 instructions per bf16 pair
+    float k[16][2];
+    float mx[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const bf16* row = T0 + (i * 8 + sq) * LAM_TP;
+      const __nv_bfloat162 a = *reinterpret_cast<const __nv_bfloat162*>(row + 2 * pA);
+      const __nv_bfloat162 c = *reinterpret_cast<const __nv_bfloat162*>(row + 2 * pB);
+      k[i][0] = __low2float(a); k[i][1] = __high2float(a);
+      k[8 + i][0] = __low2float(c); k[8 + i][1] = __high2float(c);
+      mx[0] = fmaxf(mx[0], k[i][0]); mx[1] = fmaxf(mx[1], k[i][1]);
+      mx[2] = fmaxf(mx[2], k[8 + i][0]); mx[3] = fmaxf(mx[3], k[8 + i][1]);
     }
-    const int nvalid = min(LA_PIX, N - ch * LA_PIX);
-    if constexpr (SHFL) {
-      // branch-free: rows past the image hold k = -1e30 (see issue_load); ~13 instructions per bf16 pair
-      float k[16][2];
-      float mx[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
+    float mn[4], mnl[4], ps[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const bf16* row = T0 + (i * 8 + sq) * LAM_TP;
-        const __nv_bfloat162 a = *reinterpret_cast<const __nv_bfloat162*>(row + 2 * pA);
-        const __nv_bfloat162 c = *reinterpret_cast<const __nv_bfloat162*>(row + 2 * pB);
-        k[i][0] = __low2float(a); k[i][1] = __high2float(a);
-        k[8 + i][0] = __low2float(c); k[8 + i][1] = __high2float(c);
-        mx[0] = fmaxf(mx[0], k[i][0]); mx[1] = fmaxf(mx[1], k[i][1]);
-        mx[2] = fmaxf(mx[2], k[8 + i][0]); mx[3] = fmaxf(mx[3], k[8 + i][1]);
-      }
-      float mn[4], mnl[4], ps[4] = {0.f, 0.f, 0.f, 0.f};
+    for (int c = 0; c < 4; ++c) {
 #pragma unroll
-      for (int c = 0; c < 4; ++c) {
-#pragma unroll
-        for (int o = 4; o < 32; o <<= 1) mx[c] = fmaxf(mx[c], __shfl_xor_sync(0xffffffffu, mx[c], o));
-        mn[c] = fmaxf(mr[c], mx[c]);
-        mnl[c] = mn[c] * LOG2E;
-      }
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        bf16* prow = Ps + (i * 8 + sq) * LAM_PP;
-        const __nv_bfloat162 qa = __floats2bfloat162_rn(ex2_approx(fmaf(k[i][0], LOG2E, -mnl[0])), ex2_approx(fmaf(k[i][1], LOG2E, -mnl[1])));
-        const __nv_bfloat162 qb = __floats2bfloat162_rn(ex2_approx(fmaf(k[8 + i][0], LOG2E, -mnl[2])), ex2_approx(fmaf(k[8 + i][1], LOG2E, -mnl[3])));
-        ps[0] += __low2float(qa);   // sum the rounded values the MMA will actually use
-        ps[1] += __high2float(qa);
-        ps[2] += __low2float(qb);
-        ps[3] += __high2float(qb);
-        *reinterpret_cast<__nv_bfloat162*>(prow + 2 * pA) = qa;
-        *reinterpret_cast<__nv_bfloat162*>(prow + 2 * pB) = qb;
-      }
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-#pragma unroll
-        for (int o = 4; o < 32; o <<= 1) ps[c] += __shfl_xor_sync(0xffffffffu, ps[c], o);
-        const float a = ex2_approx((mr[c] - mn[c]) * LOG2E);  // 0 on the first chunk (mr = -inf)
-        sr[c] = sr[c] * a + ps[c];
-        mr[c] = mn[c];
-        if (sq == 0) alpha_s[2 * (c < 2 ? pA : pB) + (c & 1)] = a;
-      }
-      __syncthreads();  // P and alpha visible to the MMA warps
-    } else {
-    // ---- per-channel max over the chunk
-    float mx0 = -INFINITY, mx1 = -INFINITY;
-#pragma unroll
-    for (int i = 0; i < 16; ++i) {
-      const int px = qtr * 16 + i;
-      if (px < nvalid) {
-        __nv_bfloat162 kk = *reinterpret_cast<const __nv_bfloat162*>(T0 + px * LAM_TP + cp2);
-        mx0 = fmaxf(mx0, __low2float(kk));
-        mx1 = fmaxf(mx1, __high2float(kk));
-      }
+      for (int o = 4; o < 32; o <<= 1) mx[c] = fmaxf(mx[c], __shfl_xor_sync(0xffffffffu, mx[c], o));
+      mn[c] = fmaxf(mr[c], mx[c]);
+      mnl[c] = mn[c] * LOG2E;
     }
-    red[qtr * 128 + cp2] = mx0;
-    red[qtr * 128 + cp2 + 1] = mx1;
-    __syncthreads();
-    const float mo0 = m_run[cp2], mo1 = m_run[cp2 + 1];
-    float mn0 = mo0, mn1 = mo1;
 #pragma unroll
-    for (int q = 0; q < 4; ++q) { mn0 = fmaxf(mn0, red[q * 128 + cp2]); mn1 = fmaxf(mn1, red[q * 128 + cp2 + 1]); }
-    float ps0 = 0.f, ps1 = 0.f;
+    for (int i = 0; i < 8; ++i) {
+      bf16* prow = Ps + (i * 8 + sq) * LAM_PP;
+      const __nv_bfloat162 qa = __floats2bfloat162_rn(ex2_approx(fmaf(k[i][0], LOG2E, -mnl[0])), ex2_approx(fmaf(k[i][1], LOG2E, -mnl[1])));
+      const __nv_bfloat162 qb = __floats2bfloat162_rn(ex2_approx(fmaf(k[8 + i][0], LOG2E, -mnl[2])), ex2_approx(fmaf(k[8 + i][1], LOG2E, -mnl[3])));
+      ps[0] += __low2float(qa);   // sum the rounded values the MMA will actually use
+      ps[1] += __high2float(qa);
+      ps[2] += __low2float(qb);
+      ps[3] += __high2float(qb);
+      *reinterpret_cast<__nv_bfloat162*>(prow + 2 * pA) = qa;
+      *reinterpret_cast<__nv_bfloat162*>(prow + 2 * pB) = qb;
+    }
 #pragma unroll
-    for (int i = 0; i < 16; ++i) {
-      const int px = qtr * 16 + i;
-      __nv_bfloat162 pp = __floats2bfloat162_rn(0.f, 0.f);
-      if (px < nvalid) {
-        __nv_bfloat162 kk = *reinterpret_cast<const __nv_bfloat162*>(T0 + px * LAM_TP + cp2);
-        pp = __floats2bfloat162_rn(exp2f((__low2float(kk) - mn0) * LOG2E), exp2f((__high2float(kk) - mn1) * LOG2E));
-        ps0 += __low2float(pp);   // sum the rounded values the MMA will actually use
-        ps1 += __high2float(pp);
-      }
-      *reinterpret_cast<__nv_bfloat162*>(Ps + px * LAM_PP + cp2) = pp;
+    for (int c = 0; c < 4; ++c) {
+#pragma unroll
+      for (int o = 4; o < 32; o <<= 1) ps[c] += __shfl_xor_sync(0xffffffffu, ps[c], o);
+      const float a = ex2_approx((mr[c] - mn[c]) * LOG2E);  // 0 on the first chunk (mr = -inf)
+      sr[c] = sr[c] * a + ps[c];
+      mr[c] = mn[c];
+      if (sq == 0) alpha_s[2 * (c < 2 ? pA : pB) + (c & 1)] = a;
     }
-    __syncthreads();  // all reads of red (max) done
-    red[qtr * 128 + cp2] = ps0;
-    red[qtr * 128 + cp2 + 1] = ps1;
-    __syncthreads();
-    if (qtr == 0) {
-      const float a0 = exp2f((mo0 - mn0) * LOG2E), a1 = exp2f((mo1 - mn1) * LOG2E);  // 0 on the first chunk
-      alpha_s[cp2] = a0;
-      alpha_s[cp2 + 1] = a1;
-      s_run[cp2] = s_run[cp2] * a0 + red[cp2] + red[128 + cp2] + red[256 + cp2] + red[384 + cp2];
-      s_run[cp2 + 1] = s_run[cp2 + 1] * a1 + red[cp2 + 1] + red[128 + cp2 + 1] + red[256 + cp2 + 1] + red[384 + cp2 + 1];
-      m_run[cp2] = mn0;
-      m_run[cp2 + 1] = mn1;
-    }
-    __syncthreads();
-    }  // !SHFL
+    __syncthreads();  // P and alpha visible to the MMA warps
     // ---- rescale and accumulate: rows g / g+8 of this warp's 16 d-rows
     {
       const float al_lo = alpha_s[dbase + (lane >> 2)], al_hi = alpha_s[dbase + (lane >> 2) + 8];
@@ -885,19 +696,13 @@ __global__ void __launch_bounds__(256) la_kv_mma_kernel(const bf16* __restrict__
   }
   __syncthreads();
   float* rec = part + ((long long)b * LA_MAXBLK + blk) * LA_REC;
-  if constexpr (SHFL) {
-    if (sq == 0) {
+  if (sq == 0) {
 #pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        const int chn = 2 * (c < 2 ? pA : pB) + (c & 1);
-        rec[(chn >> 5) * 1088 + (chn & 31)] = mr[c];
-        rec[(chn >> 5) * 1088 + 32 + (chn & 31)] = sr[c];
-      }
+    for (int c = 0; c < 4; ++c) {
+      const int chn = 2 * (c < 2 ? pA : pB) + (c & 1);
+      rec[(chn >> 5) * 1088 + (chn & 31)] = mr[c];
+      rec[(chn >> 5) * 1088 + 32 + (chn & 31)] = sr[c];
     }
-  } else if (tid < 128) {
-    const int hh = tid >> 5, dd = tid & 31;
-    rec[hh * 1088 + dd] = m_run[tid];
-    rec[hh * 1088 + 32 + dd] = s_run[tid];
   }
   {
     const int g = lane >> 2, t4 = lane & 3, drow = (warp & 1) * 16 + g;
@@ -925,8 +730,7 @@ template <>
 void launch_la_kv<bf16>(const bf16* qkv, int qkv_pitch, float* partial, int B, int N, int nchunks, int nblk, size_t smem,
                         cudaStream_t st) {
   if (qkv_pitch % 8 == 0 && ((uintptr_t)qkv % 16) == 0)
-    if (g_hbm_new & 8) pdl_launch(la_kv_mma_kernel<true>, dim3(nblk, B), 256, LAM_SMEM, st, qkv, qkv_pitch, partial, N, nchunks, nblk);
-    else pdl_launch(la_kv_mma_kernel<false>, dim3(nblk, B), 256, LAM_SMEM, st, qkv, qkv_pitch, partial, N, nchunks, nblk);
+    pdl_launch(la_kv_mma_kernel, dim3(nblk, B), 256, LAM_SMEM, st, qkv, qkv_pitch, partial, N, nchunks, nblk);
   else
     pdl_launch(la_kv_kernel<bf16>, dim3(nblk, B), 256, smem, st, qkv, qkv_pitch, partial, N, nchunks, nblk);
 }
@@ -939,14 +743,11 @@ void launch_linattn_ctx(const T* qkv, int qkv_pitch, float* partial, float* ctx,
   if (!g_la_attr_done) {
     cudaFuncSetAttribute(la_kv_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     cudaFuncSetAttribute(la_kv_kernel<bf16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    cudaFuncSetAttribute(la_kv_mma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LAM_SMEM);
-    cudaFuncSetAttribute(la_kv_mma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LAM_SMEM);
+    cudaFuncSetAttribute(la_kv_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LAM_SMEM);
     g_la_attr_done = true;
   }
   launch_la_kv<T>(qkv, qkv_pitch, partial, B, N, nchunks, nblk, smem, st);
-  if (g_hbm_new & 16) pdl_launch(la_combine8_kernel, B * 4 * 8, 256, 0, st, partial, ctx, N, nblk);
-  else if (g_hbm_new & 2) pdl_launch(la_combine4_kernel, B * 4 * 8, 32, 0, st, partial, ctx, N, nblk);
-  else pdl_launch(la_combine_kernel, B * 4 * 4, 256, 0, st, partial, ctx, N, nblk);
+  pdl_launch(la_combine8_kernel, B * 4 * 8, 256, 0, st, partial, ctx, N, nblk);
 }
 template void launch_linattn_ctx<float>(const float*, int, float*, float*, int, int, cudaStream_t);
 template void launch_linattn_ctx<bf16>(const bf16*, int, float*, float*, int, int, cudaStream_t);
@@ -963,25 +764,9 @@ template void launch_linattn<bf16>(const bf16*, int, float*, float*, bf16*, int,
 // Fold the per-image context into the to_out 1x1 weights so that pass C and the to_out conv become ONE
 // per-image-weight GEMM on the (head-softmaxed) q:  y[px][c] = sum_k qs[px][k] * Mb[b][c][k],
 // Mb[b][c][h*32+d] = sum_e Wout[c][h*32+e] * ctx[b][h][d][e]   (module_util.py:176-178 re-associated).
-__global__ void la_fold_kernel(const float* __restrict__ ctx, const float* __restrict__ wout, bf16* __restrict__ Mb, int C) {
-  PDL_ENTRY();
-  __shared__ float cs[4][32][33];
-  const int b = blockIdx.y;
-  for (int i = threadIdx.x; i < 4096; i += blockDim.x) cs[i >> 10][(i >> 5) & 31][i & 31] = ctx[(long long)b * 4096 + i];
-  __syncthreads();
-  const int c = blockIdx.x * 2 + (threadIdx.x >> 7), k = threadIdx.x & 127;
-  if (c >= C) return;
-  const int h = k >> 5, d = k & 31;
-  const float* w = wout + (long long)c * 128 + h * 32;
-  float acc = 0.f;
-#pragma unroll
-  for (int e = 0; e < 32; ++e) acc += w[e] * cs[h][d][e];
-  Mb[((long long)b * C + c) * 128 + k] = __float2bfloat16_rn(acc);
-}
-// 16-row fold: la_fold_kernel stages the image's whole 16 KB context in shared memory for TWO output rows (2 048 blocks x
-// 16 KB of L2 reads at C = 512).  Here a block owns 16 output rows: a thread keeps ITS context row (h, d, 0..31) in
-// registers (eight 128-bit loads, no staging), the 16 weight rows go through shared memory once, and all loads of the block
-// are one round trip.  Same per-entry sum order as above (bit-identical Mb).
+// A block owns 16 output rows: a thread keeps ITS context row (h, d, 0..31) in registers (eight 128-bit loads, no
+// staging), the 16 weight rows go through shared memory once, and all loads of the block are one round trip.  Each entry
+// is one sum over e = 0..31 in ascending order, whatever the block shape.
 __global__ void __launch_bounds__(256) la_fold16_kernel(const float* __restrict__ ctx, const float* __restrict__ wout,
                                                         bf16* __restrict__ Mb, int C) {
   PDL_ENTRY();
@@ -1014,8 +799,7 @@ __global__ void __launch_bounds__(256) la_fold16_kernel(const float* __restrict_
   }
 }
 void launch_la_fold(const float* ctx, const float* wout, bf16* Mb, int B, int C, cudaStream_t st) {
-  if (g_hbm_new & 4) pdl_launch(la_fold16_kernel, dim3((C + 15) / 16, B), 256, 0, st, ctx, wout, Mb, C);
-  else pdl_launch(la_fold_kernel, dim3((C + 1) / 2, B), 256, 0, st, ctx, wout, Mb, C);
+  pdl_launch(la_fold16_kernel, dim3((C + 15) / 16, B), 256, 0, st, ctx, wout, Mb, C);
 }
 
 // =============================================================================================
@@ -1259,8 +1043,7 @@ void launch_fullattn(const T* qkv, int qkv_pitch, T* hidden, int hid_pitch, int 
 }
 template <>
 void launch_fullattn<bf16>(const bf16* qkv, int qkv_pitch, bf16* hidden, int hid_pitch, int B, int N, cudaStream_t st) {
-  static const bool force_scalar = getenv("IRSDE_FULLATTN_SCALAR") && getenv("IRSDE_FULLATTN_SCALAR")[0] == '1';
-  if (!force_scalar && qkv_pitch % 8 == 0 && hid_pitch % 2 == 0 && ((uintptr_t)qkv % 16) == 0 && ((uintptr_t)hidden % 4) == 0)
+  if (qkv_pitch % 8 == 0 && hid_pitch % 2 == 0 && ((uintptr_t)qkv % 16) == 0 && ((uintptr_t)hidden % 4) == 0)
     pdl_launch(fullattn_mma_kernel, dim3((N + FA_Q - 1) / FA_Q, B * 4), 128, 0, st, qkv, qkv_pitch, hidden, hid_pitch, N);
   else
     pdl_launch(fullattn_kernel<bf16>, dim3((N + 127) / 128, B * 4), 128, 0, st, qkv, qkv_pitch, hidden, hid_pitch, N);

@@ -193,7 +193,6 @@ TcConvDesc* tc_conv_create_f32x3(const float* in_split /*[2][planes][B][H][W][Ci
                                  int nphases, const Epilogue& ep, float* out, int out_pitch, int Hout, int Wout, std::string* err);
 // hi = rn_tf32(x), lo = rn_tf32(x - hi) of a pitched NHWC fp32 view -> dense out[0][npix][C] (hi), out[1][npix][C] (lo)
 void launch_split_tf32(const float* in, int in_pitch, float* out, long long npix, int C, cudaStream_t st);
-bool tc_fused_attention_available();
 void tc_conv_destroy(TcConvDesc*);
 void tc_conv_set_runtime(TcConvDesc*, const float* ss, const int* t_ptr, int ss_img_stride);
 void tc_conv_set_out_nchw(TcConvDesc*, float* out, int cropH, int cropW);  // out==nullptr at create => fp32 NCHW output

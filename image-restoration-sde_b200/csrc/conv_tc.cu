@@ -51,7 +51,6 @@ struct TcParams {
   int out_pitch;
   float* out_nchw;      // if set: write fp32 NCHW cropped to (cropH, cropW) instead of the NHWC view
   int cropH, cropW;
-  int tma_store;        // persistent kernel: bf16 NHWC output through smem + TMA bulk store
   int qsm;              // LinearAttention q: softmax over each 32-channel head * 32^-0.5 for output channels < 128
   int w_per_image;      // weights tensor is [B][Cout][Cin]: third TMA coordinate = image index
   float* out_f32;       // MODE 3 (fp32x3): fp32 NHWC output view (channel offset applied), pitch = out_pitch
@@ -239,14 +238,14 @@ struct TcCfgP {
   static constexpr bool COMPACT = (BN == 256 && MODE == 0) || (BN == 128 && MODE == 2);
   static constexpr int ACC_COLS = COMPACT ? 32 : 64;      // fp32 columns staged per pass
   static constexpr int ACC_PITCH = ACC_COLS + 4;          // + 4: conflict-free 16-byte row reads
-  // Epilogue staging for the TMA stores: one 2 KB tile per consumer warp (STG_BUFS = 2 alternates two tiles per warp;
-  // 0: no TMA store (fp32x3) or the tile is inside the fp32 staging rows (COMPACT)).
+  // Epilogue staging for the TMA stores: STG_BUFS = 1 is one 2 KB tile per consumer warp; 0: no TMA store (fp32x3) or the
+  // tile is inside the fp32 staging rows (COMPACT).
   static constexpr int STG_BUFS = (TF3 || COMPACT) ? 0 : 1;
   static constexpr int BSUB = ROWS ? 3 : (TF3 ? 2 : 1);  // weight tiles per stage
   static constexpr int A_SLOT = TF3 ? 2 * A_STAGE_BYTES : (ROWS ? ROWS_A_SLOT : A_STAGE_BYTES);
   static constexpr int STAGE_BYTES = A_SLOT + BSUB * B_STAGE_BYTES;
   static constexpr int EPI_FLOATS = 2 * BN;
-  static constexpr int STG_BYTES = STG_BUFS * 8 * 2048;  // per consumer warp: STG_BUFS 32 rows x 64 B staging tiles
+  static constexpr int STG_BYTES = STG_BUFS * 8 * 2048;  // per consumer warp: a 32 rows x 64 B staging tile
   static constexpr int ACC_WG_BYTES = 64 * ACC_PITCH * 4;  // fp32 staging of one warpgroup: 64 rows x ACC_COLS columns
   static constexpr int ACC_BYTES = 2 * ACC_WG_BYTES;
   static constexpr int FIXED_BYTES = 1024 + STG_BYTES + ACC_BYTES + EPI_FLOATS * 4 + 256;
@@ -288,7 +287,6 @@ __device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, const void*
 }
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_read1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 struct TileCoord {
@@ -446,11 +444,9 @@ __global__ void __launch_bounds__(288, 1) conv_tc_persist_kernel(const __grid_co
   const bool affine = (P.ss != nullptr) || (P.bias != nullptr) || (P.mult_vec != nullptr);
   constexpr int ACC_PITCH = Cfg::ACC_PITCH;
   float* const acc_stg = s_acc + wg * 64 * ACC_PITCH;
-  uint8_t* const stg_base = Cfg::COMPACT ? reinterpret_cast<uint8_t*>(acc_stg) + wq * 2048
-                                         : smem_stg + warp * 2048 * (Cfg::STG_BUFS > 0 ? Cfg::STG_BUFS : 1);
+  uint8_t* const stg = Cfg::COMPACT ? reinterpret_cast<uint8_t*>(acc_stg) + wq * 2048 : smem_stg + warp * 2048;
   const uint32_t a_off = (uint32_t)(wg * 64 * 128);  // this warpgroup's 64 pixel rows inside every A box
   const bool signaller = (threadIdx.x & 127) == 0;
-  int stg_i = 0;  // staging tile used by the next bulk store (alternates when STG_BUFS == 2)
   long long w_full = 0, t_start = clock64();
   int it = 0, lt = 0, epi_n0 = -1, epi_b = -1;
   for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++lt) {
@@ -563,11 +559,10 @@ __global__ void __launch_bounds__(288, 1) conv_tc_persist_kernel(const __grid_co
     const int hh = t.h0 + (m >> P.logBW), ww = t.w0 + (m & (P.BW - 1));
     const bool pvalid = hh < P.H && ww < P.W;
     const long long opix = ((long long)t.b * P.Hout + (hh * P.os + t.py)) * P.Wout + (ww * P.os + t.px);
-    bf16* orow = P.out + opix * P.out_pitch + t.n0;
     const bf16* rrow = P.res ? P.res + opix * P.res_pitch + t.n0 : nullptr;
       // KC: std::integral_constant<int, KIND>.  KIND = the EK_* features this conv has, fixed per launch: feature blocks
       // outside KIND do not exist in the instantiation (the compiler had turned several of them into predicated code that
-      // was issued for every chunk), EK_GENERIC keeps every run-time check (fp32 NCHW output, no-TMA-store fallback).
+      // was issued for every chunk), EK_GENERIC keeps every run-time check and the fp32 NCHW output.
       auto process = [&](auto KC, uint32_t* v, const int c0) __attribute__((always_inline)) {
         constexpr int KIND = decltype(KC)::value;
         constexpr bool GEN = KIND == EK_GENERIC;
@@ -670,30 +665,20 @@ __global__ void __launch_bounds__(288, 1) conv_tc_persist_kernel(const __grid_co
 #pragma unroll
           for (int j = 0; j < 4; ++j) o2[j] = __floats2bfloat162_rn(f[2 * j], f[2 * j + 1]);
         }
-        if (!GEN || P.tma_store) {
-          // bf16 NHWC through shared memory + TMA store: each lane owns one pixel row of 32 channels (64 B); the
-          // staging tile uses the 64B swizzle so the 16-byte st.shared are conflict free and the bulk store writes
-          // full, coalesced lines (out-of-range pixels / channels are clipped by TMA).
-          uint8_t* stg = stg_base + stg_i * 2048;
-          if (lane == 0) {  // the bulk store that last used THIS tile has finished reading it
-            if constexpr (Cfg::STG_BUFS == 2) bulk_wait_read1(); else bulk_wait_read0();
-          }
-          if constexpr (Cfg::STG_BUFS == 2) stg_i ^= 1;
-          __syncwarp();
+        // bf16 NHWC through shared memory + TMA store: each lane owns one pixel row of 32 channels (64 B); the
+        // staging tile uses the 64B swizzle so the 16-byte st.shared are conflict free and the bulk store writes
+        // full, coalesced lines (out-of-range pixels / channels are clipped by TMA).
+        if (lane == 0) bulk_wait_read0();  // the bulk store that last used the tile has finished reading it
+        __syncwarp();
 #pragma unroll
-          for (int g = 0; g < 4; ++g)
-            *reinterpret_cast<uint4*>(stg + lane * 64 + ((g ^ ((lane >> 1) & 3)) << 4)) = ov[g];
-          fence_proxy_async();
-          __syncwarp();
-          if (lane == 0) {
-            const int m0 = quad * 32;
-            tma_store_4d(&map_o.m[t.phase], stg, t.n0 + c0, t.w0 + (m0 & (P.BW - 1)), t.h0 + (m0 >> P.logBW), t.b);
-            bulk_commit();
-          }
-        } else if (pvalid) {
-#pragma unroll
-          for (int g = 0; g < 4; ++g)
-            if (t.n0 + c0 + g * 8 < P.Cout) *reinterpret_cast<uint4*>(orow + c0 + g * 8) = ov[g];
+        for (int g = 0; g < 4; ++g)
+          *reinterpret_cast<uint4*>(stg + lane * 64 + ((g ^ ((lane >> 1) & 3)) << 4)) = ov[g];
+        fence_proxy_async();
+        __syncwarp();
+        if (lane == 0) {
+          const int m0 = quad * 32;
+          tma_store_4d(&map_o.m[t.phase], stg, t.n0 + c0, t.w0 + (m0 & (P.BW - 1)), t.h0 + (m0 >> P.logBW), t.b);
+          bulk_commit();
         }
       };
 
@@ -776,10 +761,6 @@ __global__ void __launch_bounds__(288, 1) conv_tc_persist_kernel(const __grid_co
 }
 
 int g_num_sms = 132;
-bool g_tma_store = true;
-bool g_rows = true;
-int g_epi_spec = 3;  // specialised epilogues: 1 = the per-tap 1x1 layers, 2 = + the ROWS 3x3 ResBlock convs, 3 = + the BN = 256
-                     // biased / plain per-tap convs; IRSDE_TC_EPI_SPEC=0: generic only
 
 }  // namespace
 
@@ -833,13 +814,7 @@ bool tc_init(std::string* err) {
     int dev = 0, n = 0;
     cudaGetDevice(&dev);
     if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0) g_num_sms = n;
-    const char* e = getenv("IRSDE_TC_TMA_STORE");
-    g_tma_store = !(e && e[0] == '0');
-    e = getenv("IRSDE_TC_ROWS");
-    g_rows = !(e && e[0] == '0');
-    e = getenv("IRSDE_TC_EPI_SPEC");
-    if (e && e[0] >= '0' && e[0] <= '3') g_epi_spec = e[0] - '0';
-    e = getenv("IRSDE_PDL");
+    const char* e = getenv("IRSDE_PDL");
     g_pdl = (e && e[0] == '1');  // opt-in (see common.cuh)
   }
   cudaError_t le = cudaGetLastError();
@@ -872,7 +847,7 @@ static void tc_fill_magic(TcConvDesc* d) {
   if (P.res) k |= EK_RES;
   const bool known = k == 0 || k == EK_QSM || k == EK_AFF || k == EK_SILU || k == (EK_AFF | EK_SILU) || k == (EK_AFF | EK_RES) ||
                      k == (EK_SILU | EK_RES);
-  P.epi_kind = (d->mode != 3 && P.tma_store && P.out && known) ? k : EK_GENERIC;
+  P.epi_kind = (d->mode != 3 && P.out && known) ? k : EK_GENERIC;
 }
 
 TcConvDesc* tc_conv_create(const bf16* in, int in_pitch, int B, int Hin, int Win, int Cin, int planes,
@@ -906,11 +881,10 @@ TcConvDesc* tc_conv_create(const bf16* in, int in_pitch, int B, int Hin, int Win
   P.qsm = (flags & TC_FLAG_QSOFTMAX) ? 1 : 0;
   P.w_per_image = (flags & TC_FLAG_W_PER_IMAGE) ? 1 : 0;
   if (P.w_per_image && (ntaps != 1 || nphases != 1)) return bad("per-image weights need a 1x1 conv");
-  if ((P.qsm || P.w_per_image) && !g_tma_store) return bad("fused attention epilogues need the TMA-store epilogue");
   int BN = Cout >= 256 ? 256 : (Cout > 64 ? 128 : (Cout > 32 ? 64 : 32));
   if (BN == 256 && Cout % 256 != 0 && Cout % 128 == 0) BN = 128;  // e.g. to_qkv (384): no half-empty N tile
   bool rows = false;
-  if (g_rows && nphases == 1 && planes == 1 && ntaps == 9 && BN <= 128) {
+  if (nphases == 1 && planes == 1 && ntaps == 9 && BN <= 128) {
     rows = true;
     for (int i = 0; rows && i < 9; ++i) rows = taps[i].dh == i / 3 - 1 && taps[i].dw == i % 3 - 1 && taps[i].plane == 0;
   }
@@ -993,11 +967,9 @@ TcConvDesc* tc_conv_create(const bf16* in, int in_pitch, int B, int Hin, int Win
   // output maps for the TMA-store epilogue: [B][H][W][C] view of the destination (channel offset already in
   // `out`), pixel stride os*pitch; one map per upsample phase (base shifted by (py,px))
   memset(&d->map_o, 0, sizeof d->map_o);
-  P.tma_store = 0;
-  if (!nchw_out && g_tma_store) {
+  if (!nchw_out) {
     const int bw = P.BW < 32 ? P.BW : 32, bh = 32 / bw;
-    bool ok = true;
-    for (int ph = 0; ph < nphases && ok; ++ph) {
+    for (int ph = 0; ph < nphases; ++ph) {
       const int py = ph >> 1, px = ph & 1;
       bf16* base = out + ((long long)py * Wout + px) * out_pitch;
       cuuint64_t dims[4] = {(cuuint64_t)Cout, (cuuint64_t)Win, (cuuint64_t)Hin, (cuuint64_t)B};
@@ -1008,9 +980,12 @@ TcConvDesc* tc_conv_create(const bf16* in, int in_pitch, int B, int Hin, int Win
       CUresult r = g_encode(&d->map_o.m[ph], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, (void*)base, dims, strides, box, es,
                             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
                             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      ok = (r == CUDA_SUCCESS);
+      if (r != CUDA_SUCCESS) {
+        delete d;
+        if (err) { char b[96]; snprintf(b, sizeof b, "cuTensorMapEncodeTiled(out) failed: %d", (int)r); *err = b; }
+        return nullptr;
+      }
     }
-    P.tma_store = ok ? 1 : 0;
   }
   tc_fill_magic(d);
   return d;
@@ -1100,14 +1075,11 @@ TcConvDesc* tc_conv_create_f32x3(const float* in_split, int B, int Hin, int Win,
     }
   }
   memset(&d->map_o, 0, sizeof d->map_o);
-  P.tma_store = 0;
   tc_fill_magic(d);
   return d;
 }
 
 void tc_conv_destroy(TcConvDesc* d) { delete d; }
-
-bool tc_fused_attention_available() { return g_tma_store; }
 
 void tc_conv_set_out_nchw(TcConvDesc* d, float* out, int cropH, int cropW) {
   d->P.out_nchw = out;
@@ -1126,19 +1098,16 @@ void tc_conv_set_runtime(TcConvDesc* d, const float* ss, const int* t_ptr, int s
 }
 
 // EKT of the conv_tc_persist_kernel instantiation that runs this descriptor: its epilogue kind where an instantiation is
-// specialised for it (and the IRSDE_TC_EPI_SPEC level enables that class), EK_GENERIC otherwise.  tc_conv_launch and
-// tc_conv_query both read it, so what the query reports is what runs.
+// specialised for it, EK_GENERIC otherwise.  tc_conv_launch and tc_conv_query both read it, so what the query reports is
+// what runs.
 static int tc_launch_ekt(const TcConvDesc* d) {
   if (d->mode == 3) return EK_GENERIC;
-  if (d->mode == 2) {
-    const int ek = g_epi_spec >= 2 ? d->P.epi_kind : EK_GENERIC;
-    return d->BN != 32 && (ek == (EK_AFF | EK_SILU) || ek == (EK_SILU | EK_RES)) ? ek : EK_GENERIC;
-  }
-  const int ek = g_epi_spec >= 1 ? d->P.epi_kind : EK_GENERIC;
+  const int ek = d->P.epi_kind;
+  if (d->mode == 2) return d->BN != 32 && (ek == (EK_AFF | EK_SILU) || ek == (EK_SILU | EK_RES)) ? ek : EK_GENERIC;
   switch (d->BN) {
     case 64: return ek == 0 || ek == EK_AFF ? ek : EK_GENERIC;
     case 128: return ek == 0 || ek == EK_AFF || ek == EK_QSM ? ek : EK_GENERIC;
-    case 256: return g_epi_spec >= 3 && (ek == 0 || ek == EK_AFF) ? ek : EK_GENERIC;  // deep res_conv; downsample / to_out (bias)
+    case 256: return ek == 0 || ek == EK_AFF ? ek : EK_GENERIC;  // deep res_conv; downsample / to_out (bias)
     default: return EK_GENERIC;
   }
 }

@@ -757,7 +757,7 @@ struct Builder {
     mark_out(V{xn, C, C}, H, W);
     T* qkv = tmp(npix * 384);
     if constexpr (std::is_same<T, bf16>::value) {
-      if (!full && ctx->use_tc && tc_fused_attention_available() && C % 8 == 0) {
+      if (!full && ctx->use_tc && C % 8 == 0) {
         // Fused LinearAttention: (1) the to_qkv GEMM epilogue applies softmax_d(q)*32^-.5 per head, (2) k,v -> ctx,
         // (3) ctx is folded into the to_out weights per image, (4) ONE per-image-weight 1x1 GEMM on q gives to_out's
         // output (module_util.py:163-178 with the two einsums + to_out conv re-associated), (5) LayerNorm + residual.
