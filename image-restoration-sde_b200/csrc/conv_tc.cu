@@ -992,7 +992,7 @@ TcConvDesc* tc_conv_create(const bf16* in, int in_pitch, int B, int Hin, int Win
 }
 
 // fp32x3 mode: `in_split` is the conv input split by launch_split_tf32: [2 (hi, lo)][planes][B][Hin][Win][Cin] fp32 (dense,
-// pixel pitch Cin); `wsplit` is [phase*ntaps][2 (hi, lo)][Cout_w][Cin] fp32 (pack_tc3_* kernels); fp32 NHWC output view.
+// pixel pitch Cin); `wsplit` is [phase*ntaps][2 (hi, lo)][Cout_w][Cin] fp32 (pack_tc_*_kernel<float>); fp32 NHWC output view.
 TcConvDesc* tc_conv_create_f32x3(const float* in_split, int B, int Hin, int Win, int Cin, int planes, const float* wsplit, int Cout,
                                  int ntaps, const TcTap* taps, int nphases, const Epilogue& ep, float* out, int out_pitch, int Hout,
                                  int Wout, std::string* err) {

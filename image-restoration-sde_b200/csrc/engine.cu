@@ -175,40 +175,6 @@ __global__ void pack_simt_kernel(const float* __restrict__ w, float* __restrict_
   int r = tap / KW, s = tap % KW;
   o[idx] = w[(((long long)co * Cin + c) * KH + r) * KW + s];
 }
-// [tap][Cout][Cin] bf16
-__global__ void pack_tc_kernel(const float* __restrict__ w, bf16* __restrict__ o, int Cout, int Cin, int KH, int KW) {
-  long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  long long total = (long long)Cout * Cin * KH * KW;
-  if (idx >= total) return;
-  int c = idx % Cin;
-  int co = (idx / Cin) % Cout;
-  int tap = idx / ((long long)Cout * Cin);
-  int r = tap / KW, s = tap % KW;
-  o[idx] = __float2bfloat16_rn(w[(((long long)co * Cin + c) * KH + r) * KW + s]);
-}
-// nearest-x2 upsample followed by 3x3/pad1 == four 2x2 phase convolutions on the low-res input with
-// pre-summed weights: [phase=(py,px)][tap=(a,b)][Cout][Cin]
-__global__ void pack_tc_up_kernel(const float* __restrict__ w, bf16* __restrict__ o, int Cout, int Cin) {
-  long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  long long total = (long long)16 * Cout * Cin;
-  if (idx >= total) return;
-  int c = idx % Cin;
-  int co = (idx / Cin) % Cout;
-  int tap = (idx / ((long long)Cout * Cin)) % 4;
-  int phase = idx / ((long long)4 * Cout * Cin);
-  int py = phase >> 1, px = phase & 1, a = tap >> 1, b = tap & 1;
-  // rows of the 3x3 kernel that fall on low-res offset a for phase py
-  int r0, r1, s0, s1;
-  if (py == 0) { if (a == 0) { r0 = 0; r1 = 0; } else { r0 = 1; r1 = 2; } }
-  else         { if (a == 0) { r0 = 0; r1 = 1; } else { r0 = 2; r1 = 2; } }
-  if (px == 0) { if (b == 0) { s0 = 0; s1 = 0; } else { s0 = 1; s1 = 2; } }
-  else         { if (b == 0) { s0 = 0; s1 = 1; } else { s0 = 2; s1 = 2; } }
-  float acc = 0.f;
-  for (int r = r0; r <= r1; ++r)
-    for (int s = s0; s <= s1; ++s) acc += w[(((long long)co * Cin + c) * 3 + r) * 3 + s];
-  o[idx] = __float2bfloat16_rn(acc);
-}
-
 // 7x7 stem as 7 row-taps with K=64 = 8 pixels x 8 channels (see conv_tc.cu): [r][Cout][s*8+c]
 __global__ void pack_tc_stem_kernel(const float* __restrict__ w, bf16* __restrict__ o, int Cout, int Cin) {
   long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -221,26 +187,26 @@ __global__ void pack_tc_stem_kernel(const float* __restrict__ w, bf16* __restric
   float v = (s < 7 && c < Cin) ? w[(((long long)co * Cin + c) * 7 + r) * 7 + s] : 0.f;
   o[idx] = __float2bfloat16_rn(v);
 }
-// [tap][Cout_pad][Cin] with zero rows for co >= Cout (head conv, Cout=3)
-__global__ void pack_tc_padded_kernel(const float* __restrict__ w, bf16* __restrict__ o, int Cout, int Cout_pad, int Cin,
-                                      int KH, int KW) {
-  long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  long long total = (long long)Cout_pad * Cin * KH * KW;
-  if (idx >= total) return;
-  int c = idx % Cin;
-  int co = (idx / Cin) % Cout_pad;
-  int tap = idx / ((long long)Cout_pad * Cin);
-  int r = tap / KW, s = tap % KW;
-  o[idx] = __float2bfloat16_rn(co < Cout ? w[(((long long)co * Cin + c) * KH + r) * KW + s] : 0.f);
-}
 
-// fp32x3 weights: [tap][2 (hi, lo)][Cout_pad][Cin] fp32, hi = rn_tf32(w), lo = rn_tf32(w - hi) (zero rows for co >= Cout)
+// Tap-GEMM weight element (tap, co, c) of a [tap][Cout_pad][Cin] layout.  bf16: one value.  fp32x3: [tap][2 (hi, lo)]
+// [Cout_pad][Cin] fp32, hi = rn_tf32(w), lo = rn_tf32(w - hi).
 __device__ __forceinline__ float rn_tf32_w(float x) {
   uint32_t u;
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x));
   return __uint_as_float(u);
 }
-__global__ void pack_tc3_kernel(const float* __restrict__ w, float* __restrict__ o, int Cout, int Cout_pad, int Cin, int KH, int KW) {
+__device__ __forceinline__ void store_tc_w(bf16* o, int tap, int co, int c, int Cout_pad, int Cin, float v) {
+  o[((long long)tap * Cout_pad + co) * Cin + c] = __float2bfloat16_rn(v);
+}
+__device__ __forceinline__ void store_tc_w(float* o, int tap, int co, int c, int Cout_pad, int Cin, float v) {
+  const float hi = rn_tf32_w(v);
+  const long long base = ((long long)tap * 2 * Cout_pad + co) * Cin + c;
+  o[base] = hi;
+  o[base + (long long)Cout_pad * Cin] = rn_tf32_w(v - hi);
+}
+// [tap][Cout_pad][Cin] with zero rows for co >= Cout (head conv, Cout=3)
+template <typename S>
+__global__ void pack_tc_taps_kernel(const float* __restrict__ w, S* __restrict__ o, int Cout, int Cout_pad, int Cin, int KH, int KW) {
   long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   long long total = (long long)Cout_pad * Cin * KH * KW;
   if (idx >= total) return;
@@ -248,14 +214,12 @@ __global__ void pack_tc3_kernel(const float* __restrict__ w, float* __restrict__
   int co = (idx / Cin) % Cout_pad;
   int tap = idx / ((long long)Cout_pad * Cin);
   int r = tap / KW, s = tap % KW;
-  float v = co < Cout ? w[(((long long)co * Cin + c) * KH + r) * KW + s] : 0.f;
-  float hi = rn_tf32_w(v);
-  long long base = ((long long)tap * 2 * Cout_pad + co) * Cin + c;
-  o[base] = hi;
-  o[base + (long long)Cout_pad * Cin] = rn_tf32_w(v - hi);
+  store_tc_w(o, tap, co, c, Cout_pad, Cin, co < Cout ? w[(((long long)co * Cin + c) * KH + r) * KW + s] : 0.f);
 }
-// nearest-x2 + 3x3 as four 2x2 phase convolutions (see pack_tc_up_kernel): [phase][tap][2][Cout_pad][Cin]
-__global__ void pack_tc3_up_kernel(const float* __restrict__ w, float* __restrict__ o, int Cout, int Cout_pad, int Cin) {
+// nearest-x2 upsample followed by 3x3/pad1 == four 2x2 phase convolutions on the low-res input with
+// pre-summed weights: [phase=(py,px)][tap=(a,b)][Cout_pad][Cin]
+template <typename S>
+__global__ void pack_tc_up_kernel(const float* __restrict__ w, S* __restrict__ o, int Cout, int Cout_pad, int Cin) {
   long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   long long total = (long long)16 * Cout_pad * Cin;
   if (idx >= total) return;
@@ -264,19 +228,84 @@ __global__ void pack_tc3_up_kernel(const float* __restrict__ w, float* __restric
   int tap = (idx / ((long long)Cout_pad * Cin)) % 4;
   int phase = idx / ((long long)4 * Cout_pad * Cin);
   int py = phase >> 1, px = phase & 1, a = tap >> 1, b = tap & 1;
+  // rows of the 3x3 kernel that fall on low-res offset a for phase py
   int r0, r1, s0, s1;
   if (py == 0) { if (a == 0) { r0 = 0; r1 = 0; } else { r0 = 1; r1 = 2; } }
   else         { if (a == 0) { r0 = 0; r1 = 1; } else { r0 = 2; r1 = 2; } }
   if (px == 0) { if (b == 0) { s0 = 0; s1 = 0; } else { s0 = 1; s1 = 2; } }
   else         { if (b == 0) { s0 = 0; s1 = 1; } else { s0 = 2; s1 = 2; } }
-  float acc = 0.f;
+  float acc = 0.f;  // fp32 sum in this order, then one rounding
   if (co < Cout)
     for (int r = r0; r <= r1; ++r)
-      for (int q = s0; q <= s1; ++q) acc += w[(((long long)co * Cin + c) * 3 + r) * 3 + q];
-  float hi = rn_tf32_w(acc);
-  long long base = (((long long)(phase * 4 + tap) * 2) * Cout_pad + co) * Cin + c;
-  o[base] = hi;
-  o[base + (long long)Cout_pad * Cin] = rn_tf32_w(acc - hi);
+      for (int s = s0; s <= s1; ++s) acc += w[(((long long)co * Cin + c) * 3 + r) * 3 + s];
+  store_tc_w(o, phase * 4 + tap, co, c, Cout_pad, Cin, acc);
+}
+
+// Packed conv weight layouts.  SIMT: [KH*KW][Cin][Cout] fp32.  Tap-GEMM (stored as S: bf16, or float for the fp32x3 engine's
+// tf32 hi/lo pairs): plain taps [KH*KW][Cout_pad][Cin]; upsample phases (nearest x2 + 3x3) [4][4][Cout_pad][Cin]; the bf16
+// 7x7 stem [7][Cout][64]; per-image 1x1 weights [B*Cout][Cin] from a raw [B][Cout][Cin].
+enum WLayout { WL_SIMT, WL_TAPS, WL_UP, WL_STEM, WL_PER_IMAGE };
+// rows per tap of a tap-GEMM layout: Cout padded to 8, except the bf16 upsample layout (Cout rows) and per-image weights
+template <typename S>
+int packed_rows(WLayout l, int Cout, int B) {
+  if (l == WL_PER_IMAGE) return B * Cout;
+  return l == WL_UP && std::is_same<S, bf16>::value ? Cout : (Cout + 7) / 8 * 8;
+}
+template <typename S>
+long long packed_weight_elems(WLayout l, int Cout, int Cin, int KH, int KW, int B = 1) {
+  const long long parts = std::is_same<S, float>::value ? 2 : 1, rows = packed_rows<S>(l, Cout, B);
+  switch (l) {
+    case WL_SIMT: return (long long)Cout * Cin * KH * KW;
+    case WL_STEM: return 7LL * Cout * 64;
+    case WL_UP: return 16 * parts * rows * Cin;
+    default: return parts * rows * Cin * KH * KW;
+  }
+}
+template <typename S>
+void pack_weight(WLayout l, const float* w, S* o, int Cout, int Cin, int KH, int KW, int B, cudaStream_t st) {
+  const long long n = packed_weight_elems<S>(l, Cout, Cin, KH, KW, B);
+  const int rows = packed_rows<S>(l, Cout, B);
+  if constexpr (std::is_same<S, float>::value) {
+    if (l == WL_SIMT) { pack_simt_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(w, o, Cout, Cin, KH, KW); return; }
+  } else {
+    if (l == WL_STEM) { pack_tc_stem_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(w, o, Cout, Cin); return; }
+  }
+  const long long nt = n / (std::is_same<S, float>::value ? 2 : 1);  // one thread per (hi, lo) pair
+  if (l == WL_UP) pack_tc_up_kernel<S><<<(unsigned)((nt + 255) / 256), 256, 0, st>>>(w, o, Cout, rows, Cin);
+  else pack_tc_taps_kernel<S><<<(unsigned)((nt + 255) / 256), 256, 0, st>>>(w, o, l == WL_PER_IMAGE ? rows : Cout, rows, Cin, KH, KW);
+}
+
+// How the tap-GEMM runs a conv shape (callers have checked stride and padding): 3x3/1, nearest x2 + 3x3/1 (four 2x2 phase
+// convolutions), 1x1, 4x4/2 and 2x2/2 (over space-to-depth planes), and the 7x7 stem (7 row taps over its padded layout).
+struct TapTable {
+  TcTap taps[16];
+  int ntaps = 0;
+  int nph = 1;     // upsample phases
+  int planes = 1;  // A planes: 4 after the space-to-depth pass, -1 for the stem
+  bool s2d() const { return planes == 4; }
+};
+TapTable tap_table(int K, int up) {
+  TapTable t;
+  if (K == 7) {
+    for (int r = 0; r < 7; ++r) t.taps[t.ntaps++] = TcTap{r, 0, 0};
+    t.planes = -1;
+  } else if (K == 3 && up == 1) {
+    for (int r = 0; r < 3; ++r) for (int q = 0; q < 3; ++q) t.taps[t.ntaps++] = TcTap{r - 1, q - 1, 0};
+  } else if (K == 3) {
+    t.nph = 4;
+    for (int a = 0; a < 2; ++a) for (int q = 0; q < 2; ++q) t.taps[t.ntaps++] = TcTap{a - 1, q - 1, 0};
+  } else if (K == 1) {
+    t.taps[t.ntaps++] = TcTap{0, 0, 0};
+  } else {  // stride 2 over space-to-depth planes: 4x4 pad 1 (UNet Downsample) or 2x2 pad 0 (NAFNet downs)
+    static const int PY[4] = {1, 0, 1, 0}, DH[4] = {-1, 0, 0, 1};
+    if (K == 4) {
+      for (int r = 0; r < 4; ++r) for (int q = 0; q < 4; ++q) t.taps[t.ntaps++] = TcTap{DH[r], DH[q], PY[r] * 2 + PY[q]};
+    } else {
+      for (int r = 0; r < 2; ++r) for (int q = 0; q < 2; ++q) t.taps[t.ntaps++] = TcTap{0, 0, r * 2 + q};
+    }
+    t.planes = 4;
+  }
+  return t;
 }
 
 // ---- architecture description --------------------------------------------------------------------
@@ -565,8 +594,11 @@ struct Builder {
     g.Wout = (Win * up + 2 * pad - K) / stride + 1;
     g.Cout = Cout;
     double simt_flops = 2.0 * plan->B * g.Hout * g.Wout * (double)Cout * in.C * K * K;
-    // the tensor-core engine runs nearest-x2 + 3x3 as four 2x2 phase convolutions: 4 taps per output pixel
-    double tc_flops = (K == 3 && up == 2) ? simt_flops * 4.0 / 9.0 : simt_flops;
+    // the tensor-core engine runs nearest-x2 + 3x3 as four 2x2 phase convolutions (4 taps per output pixel) and the 7x7 stem
+    // as 7 row taps of 8 pixels x 8 channels
+    double tc_flops = (K == 3 && up == 2) ? simt_flops * 4.0 / 9.0
+                      : K == 7            ? 2.0 * plan->B * g.Hout * g.Wout * (double)Cout * 448
+                                          : simt_flops;
     Epilogue ep;
     memset(&ep, 0, sizeof ep);
     ep.bias = bias ? fw(bias) : nullptr;
@@ -580,146 +612,73 @@ struct Builder {
     if (res) { ep.res = res->p; ep.res_pitch = res->pitch; }
     irsde_ctx* c = ctx;
     bool nchw = out_nchw_slot != nullptr;
-    if constexpr (std::is_same<T, bf16>::value) {
-      bool shape_ok = (K == 3 && stride == 1 && pad == 1) || (K == 1 && stride == 1 && pad == 0 && up == 1) ||
-                      (K == 4 && stride == 2 && pad == 1 && up == 1 && Hin % 2 == 0 && Win % 2 == 0) ||
-                      (K == 2 && stride == 2 && pad == 0 && up == 1 && Hin % 2 == 0 && Win % 2 == 0);
-      bool stem_tc = ctx->use_tc && stem_padded && K == 7 && Cout % 8 == 0 && out.pitch % 8 == 0;
-      if (stem_tc) {
-        const bf16* wt = ctx->w_tc[wname];
-        if (!wt) { ok = false; err = "unpacked tc weight " + wname; return; }
-        TcTap taps[16];
-        for (int r = 0; r < 7; ++r) taps[r] = TcTap{r, 0, 0};
-        std::string terr;
-        TcConvDesc* d = tc_conv_create(in.p, 8, plan->B, Hin, Win, 64, -1, wt, Cout, 7, taps, 1, ep, out.p, out.pitch, g.Hout,
-                                       g.Wout, &terr);
-        if (!d) { ok = false; err = "tc_conv_create(stem): " + terr; return; }
-        plan->tc_descs.push_back(d);
-        double fl = 2.0 * plan->B * g.Hout * g.Wout * (double)Cout * 448;
-        plan->ops.push_back(OpRec{CAT_TC, fl, [=](Plan*, cudaStream_t st) {
-          tc_conv_launch(d, st);
+    const int cH = nchw_H ? nchw_H : plan->H, cW = nchw_W ? nchw_W : plan->W;  // crop of the fp32 NCHW output
+    constexpr bool f32 = std::is_same<T, float>::value;  // fp32x3 engine: tf32 hi/lo split operands
+    constexpr int al = f32 ? 4 : 8;                       // elements per 16 bytes
+    const bool stem = !f32 && stem_padded && K == 7 && Cout % al == 0 && out.pitch % al == 0;
+    bool shape_ok = (K == 3 && stride == 1 && pad == 1) || (K == 1 && stride == 1 && pad == 0 && up == 1) ||
+                    (K == 4 && stride == 2 && pad == 1 && up == 1 && Hin % 2 == 0 && Win % 2 == 0) ||
+                    (K == 2 && stride == 2 && pad == 0 && up == 1 && Hin % 2 == 0 && Win % 2 == 0);
+    shape_ok = shape_ok && in.C % al == 0 && in.pitch % al == 0 &&
+               (nchw ? (K == 3 && up == 1) : (Cout % al == 0 && out.pitch % al == 0));
+    // fused-attention flags and per-image weights are bf16-only epilogues
+    const bool engine_on = f32 ? ctx->use_tc3 && !tc_flags && !w_override && (((uintptr_t)in.p) & 15) == 0 : ctx->use_tc;
+    if (engine_on && (stem || shape_ok)) {
+      const T* wt;
+      if constexpr (f32) wt = ctx->w_tc3[wname];
+      else wt = w_override ? w_override : ctx->w_tc[wname];
+      if (!wt) { ok = false; err = (f32 ? "unpacked fp32x3 weight " : "unpacked tc weight ") + wname; return; }
+      const TapTable t = tap_table(K, up);
+      const int Ha = t.s2d() ? Hin / 2 : Hin, Wa = t.s2d() ? Win / 2 : Win;
+      const T* a = in.p;
+      int a_pitch = in.pitch;
+      if (t.s2d()) {
+        T* s2d = tmp((long long)plan->B * Hin * Win * in.C);
+        int Bc = plan->B, Cc = in.C;
+        plan->ops.push_back(OpRec{CAT_MISC, 0.0, [=](Plan*, cudaStream_t st) {
+          launch_space_to_depth<T>(in.p, in.pitch, s2d, Bc, Hin, Win, Cc, st);
           c->launches++;
         }});
-        return;
+        a = s2d; a_pitch = in.C;
+        release(s2d);  // safe: stream order; the next tmp user runs after this conv
       }
-      if (ctx->use_tc && shape_ok && in.C % 8 == 0 && in.pitch % 8 == 0 &&
-          (nchw ? (K == 3 && up == 1) : (Cout % 8 == 0 && out.pitch % 8 == 0))) {
-        const bf16* wt = w_override ? w_override : ctx->w_tc[wname];
-        if (!wt) { ok = false; err = "unpacked tc weight " + wname; return; }
-        TcTap taps[16];
-        int ntaps = 0, nph = 1, planes = 1, Ha = Hin, Wa = Win, a_pitch = in.pitch;
-        const bf16* a_ptr = in.p;
-        if (K == 3 && up == 1) {
-          for (int r = 0; r < 3; ++r) for (int q = 0; q < 3; ++q) taps[ntaps++] = TcTap{r - 1, q - 1, 0};
-        } else if (K == 3 && up == 2) {
-          nph = 4;
-          for (int a = 0; a < 2; ++a) for (int q = 0; q < 2; ++q) taps[ntaps++] = TcTap{a - 1, q - 1, 0};
-        } else if (K == 1) {
-          taps[ntaps++] = TcTap{0, 0, 0};
-        } else {  // stride 2 over space-to-depth planes: 4x4 pad 1 (UNet Downsample) or 2x2 pad 0 (NAFNet downs)
-          static const int PY[4] = {1, 0, 1, 0}, DH[4] = {-1, 0, 0, 1};
-          if (K == 4) {
-            for (int r = 0; r < 4; ++r) for (int q = 0; q < 4; ++q) taps[ntaps++] = TcTap{DH[r], DH[q], PY[r] * 2 + PY[q]};
-          } else {
-            for (int r = 0; r < 2; ++r) for (int q = 0; q < 2; ++q) taps[ntaps++] = TcTap{0, 0, r * 2 + q};
-          }
-          planes = 4; Ha = Hin / 2; Wa = Win / 2; a_pitch = in.C;
-          bf16* s2d = tmp((long long)plan->B * Hin * Win * in.C);
-          int Bc = plan->B, Cc = in.C;
-          plan->ops.push_back(OpRec{CAT_MISC, 0.0, [=](Plan*, cudaStream_t st) {
-            launch_space_to_depth<bf16>(in.p, in.pitch, s2d, Bc, Hin, Win, Cc, st);
-            c->launches++;
-          }});
-          a_ptr = s2d;
-          release(s2d);  // safe: stream order; the next tmp user runs after this conv
-        }
-        std::string terr;
-        TcConvDesc* d = tc_conv_create(a_ptr, a_pitch, plan->B, Ha, Wa, in.C, planes, wt, Cout, ntaps, taps, nph, ep, out.p,
-                                       out.pitch, g.Hout, g.Wout, &terr, tc_flags);
-        if (!d) { ok = false; err = "tc_conv_create(" + wname + "): " + terr; return; }
-        plan->tc_descs.push_back(d);
-        int cH = nchw_H ? nchw_H : plan->H, cW = nchw_W ? nchw_W : plan->W;
-        plan->ops.push_back(OpRec{CAT_TC, tc_flops, [=](Plan* p, cudaStream_t st) {
-          if (use_ss) tc_conv_set_runtime(d, p->cur.ss, p->cur.t_ptr, p->cur.ss_img_stride);
-          if (nchw) tc_conv_set_out_nchw(d, p->cur.out, cH, cW);
-          tc_conv_launch(d, st);
-          c->launches++;
-        }});
-        return;
-      }
-    }
-    if constexpr (std::is_same<T, float>::value) {
-      bool shape_ok = (K == 3 && stride == 1 && pad == 1) || (K == 1 && stride == 1 && pad == 0 && up == 1) ||
-                      (K == 4 && stride == 2 && pad == 1 && up == 1 && Hin % 2 == 0 && Win % 2 == 0) ||
-                      (K == 2 && stride == 2 && pad == 0 && up == 1 && Hin % 2 == 0 && Win % 2 == 0);
-      if (ctx->use_tc3 && shape_ok && !tc_flags && !w_override && in.C % 4 == 0 && in.pitch % 4 == 0 &&
-          (((uintptr_t)in.p) & 15) == 0 && (nchw ? (K == 3 && up == 1) : (Cout % 4 == 0 && out.pitch % 4 == 0))) {
-        const float* wt = ctx->w_tc3[wname];
-        if (!wt) { ok = false; err = "unpacked fp32x3 weight " + wname; return; }
-        TcTap taps[16];
-        int ntaps = 0, nph = 1, planes = 1, Ha = Hin, Wa = Win;
-        const float* a_src = in.p;
-        int a_pitch = in.pitch;
-        if (K == 3 && up == 1) {
-          for (int r = 0; r < 3; ++r) for (int q = 0; q < 3; ++q) taps[ntaps++] = TcTap{r - 1, q - 1, 0};
-        } else if (K == 3 && up == 2) {
-          nph = 4;
-          for (int a = 0; a < 2; ++a) for (int q = 0; q < 2; ++q) taps[ntaps++] = TcTap{a - 1, q - 1, 0};
-        } else if (K == 1) {
-          taps[ntaps++] = TcTap{0, 0, 0};
-        } else {
-          static const int PY[4] = {1, 0, 1, 0}, DH[4] = {-1, 0, 0, 1};
-          if (K == 4) {
-            for (int r = 0; r < 4; ++r) for (int q = 0; q < 4; ++q) taps[ntaps++] = TcTap{DH[r], DH[q], PY[r] * 2 + PY[q]};
-          } else {
-            for (int r = 0; r < 2; ++r) for (int q = 0; q < 2; ++q) taps[ntaps++] = TcTap{0, 0, r * 2 + q};
-          }
-          planes = 4; Ha = Hin / 2; Wa = Win / 2;
-          float* s2d = tmp((long long)plan->B * Hin * Win * in.C);
-          int Bc = plan->B, Cc = in.C;
-          plan->ops.push_back(OpRec{CAT_MISC, 0.0, [=](Plan*, cudaStream_t st) {
-            launch_space_to_depth<float>(in.p, in.pitch, s2d, Bc, Hin, Win, Cc, st);
-            c->launches++;
-          }});
-          a_src = s2d; a_pitch = in.C;
-          release(s2d);
-        }
+      std::string terr;
+      TcConvDesc* d;
+      if constexpr (f32) {
         // operand split (hi, lo) of the conv input: [2][planes][B][Ha][Wa][C]
-        const long long npix_a = (long long)planes * plan->B * Ha * Wa;
+        const long long npix_a = (long long)t.planes * plan->B * Ha * Wa;
         float* split = tmp(2 * npix_a * in.C);
-        {
-          int Cc = in.C;
-          plan->ops.push_back(OpRec{CAT_MISC, 0.0, [=](Plan*, cudaStream_t st) {
-            launch_split_tf32(a_src, a_pitch, split, npix_a, Cc, st);
-            c->launches++;
-          }});
-          plan->ops.back().label = wname + " tf32 hi/lo split of the input";
-          plan->ops.back().bytes = 3.0 * npix_a * in.C * 4.0;
-        }
-        std::string terr;
-        TcConvDesc* d = tc_conv_create_f32x3(split, plan->B, Ha, Wa, in.C, planes, wt, Cout, ntaps, taps, nph, ep, out.p, out.pitch,
-                                             g.Hout, g.Wout, &terr);
-        release(split);
-        if (!d) { ok = false; err = "tc_conv_create_f32x3(" + wname + "): " + terr; return; }
-        plan->tc_descs.push_back(d);
-        int cH = nchw_H ? nchw_H : plan->H, cW = nchw_W ? nchw_W : plan->W;
-        plan->ops.push_back(OpRec{CAT_TC, tc_flops, [=](Plan* p, cudaStream_t st) {
-          if (use_ss) tc_conv_set_runtime(d, p->cur.ss, p->cur.t_ptr, p->cur.ss_img_stride);
-          if (nchw) tc_conv_set_out_nchw(d, p->cur.out, cH, cW);
-          tc_conv_launch(d, st);
+        int Cc = in.C;
+        plan->ops.push_back(OpRec{CAT_MISC, 0.0, [=](Plan*, cudaStream_t st) {
+          launch_split_tf32(a, a_pitch, split, npix_a, Cc, st);
           c->launches++;
         }});
-        return;
+        plan->ops.back().label = wname + " tf32 hi/lo split of the input";
+        plan->ops.back().bytes = 3.0 * npix_a * in.C * 4.0;
+        d = tc_conv_create_f32x3(split, plan->B, Ha, Wa, in.C, t.planes, wt, Cout, t.ntaps, t.taps, t.nph, ep, out.p, out.pitch,
+                                 g.Hout, g.Wout, &terr);
+        release(split);
+      } else {
+        d = tc_conv_create(a, a_pitch, plan->B, Ha, Wa, stem ? 64 : in.C, t.planes, wt, Cout, t.ntaps, t.taps, t.nph, ep, out.p,
+                           out.pitch, g.Hout, g.Wout, &terr, tc_flags);
       }
+      if (!d) { ok = false; err = (f32 ? "tc_conv_create_f32x3(" : "tc_conv_create(") + wname + "): " + terr; return; }
+      plan->tc_descs.push_back(d);
+      plan->ops.push_back(OpRec{CAT_TC, tc_flops, [=](Plan* p, cudaStream_t st) {
+        if (use_ss) tc_conv_set_runtime(d, p->cur.ss, p->cur.t_ptr, p->cur.ss_img_stride);
+        if (nchw) tc_conv_set_out_nchw(d, p->cur.out, cH, cW);
+        tc_conv_launch(d, st);
+        c->launches++;
+      }});
+      return;
     }
     if (tc_flags || w_override) { ok = false; err = "fused attention conv needs the tensor-core engine: " + wname; return; }
     const float* w = ctx->w_simt[wname];
     if (!w) { ok = false; err = "unpacked weight " + wname; return; }
-    int H = nchw_H ? nchw_H : plan->H, Wd = nchw_W ? nchw_W : plan->W;
     plan->ops.push_back(OpRec{CAT_SIMT, simt_flops, [=](Plan* p, cudaStream_t st) {
       Epilogue e = ep;
       if (use_ss) { e.ss = p->cur.ss; e.t_ptr = p->cur.t_ptr; e.ss_img_stride = p->cur.ss_img_stride; }
-      launch_conv_simt<T>(g, in.p, in.pitch, w, e, out.p, out.pitch, nchw ? p->cur.out : nullptr, H, Wd, st);
+      launch_conv_simt<T>(g, in.p, in.pitch, w, e, out.p, out.pitch, nchw ? p->cur.out : nullptr, cH, cW, st);
       c->launches++;
     }});
   }
@@ -1407,6 +1366,67 @@ int ensure_chain_table(irsde_ctx* ctx, Plan* p, int T, cudaStream_t st) {
   return IRSDE_OK;
 }
 
+// ---- one tap-GEMM conv outside a plan (irsde_conv2d_ex, irsde_conv2d_fused) ------------------------------------------
+__global__ void cast_f32_bf16_kernel(const float* __restrict__ in, bf16* __restrict__ out, long long n) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    out[i] = __float2bfloat16_rn(in[i]);
+}
+__global__ void cast_bf16_f32_kernel(const bf16* __restrict__ in, float* __restrict__ out, long long n) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    out[i] = __bfloat162float(in[i]);
+}
+
+// Runs the conv the plan builder would make of this shape: `in` is an NHWC view in the engine's storage type S (bf16, or
+// fp32 for the fp32x3 engine; the stem's padded layout for K == 7), `w` is packed by pack_weight<S>.  Output: the NHWC view
+// (out, out_pitch), or with out == nullptr fp32 NCHW at out_nchw cropped to crop_h x crop_w.  As in a plan, the time table
+// of `ep` (ss, t_ptr, ss_img_stride) is attached after the descriptor is created.  info (may be null) receives
+// tc_conv_query.  Waits for the stream before it frees its scratch; `what` prefixes the error of a failed launch.
+template <typename S>
+int run_tc_conv(irsde_ctx* ctx, const char* what, const S* in, int in_pitch, int B, int H, int W, int Cin, int K, int up,
+                const S* w, int Cout, int Ho, int Wo, const Epilogue& ep, S* out, int out_pitch, float* out_nchw, int crop_h,
+                int crop_w, int flags, int32_t* info, cudaStream_t st) {
+  constexpr bool f32 = std::is_same<S, float>::value;
+  const TapTable t = tap_table(K, up);
+  const int Ha = t.s2d() ? H / 2 : H, Wa = t.s2d() ? W / 2 : W;
+  const long long npix = (long long)B * H * W;  // A pixels, also after the space-to-depth pass (4 planes of Ha x Wa)
+  std::vector<void*> scratch;
+  S* s2d = t.s2d() ? (S*)dev_alloc(ctx, npix * Cin * sizeof(S), &scratch) : nullptr;
+  float* split = f32 ? (float*)dev_alloc(ctx, 2 * npix * Cin * 4, &scratch) : nullptr;
+  if ((t.s2d() && !s2d) || (f32 && !split)) {
+    for (void* q : scratch) cudaFree(q);
+    return fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
+  }
+  if (s2d) {
+    launch_space_to_depth<S>(in, in_pitch, s2d, B, H, W, Cin, st);
+    in = s2d;
+    in_pitch = Cin;
+  }
+  Epilogue e0 = ep;
+  e0.ss = nullptr; e0.t_ptr = nullptr; e0.ss_img_stride = 0;
+  std::string terr;
+  TcConvDesc* d;
+  if constexpr (f32) {
+    launch_split_tf32(in, in_pitch, split, npix, Cin, st);
+    d = tc_conv_create_f32x3(split, B, Ha, Wa, Cin, t.planes, w, Cout, t.ntaps, t.taps, t.nph, e0, out, out_pitch, Ho, Wo, &terr);
+  } else {
+    d = tc_conv_create(in, in_pitch, B, Ha, Wa, t.planes < 0 ? 64 : Cin, t.planes, w, Cout, t.ntaps, t.taps, t.nph, e0, out,
+                       out_pitch, Ho, Wo, &terr, flags);
+  }
+  int rc = d ? IRSDE_OK : fail(ctx, IRSDE_ERR_INVALID, std::string(f32 ? "tc_conv_create_f32x3: " : "tc_conv_create: ") + terr);
+  if (d) {
+    if (ep.ss) tc_conv_set_runtime(d, ep.ss, ep.t_ptr, ep.ss_img_stride);
+    if (!out) tc_conv_set_out_nchw(d, out_nchw, crop_h, crop_w);
+    if (info) tc_conv_query(d, info);
+    tc_conv_launch(d, st);
+    tc_conv_destroy(d);
+  }
+  cudaError_t ce = cudaStreamSynchronize(st);
+  if (!rc && ce == cudaSuccess) ce = cudaGetLastError();
+  if (!rc && ce != cudaSuccess) rc = fail(ctx, IRSDE_ERR_CUDA, std::string(what) + cudaGetErrorString(ce));
+  for (void* q : scratch) cudaFree(q);
+  return rc;
+}
+
 }  // namespace
 
 // =====================================================================================================
@@ -1703,42 +1723,21 @@ int irsde_finalize_weights(irsde_ctx* ctx) {
     if (ctx->naf.on && (s.shape[0] == 1 || s.name.find("conv2.weight") != std::string::npos ||
                         s.name.find("sca.1.weight") != std::string::npos))
       continue;  // beta/gamma vectors, depthwise and SCA weights are consumed raw
-    int Cout = (int)s.shape[0], Cin = (int)s.shape[1], KH = (int)s.shape[2], KW = (int)s.shape[3];
-    long long n = (long long)Cout * Cin * KH * KW;
-    float*& ws = ctx->w_simt[s.name];
-    if (!ws) ws = (float*)dev_alloc(ctx, (size_t)n * 4, &ctx->allocs);
-    if (!ws) return fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
-    pack_simt_kernel<<<(unsigned)((n + 255) / 256), 256>>>(ctx->raw[s.name].dev, ws, Cout, Cin, KH, KW);
-    if (ctx->cfg.precision == IRSDE_PREC_FP32X3 && !(KH == 7)) {
-      bool is_up = s.name.find(".3.1.weight") != std::string::npos && KH == 3;
-      int Cout_pad = (Cout + 7) / 8 * 8;
-      long long nt = (long long)(is_up ? 16 : KH * KW) * 2 * Cout_pad * Cin;
-      float*& wt = ctx->w_tc3[s.name];
-      if (!wt) wt = (float*)dev_alloc(ctx, (size_t)nt * 4, &ctx->allocs);
-      if (!wt) return fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
-      long long nthreads = nt / 2;
-      if (is_up)
-        pack_tc3_up_kernel<<<(unsigned)((nthreads + 255) / 256), 256>>>(ctx->raw[s.name].dev, wt, Cout, Cout_pad, Cin);
-      else
-        pack_tc3_kernel<<<(unsigned)((nthreads + 255) / 256), 256>>>(ctx->raw[s.name].dev, wt, Cout, Cout_pad, Cin, KH, KW);
-    }
-    if (ctx->cfg.precision == IRSDE_PREC_BF16) {
-      bool is_up = s.name.find(".3.1.weight") != std::string::npos;
-      bool is_stem = s.name == "init_conv.weight" && KH == 7;
-      int Cout_pad = (Cout + 7) / 8 * 8;
-      long long nt = is_up ? (long long)16 * Cout * Cin : (is_stem ? (long long)7 * Cout * 64 : (long long)Cout_pad * Cin * KH * KW);
-      bf16*& wt = ctx->w_tc[s.name];
-      if (!wt) wt = (bf16*)dev_alloc(ctx, (size_t)nt * 2, &ctx->allocs);
-      if (!wt) return fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
-      if (is_up)
-        pack_tc_up_kernel<<<(unsigned)((nt + 255) / 256), 256>>>(ctx->raw[s.name].dev, wt, Cout, Cin);
-      else if (is_stem && Cin <= 8)
-        pack_tc_stem_kernel<<<(unsigned)((nt + 255) / 256), 256>>>(ctx->raw[s.name].dev, wt, Cout, Cin);
-      else if (Cout_pad != Cout)
-        pack_tc_padded_kernel<<<(unsigned)((nt + 255) / 256), 256>>>(ctx->raw[s.name].dev, wt, Cout, Cout_pad, Cin, KH, KW);
-      else
-        pack_tc_kernel<<<(unsigned)((n + 255) / 256), 256>>>(ctx->raw[s.name].dev, wt, Cout, Cin, KH, KW);
-    }
+    const int Cout = (int)s.shape[0], Cin = (int)s.shape[1], KH = (int)s.shape[2], KW = (int)s.shape[3];
+    const float* raw = ctx->raw[s.name].dev;
+    auto pack_into = [&](auto*& buf, WLayout l) {
+      using S = std::remove_reference_t<decltype(*buf)>;
+      if (!buf) buf = (S*)dev_alloc(ctx, (size_t)packed_weight_elems<S>(l, Cout, Cin, KH, KW) * sizeof(S), &ctx->allocs);
+      if (buf) pack_weight<S>(l, raw, buf, Cout, Cin, KH, KW, 1, 0);
+      return buf != nullptr;
+    };
+    if (!pack_into(ctx->w_simt[s.name], WL_SIMT)) return fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
+    // the tap-GEMM runs a 7x7 conv only as the bf16 stem over at most 8 input channels; the Upsample convs (".3.1.") are
+    // nearest x2 + 3x3
+    const bool bf = ctx->cfg.precision == IRSDE_PREC_BF16;
+    if (ctx->cfg.precision == IRSDE_PREC_FP32 || (KH == 7 && !(bf && Cin <= 8))) continue;
+    const WLayout l = KH == 7 ? WL_STEM : (KH == 3 && s.name.find(".3.1.weight") != std::string::npos ? WL_UP : WL_TAPS);
+    if (!(bf ? pack_into(ctx->w_tc[s.name], l) : pack_into(ctx->w_tc3[s.name], l))) return fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
   }
   // time-modulation: concatenate every block's mlp.1 into one [S][td_in] matrix
   // (UNet ResBlock: Linear(4nf -> 2*Cout); NAFBlock: Linear(2w -> 4c))
@@ -2089,10 +2088,8 @@ int irsde_conv2d_ex(irsde_ctx* ctx, int32_t engine, const float* x, const float*
     int Cout_pad = (Cout + 7) / 8 * 8;
     std::vector<void*> tmp;
     long long nin = k7 ? (long long)B * (H + 6) * (W + 8) * 8 + 64 : (long long)B * H * W * Cin;
-    long long nw = (long long)Cout * Cin * KH * KW, nout = (long long)B * Ho * Wo * Cout_pad;
-    long long nwt = (k3 && up == 2) ? (long long)16 * Cout * Cin : (k7 ? (long long)7 * Cout * 64 : (long long)Cout_pad * Cin * KH * KW);
-    if (f_wimg) nwt *= B;  // w is [B][Cout][Cin]
-    (void)nw;
+    long long nout = (long long)B * Ho * Wo * Cout_pad;
+    const WLayout wl = k7 ? WL_STEM : f_wimg ? WL_PER_IMAGE : (k3 && up == 2) ? WL_UP : WL_TAPS;  // per-image: w is [B][Cout][Cin]
     bf16* resb = nullptr;
     if (residual) {
       if (nchw) return fail(ctx, IRSDE_ERR_UNSUPPORTED, "residual needs Cout % 8 == 0");
@@ -2101,56 +2098,34 @@ int irsde_conv2d_ex(irsde_ctx* ctx, int32_t engine, const float* x, const float*
       launch_nchw_to_nhwc<bf16>(residual, resb, B, Cout, Ho, Wo, Cout, st);
     }
     bf16* xin = (bf16*)dev_alloc(ctx, nin * 2, &tmp);
-    bf16* xs2d = (bf16*)dev_alloc(ctx, nin * 2, &tmp);
-    bf16* wp = (bf16*)dev_alloc(ctx, nwt * 2, &tmp);
+    bf16* wp = (bf16*)dev_alloc(ctx, packed_weight_elems<bf16>(wl, Cout, Cin, KH, KW, B) * 2, &tmp);
     bf16* yo = (bf16*)dev_alloc(ctx, nout * 2, &tmp);
     int rc = IRSDE_OK;
-    TcConvDesc* d = nullptr;
-    if (!xin || !xs2d || !wp || !yo) rc = fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
+    if (!xin || !wp || !yo) rc = fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
     if (!rc) {
       if (k7) {
         cudaMemsetAsync(xin, 0, nin * 2, st);
         launch_prep_input<bf16>(x, nullptr, xin, B, Cin, H, W, H, W, 8, 0, st, 3, 3, W + 8, H + 6);
-        pack_tc_stem_kernel<<<(unsigned)((nwt + 255) / 256), 256, 0, st>>>(w, wp, Cout, Cin);
       } else {
         launch_nchw_to_nhwc<bf16>(x, xin, B, Cin, H, W, Cin, st);
-        if (k3 && up == 2) pack_tc_up_kernel<<<(unsigned)((nwt + 255) / 256), 256, 0, st>>>(w, wp, Cout, Cin);
-        else if (f_wimg) pack_tc_kernel<<<(unsigned)((nwt + 255) / 256), 256, 0, st>>>(w, wp, B * Cout, Cin, 1, 1);
-        else pack_tc_padded_kernel<<<(unsigned)((nwt + 255) / 256), 256, 0, st>>>(w, wp, Cout, Cout_pad, Cin, KH, KW);
       }
-      TcTap taps[16];
-      int ntaps = 0, nph = 1, planes = 1, Ha = H, Wa = W, Ca = Cin, a_pitch = Cin;
-      const bf16* a_ptr = xin;
-      if (k7) { for (int r = 0; r < 7; ++r) taps[ntaps++] = TcTap{r, 0, 0}; planes = -1; Ca = 64; a_pitch = 8; }
-      else if (k3 && up == 1) { for (int r = 0; r < 3; ++r) for (int q = 0; q < 3; ++q) taps[ntaps++] = TcTap{r - 1, q - 1, 0}; }
-      else if (k3) { nph = 4; for (int a = 0; a < 2; ++a) for (int q = 0; q < 2; ++q) taps[ntaps++] = TcTap{a - 1, q - 1, 0}; }
-      else if (k1) { taps[ntaps++] = TcTap{0, 0, 0}; }
-      else {
-        static const int PY[4] = {1, 0, 1, 0}, DH[4] = {-1, 0, 0, 1};
-        for (int r = 0; r < 4; ++r) for (int q = 0; q < 4; ++q) taps[ntaps++] = TcTap{DH[r], DH[q], PY[r] * 2 + PY[q]};
-        planes = 4; Ha = H / 2; Wa = W / 2;
-        launch_space_to_depth<bf16>(xin, Cin, xs2d, B, H, W, Cin, st);
-        a_ptr = xs2d;
-      }
+      pack_weight<bf16>(wl, w, wp, Cout, Cin, KH, KW, B, st);
       Epilogue ep;
       memset(&ep, 0, sizeof ep);
       ep.bias = bias;
       ep.silu = silu;
       if (resb) { ep.res = resb; ep.res_pitch = Cout; }
-      d = tc_conv_create(a_ptr, a_pitch, B, Ha, Wa, Ca, planes, wp, Cout, ntaps, taps, nph, ep, nchw ? nullptr : yo, Cout, Ho, Wo, &terr,
-                         (f_qsm ? TC_FLAG_QSOFTMAX : 0) | (f_wimg ? TC_FLAG_W_PER_IMAGE : 0));
-      if (!d) rc = fail(ctx, IRSDE_ERR_INVALID, "tc_conv_create: " + terr);
+      rc = run_tc_conv<bf16>(ctx, "tensor-core conv2d failed: ", xin, k7 ? 8 : Cin, B, H, W, Cin, KH, up, wp, Cout, Ho, Wo, ep,
+                             nchw ? nullptr : yo, Cout, y, Ho, Wo,
+                             (f_qsm ? TC_FLAG_QSOFTMAX : 0) | (f_wimg ? TC_FLAG_W_PER_IMAGE : 0), nullptr, st);
     }
     if (!rc) {
-      if (nchw) tc_conv_set_out_nchw(d, y, Ho, Wo);
-      tc_conv_launch(d, st);
       if (!nchw) launch_nhwc_to_nchw<bf16>(yo, Cout, y, B, Cout, Ho, Wo, st);
       ctx->launches += 4;
       cudaError_t e = cudaStreamSynchronize(st);
       if (e == cudaSuccess) e = cudaGetLastError();
       if (e != cudaSuccess) rc = fail(ctx, IRSDE_ERR_CUDA, std::string("tensor-core conv2d failed: ") + cudaGetErrorString(e));
     }
-    if (d) tc_conv_destroy(d);
     for (void* q : tmp) cudaFree(q);
     return rc;
   }
@@ -2164,56 +2139,34 @@ int irsde_conv2d_ex(irsde_ctx* ctx, int32_t engine, const float* x, const float*
     if (!(k3 || k1 || k4) || Cin % 4 || (nchw && !(k3 && up == 1)) || residual && nchw)
       return fail(ctx, IRSDE_ERR_UNSUPPORTED, "shape not supported by the fp32x3 engine");
     int Ho = (H * up + 2 * pad - KH) / stride + 1, Wo = (W * up + 2 * pad - KW) / stride + 1;
-    int Cout_pad = (Cout + 7) / 8 * 8;
     std::vector<void*> tmp;
     long long nin = (long long)B * H * W * Cin, nout = (long long)B * Ho * Wo * Cout;
-    long long nwt = (long long)((k3 && up == 2) ? 16 : KH * KW) * 2 * Cout_pad * Cin;
+    const WLayout wl = (k3 && up == 2) ? WL_UP : WL_TAPS;
     float* xin = (float*)dev_alloc(ctx, nin * 4, &tmp);
-    float* xs2d = (float*)dev_alloc(ctx, nin * 4, &tmp);
-    float* xsp = (float*)dev_alloc(ctx, 2 * nin * 4, &tmp);
-    float* wp = (float*)dev_alloc(ctx, nwt * 4, &tmp);
+    float* wp = (float*)dev_alloc(ctx, packed_weight_elems<float>(wl, Cout, Cin, KH, KW) * 4, &tmp);
     float* yo = (float*)dev_alloc(ctx, (nout + 16) * 4, &tmp);
     float* resb = residual ? (float*)dev_alloc(ctx, nout * 4, &tmp) : nullptr;
     int rc = IRSDE_OK;
-    TcConvDesc* d = nullptr;
-    if (!xin || !xs2d || !xsp || !wp || !yo || (residual && !resb)) rc = fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
+    if (!xin || !wp || !yo || (residual && !resb)) rc = fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
     if (!rc) {
       launch_nchw_to_nhwc<float>(x, xin, B, Cin, H, W, Cin, st);
       if (resb) launch_nchw_to_nhwc<float>(residual, resb, B, Cout, Ho, Wo, Cout, st);
-      if (k3 && up == 2) pack_tc3_up_kernel<<<(unsigned)((nwt / 2 + 255) / 256), 256, 0, st>>>(w, wp, Cout, Cout_pad, Cin);
-      else pack_tc3_kernel<<<(unsigned)((nwt / 2 + 255) / 256), 256, 0, st>>>(w, wp, Cout, Cout_pad, Cin, KH, KW);
-      TcTap taps[16];
-      int ntaps = 0, nph = 1, planes = 1, Ha = H, Wa = W;
-      const float* a_src = xin;
-      if (k3 && up == 1) { for (int r = 0; r < 3; ++r) for (int q = 0; q < 3; ++q) taps[ntaps++] = TcTap{r - 1, q - 1, 0}; }
-      else if (k3) { nph = 4; for (int a = 0; a < 2; ++a) for (int q = 0; q < 2; ++q) taps[ntaps++] = TcTap{a - 1, q - 1, 0}; }
-      else if (k1) { taps[ntaps++] = TcTap{0, 0, 0}; }
-      else {
-        static const int PY[4] = {1, 0, 1, 0}, DH[4] = {-1, 0, 0, 1};
-        for (int r = 0; r < 4; ++r) for (int q = 0; q < 4; ++q) taps[ntaps++] = TcTap{DH[r], DH[q], PY[r] * 2 + PY[q]};
-        planes = 4; Ha = H / 2; Wa = W / 2;
-        launch_space_to_depth<float>(xin, Cin, xs2d, B, H, W, Cin, st);
-        a_src = xs2d;
-      }
-      launch_split_tf32(a_src, Cin, xsp, (long long)planes * B * Ha * Wa, Cin, st);
+      pack_weight<float>(wl, w, wp, Cout, Cin, KH, KW, 1, st);
       Epilogue ep;
       memset(&ep, 0, sizeof ep);
       ep.bias = bias;
       ep.silu = silu;
       if (resb) { ep.res = resb; ep.res_pitch = Cout; }
-      d = tc_conv_create_f32x3(xsp, B, Ha, Wa, Cin, planes, wp, Cout, ntaps, taps, nph, ep, nchw ? nullptr : yo, Cout, Ho, Wo, &terr);
-      if (!d) rc = fail(ctx, IRSDE_ERR_INVALID, "tc_conv_create_f32x3: " + terr);
+      rc = run_tc_conv<float>(ctx, "fp32x3 conv2d failed: ", xin, Cin, B, H, W, Cin, KH, up, wp, Cout, Ho, Wo, ep,
+                              nchw ? nullptr : yo, Cout, y, Ho, Wo, 0, nullptr, st);
     }
     if (!rc) {
-      if (nchw) tc_conv_set_out_nchw(d, y, Ho, Wo);
-      tc_conv_launch(d, st);
       if (!nchw) launch_nhwc_to_nchw<float>(yo, Cout, y, B, Cout, Ho, Wo, st);
       ctx->launches += 5;
       cudaError_t e = cudaStreamSynchronize(st);
       if (e == cudaSuccess) e = cudaGetLastError();
       if (e != cudaSuccess) rc = fail(ctx, IRSDE_ERR_CUDA, std::string("fp32x3 conv2d failed: ") + cudaGetErrorString(e));
     }
-    if (d) tc_conv_destroy(d);
     for (void* q : tmp) cudaFree(q);
     return rc;
   }
@@ -2224,15 +2177,15 @@ int irsde_conv2d_ex(irsde_ctx* ctx, int32_t engine, const float* x, const float*
   g.Wout = (W * up + 2 * pad - KW) / stride + 1;
   g.Cout = Cout;
   std::vector<void*> tmp;
-  long long nin = (long long)B * H * W * Cin, nw = (long long)Cout * Cin * KH * KW, nout = (long long)B * g.Hout * g.Wout * Cout;
+  long long nin = (long long)B * H * W * Cin, nout = (long long)B * g.Hout * g.Wout * Cout;
   float* xin = (float*)dev_alloc(ctx, nin * 4, &tmp);
-  float* wp = (float*)dev_alloc(ctx, nw * 4, &tmp);
+  float* wp = (float*)dev_alloc(ctx, packed_weight_elems<float>(WL_SIMT, Cout, Cin, KH, KW) * 4, &tmp);
   float* yo = (float*)dev_alloc(ctx, nout * 4, &tmp);
   int rc = IRSDE_OK;
   if (!xin || !wp || !yo) rc = fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
   if (!rc) {
     launch_nchw_to_nhwc<float>(x, xin, B, Cin, H, W, Cin, st);
-    pack_simt_kernel<<<(unsigned)((nw + 255) / 256), 256, 0, st>>>(w, wp, Cout, Cin, KH, KW);
+    pack_weight<float>(WL_SIMT, w, wp, Cout, Cin, KH, KW, 1, st);
     Epilogue ep;
     memset(&ep, 0, sizeof ep);
     ep.bias = bias;
@@ -2244,15 +2197,6 @@ int irsde_conv2d_ex(irsde_ctx* ctx, int32_t engine, const float* x, const float*
   }
   for (void* q : tmp) { cudaFree(q); }
   return rc;
-}
-
-__global__ void cast_f32_bf16_kernel(const float* __restrict__ in, bf16* __restrict__ out, long long n) {
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-    out[i] = __float2bfloat16_rn(in[i]);
-}
-__global__ void cast_bf16_f32_kernel(const bf16* __restrict__ in, float* __restrict__ out, long long n) {
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-    out[i] = __bfloat162float(in[i]);
 }
 
 int irsde_conv2d_fused(irsde_ctx* ctx, int32_t engine, const float* x, const float* w, const irsde_conv_epilogue* epi, float* y,
@@ -2307,8 +2251,7 @@ int irsde_conv2d_fused(irsde_ctx* ctx, int32_t engine, const float* x, const flo
   cudaStream_t st = (cudaStream_t)stream;
   std::string terr;
   if (engine != 0 && !tc_init(&terr)) return fail(ctx, IRSDE_ERR_CUDA, "tc_init: " + terr);
-  const long long npix_in = (long long)B * H * W, npix_out = (long long)B * Ho * Wo;
-  const int Cout_pad = (Cout + 7) / 8 * 8;
+  const long long npix_out = (long long)B * Ho * Wo;
   std::vector<void*> tmp;
   int rc = IRSDE_OK;
   int* t_dev = (int*)dev_alloc(ctx, sizeof(int), &tmp);
@@ -2321,94 +2264,48 @@ int irsde_conv2d_fused(irsde_ctx* ctx, int32_t engine, const float* x, const flo
   ep.silu = e.silu;
   ep.ss_S = e.ss_S;
   ep.ss_off = e.ss_off;
+  if (e.ss) { ep.ss = e.ss; ep.t_ptr = t_dev; ep.ss_img_stride = e.ss_img_stride; }
   ep.res_pitch = e.res_pitch;
-  // same taps as the plan builder (conv_impl)
-  TcTap taps[16];
-  int ntaps = 0, nph = 1, planes = 1, Ha = H, Wa = W;
-  if (k3 && up == 1) { for (int r = 0; r < 3; ++r) for (int q = 0; q < 3; ++q) taps[ntaps++] = TcTap{r - 1, q - 1, 0}; }
-  else if (k3) { nph = 4; for (int a = 0; a < 2; ++a) for (int q = 0; q < 2; ++q) taps[ntaps++] = TcTap{a - 1, q - 1, 0}; }
-  else if (k1) { taps[ntaps++] = TcTap{0, 0, 0}; }
-  else {
-    static const int PY[4] = {1, 0, 1, 0}, DH[4] = {-1, 0, 0, 1};
-    for (int r = 0; r < 4; ++r) for (int q = 0; q < 4; ++q) taps[ntaps++] = TcTap{DH[r], DH[q], PY[r] * 2 + PY[q]};
-    planes = 4; Ha = H / 2; Wa = W / 2;
-  }
+  const WLayout wl = engine == 0 ? WL_SIMT : (k3 && up == 2) ? WL_UP : WL_TAPS;
   auto blocks = [](long long n) { return (unsigned)std::min<long long>((n + 255) / 256, 65536); };
-  TcConvDesc* d = nullptr;
-  bf16* yb = nullptr;
   if (!rc && engine == 0) {
     ConvGeom g;
     g.B = B; g.Hin = H; g.Win = W; g.Cin = Cin; g.up = up; g.KH = KH; g.KW = KW; g.stride = stride; g.pad = pad;
     g.Hout = Ho; g.Wout = Wo; g.Cout = Cout;
-    const long long nw = (long long)Cout * Cin * KH * KW;
-    float* wp = (float*)dev_alloc(ctx, nw * 4, &tmp);
+    float* wp = (float*)dev_alloc(ctx, packed_weight_elems<float>(wl, Cout, Cin, KH, KW) * 4, &tmp);
     if (!wp) rc = fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
     if (!rc) {
-      pack_simt_kernel<<<(unsigned)((nw + 255) / 256), 256, 0, st>>>(w, wp, Cout, Cin, KH, KW);
-      if (e.ss) { ep.ss = e.ss; ep.t_ptr = t_dev; ep.ss_img_stride = e.ss_img_stride; }
+      pack_weight<float>(wl, w, wp, Cout, Cin, KH, KW, 1, st);
       if (e.res) ep.res = e.res + e.res_off;
       launch_conv_simt<float>(g, x + e.in_off, e.in_pitch, wp, ep, nchw ? nullptr : y + e.out_off, e.out_pitch, nchw ? y : nullptr,
                               e.crop_h, e.crop_w, st);
     }
   } else if (!rc && engine == 1) {
-    const long long nin = npix_in * e.in_pitch;
-    const long long nwt = (k3 && up == 2) ? 16LL * Cout * Cin : (long long)Cout_pad * Cin * KH * KW;
+    const long long nin = (long long)B * H * W * e.in_pitch;
     bf16* xb = (bf16*)dev_alloc(ctx, nin * 2, &tmp);
-    bf16* s2d = k4 ? (bf16*)dev_alloc(ctx, npix_in * Cin * 2, &tmp) : nullptr;
-    bf16* wp = (bf16*)dev_alloc(ctx, nwt * 2, &tmp);
+    bf16* wp = (bf16*)dev_alloc(ctx, packed_weight_elems<bf16>(wl, Cout, Cin, KH, KW) * 2, &tmp);
     bf16* rb = e.res ? (bf16*)dev_alloc(ctx, npix_out * e.res_pitch * 2, &tmp) : nullptr;
-    yb = nchw ? nullptr : (bf16*)dev_alloc(ctx, npix_out * e.out_pitch * 2, &tmp);
-    if (!xb || (k4 && !s2d) || !wp || (e.res && !rb) || (!nchw && !yb)) rc = fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
+    bf16* yb = nchw ? nullptr : (bf16*)dev_alloc(ctx, npix_out * e.out_pitch * 2, &tmp);
+    if (!xb || !wp || (e.res && !rb) || (!nchw && !yb)) rc = fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
     if (!rc) {
       cast_f32_bf16_kernel<<<blocks(nin), 256, 0, st>>>(x, xb, nin);
       if (rb) cast_f32_bf16_kernel<<<blocks(npix_out * e.res_pitch), 256, 0, st>>>(e.res, rb, npix_out * e.res_pitch);
       if (yb) cast_f32_bf16_kernel<<<blocks(npix_out * e.out_pitch), 256, 0, st>>>(y, yb, npix_out * e.out_pitch);
-      if (k3 && up == 2) pack_tc_up_kernel<<<(unsigned)((nwt + 255) / 256), 256, 0, st>>>(w, wp, Cout, Cin);
-      else pack_tc_padded_kernel<<<(unsigned)((nwt + 255) / 256), 256, 0, st>>>(w, wp, Cout, Cout_pad, Cin, KH, KW);
-      const bf16* a_ptr = xb + e.in_off;
-      int a_pitch = e.in_pitch;
-      if (k4) {
-        launch_space_to_depth<bf16>(a_ptr, a_pitch, s2d, B, H, W, Cin, st);
-        a_ptr = s2d;
-        a_pitch = Cin;
-      }
+      pack_weight<bf16>(wl, w, wp, Cout, Cin, KH, KW, 1, st);
       if (rb) ep.res = rb + e.res_off;
-      d = tc_conv_create(a_ptr, a_pitch, B, Ha, Wa, Cin, planes, wp, Cout, ntaps, taps, nph, ep, nchw ? nullptr : yb + e.out_off,
-                         e.out_pitch, Ho, Wo, &terr, qsm ? TC_FLAG_QSOFTMAX : 0);
-      if (!d) rc = fail(ctx, IRSDE_ERR_INVALID, "tc_conv_create: " + terr);
+      rc = run_tc_conv<bf16>(ctx, "fused conv2d failed: ", xb + e.in_off, e.in_pitch, B, H, W, Cin, KH, up, wp, Cout, Ho, Wo, ep,
+                             nchw ? nullptr : yb + e.out_off, e.out_pitch, y, e.crop_h, e.crop_w, qsm ? TC_FLAG_QSOFTMAX : 0, info, st);
+      if (!rc && yb) cast_bf16_f32_kernel<<<blocks(npix_out * e.out_pitch), 256, 0, st>>>(yb, y, npix_out * e.out_pitch);
     }
   } else if (!rc) {
-    const long long nwt = (long long)((k3 && up == 2) ? 16 : KH * KW) * 2 * Cout_pad * Cin;
-    float* s2d = k4 ? (float*)dev_alloc(ctx, npix_in * Cin * 4, &tmp) : nullptr;
-    float* xsp = (float*)dev_alloc(ctx, 2 * npix_in * Cin * 4, &tmp);  // planes * Ha * Wa == H * W
-    float* wp = (float*)dev_alloc(ctx, nwt * 4, &tmp);
-    if ((k4 && !s2d) || !xsp || !wp) rc = fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
+    float* wp = (float*)dev_alloc(ctx, packed_weight_elems<float>(wl, Cout, Cin, KH, KW) * 4, &tmp);
+    if (!wp) rc = fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
     if (!rc) {
-      if (k3 && up == 2) pack_tc3_up_kernel<<<(unsigned)((nwt / 2 + 255) / 256), 256, 0, st>>>(w, wp, Cout, Cout_pad, Cin);
-      else pack_tc3_kernel<<<(unsigned)((nwt / 2 + 255) / 256), 256, 0, st>>>(w, wp, Cout, Cout_pad, Cin, KH, KW);
-      const float* a_src = x + e.in_off;
-      int a_pitch = e.in_pitch;
-      if (k4) {
-        launch_space_to_depth<float>(a_src, a_pitch, s2d, B, H, W, Cin, st);
-        a_src = s2d;
-        a_pitch = Cin;
-      }
-      launch_split_tf32(a_src, a_pitch, xsp, (long long)planes * B * Ha * Wa, Cin, st);
+      pack_weight<float>(wl, w, wp, Cout, Cin, KH, KW, 1, st);
       if (e.res) ep.res = e.res + e.res_off;
-      d = tc_conv_create_f32x3(xsp, B, Ha, Wa, Cin, planes, wp, Cout, ntaps, taps, nph, ep, nchw ? nullptr : y + e.out_off,
-                               e.out_pitch, Ho, Wo, &terr);
-      if (!d) rc = fail(ctx, IRSDE_ERR_INVALID, "tc_conv_create_f32x3: " + terr);
+      rc = run_tc_conv<float>(ctx, "fused conv2d failed: ", x + e.in_off, e.in_pitch, B, H, W, Cin, KH, up, wp, Cout, Ho, Wo, ep,
+                              nchw ? nullptr : y + e.out_off, e.out_pitch, y, e.crop_h, e.crop_w, 0, info, st);
     }
-  }
-  if (!rc && d) {
-    // as the plan's launch closures do: the table, its row pointer and the image stride arrive after the descriptor exists
-    if (e.ss) tc_conv_set_runtime(d, e.ss, t_dev, e.ss_img_stride);
-    if (nchw) tc_conv_set_out_nchw(d, y, e.crop_h, e.crop_w);
-    int q[4];
-    tc_conv_query(d, q);
-    for (int i = 0; i < 4; ++i) info[i] = q[i];
-    tc_conv_launch(d, st);
-    if (yb) cast_bf16_f32_kernel<<<blocks(npix_out * e.out_pitch), 256, 0, st>>>(yb, y, npix_out * e.out_pitch);
   }
   if (!rc) {
     ctx->launches += 4;
@@ -2418,7 +2315,6 @@ int irsde_conv2d_fused(irsde_ctx* ctx, int32_t engine, const float* x, const flo
   } else {
     cudaStreamSynchronize(st);  // conversions already queued read buffers freed below
   }
-  if (d) tc_conv_destroy(d);
   for (void* q : tmp) cudaFree(q);
   return rc;
 }
