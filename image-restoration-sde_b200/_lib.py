@@ -23,8 +23,10 @@ SYMBOLS = ["irsde_create", "irsde_create_ch_mult", "irsde_create_nafnet", "irsde
            "irsde_latent_decode", "irsde_tensor2img_u8", "irsde_img2tensor_u8", "irsde_sqerr_u8", "irsde_ssim_workspace", "irsde_ssim_u8", "irsde_destroy", "irsde_last_error", "irsde_version", "irsde_load_tensor",
            "irsde_finalize_weights", "irsde_set_schedule", "irsde_set_coeffs", "irsde_noise_fn", "irsde_step",
            "irsde_reverse", "irsde_noise_state", "irsde_noise_state_images", "irsde_set_image_base", "irsde_set_image_uids", "irsde_comm_unique_id", "irsde_comm_init", "irsde_broadcast_weights", "irsde_gather", "irsde_launch_count", "irsde_device_bytes", "irsde_conv2d", "irsde_profile_begin",
-           "irsde_profile_end", "irsde_profile_end_bytes", "irsde_conv2d_ex", "irsde_conv2d_fused", "irsde_plan_num_ops",
-           "irsde_plan_op_info", "irsde_trace_forward", "irsde_trim", "irsde_random_states"]
+           "irsde_profile_end", "irsde_profile_end_bytes", "irsde_conv2d_ex", "irsde_conv2d_fused", "irsde_layernorm",
+           "irsde_attention", "irsde_plan_num_ops", "irsde_plan_op_info", "irsde_trace_forward", "irsde_trim",
+           "irsde_random_states"]
+ATTN_LINEAR, ATTN_LINEAR_FOLD, ATTN_FULL = 0, 1, 2  # irsde_attention kinds
 
 
 class Config(ctypes.Structure):
@@ -43,6 +45,16 @@ class ConvEpilogue(ctypes.Structure):
                 ("in_pitch", ctypes.c_int32), ("in_off", ctypes.c_int32),
                 ("out_pitch", ctypes.c_int32), ("out_off", ctypes.c_int32),
                 ("crop_h", ctypes.c_int32), ("crop_w", ctypes.c_int32)]
+
+
+class LnArgs(ctypes.Structure):
+    """irsde_ln_args: gain, residual, time table and the views of one irsde_layernorm call (device pointers as ints)."""
+    _fields_ = [("g", ctypes.c_void_p), ("res", ctypes.c_void_p), ("ss", ctypes.c_void_p),
+                ("in_pitch", ctypes.c_int32), ("in_off", ctypes.c_int32),
+                ("res_pitch", ctypes.c_int32), ("res_off", ctypes.c_int32),
+                ("out_pitch", ctypes.c_int32), ("out_off", ctypes.c_int32),
+                ("ss_rows", ctypes.c_int32), ("ss_S", ctypes.c_int32), ("off_scale", ctypes.c_int32),
+                ("off_shift", ctypes.c_int32), ("ss_img_stride", ctypes.c_int32), ("t_row", ctypes.c_int32)]
 
 
 _lib = None
@@ -100,6 +112,10 @@ def load():
     L.irsde_conv2d_ex.restype = ctypes.c_int
     L.irsde_conv2d_fused.argtypes = [vp, i32, vp, vp, ctypes.POINTER(ConvEpilogue), vp] + [i32] * 10 + [ctypes.POINTER(i32), vp]
     L.irsde_conv2d_fused.restype = ctypes.c_int
+    L.irsde_layernorm.argtypes = [vp, i32, vp, ctypes.POINTER(LnArgs), vp, i32, i32, i32, ctypes.POINTER(i32), vp]
+    L.irsde_layernorm.restype = ctypes.c_int
+    L.irsde_attention.argtypes = [vp, i32, i32, vp, i32, i32, vp, i32, i32, vp, i32, vp, i32, i32, ctypes.POINTER(i32), vp]
+    L.irsde_attention.restype = ctypes.c_int
     L.irsde_plan_num_ops.argtypes = [vp, i32, i32, i32]
     L.irsde_plan_num_ops.restype = i32
     L.irsde_plan_op_info.argtypes = [vp, i32, i32, i32, i32, ctypes.c_char_p, i32, ctypes.POINTER(i32)]

@@ -257,6 +257,33 @@ __global__ void layernorm_scalar_kernel(const T* __restrict__ x, int x_pitch, co
   }
 }
 
+// The LayerNorm kernel launch_layernorm runs for these operands.  `lpp` lanes share a pixel: the largest power of two <= 32
+// that does not exceed the row's vectors; `per_lane` vectors of the row land on each lane.  16-byte vectors need C, every
+// pitch and every pointer aligned to 16 bytes, and at most 16 vectors per lane; otherwise the scalar kernel runs.  The
+// geo kernel takes the rows it has an instantiation for (C == N * LPP * MAXV exactly, LPP >= 8), the vec kernel the rest.
+template <typename T>
+LnPick ln_pick(int C, long long npix, int x_pitch, int res_pitch, int out_pitch, const void* x, const float* g, const void* res,
+               const void* out) {
+  constexpr int N = VecIO<T>::N;
+  const bool vec_ok = C % N == 0 && x_pitch % N == 0 && out_pitch % N == 0 && ((uintptr_t)x % 16 == 0) &&
+                      ((uintptr_t)out % 16 == 0) && ((uintptr_t)g % 16 == 0) &&
+                      (!res || (res_pitch % N == 0 && (uintptr_t)res % 16 == 0));
+  const int nvec = C / N;
+  int lpp = 1;
+  while (lpp * 2 <= 32 && lpp * 2 <= nvec) lpp *= 2;
+  const int per_lane = vec_ok ? (nvec + lpp - 1) / lpp : 999;
+  if (!vec_ok || per_lane > 16) return LnPick{LN_SCALAR, 0, 0, 0};
+  if (nvec == lpp * per_lane && (per_lane & (per_lane - 1)) == 0 && lpp >= 8 && npix > 0) {
+    // exact geometry.  Two pixels per lane group while the row fits 2 vectors per lane.
+    if (per_lane == 1 || (lpp == 32 && (per_lane <= 4 || (per_lane == 8 && sizeof(T) == 4))))
+      return LnPick{LN_GEO, per_lane, lpp, per_lane <= 2 ? 2 : 1};
+  }
+  const int mv = per_lane <= 1 ? 1 : per_lane <= 2 ? 2 : per_lane <= 4 ? 4 : per_lane <= 8 ? 8 : 16;
+  return LnPick{LN_VEC, mv, lpp, 1};
+}
+template LnPick ln_pick<float>(int, long long, int, int, int, const void*, const float*, const void*, const void*);
+template LnPick ln_pick<bf16>(int, long long, int, int, int, const void*, const float*, const void*, const void*);
+
 template <typename T>
 void launch_layernorm(const T* x, int x_pitch, const float* g, const T* res, int res_pitch, T* out, int out_pitch,
                       long long npix, int C, cudaStream_t st, const LnMod* modp) {
@@ -264,42 +291,35 @@ void launch_layernorm(const T* x, int x_pitch, const float* g, const T* res, int
   memset(&mod, 0, sizeof mod);
   if (modp) mod = *modp;
   if (mod.pix_per_img <= 0) mod.pix_per_img = 1;
-  constexpr int N = VecIO<T>::N;
-  bool vec_ok = C % N == 0 && x_pitch % N == 0 && out_pitch % N == 0 && ((uintptr_t)x % 16 == 0) &&
-                ((uintptr_t)out % 16 == 0) && ((uintptr_t)g % 16 == 0) &&
-                (!res || (res_pitch % N == 0 && (uintptr_t)res % 16 == 0));
-  int nvec = C / N;
-  int lpp = 1;
-  while (lpp * 2 <= 32 && lpp * 2 <= nvec) lpp *= 2;
-  int per_lane = vec_ok ? (nvec + lpp - 1) / lpp : 999;
-  if (!vec_ok || per_lane > 16) {
-    const int warps = 8;
+  const LnPick k = ln_pick<T>(C, npix, x_pitch, res_pitch, out_pitch, x, g, res, out);
+  const int warps = 8;
+  if (k.kind == LN_SCALAR) {
     pdl_launch(layernorm_scalar_kernel<T>, (unsigned)((npix + warps - 1) / warps), warps * 32, 0, st, x, x_pitch, g, res, res_pitch,
                                                                                             out, out_pitch, npix, C, mod);
     return;
   }
-  const int warps = 8;
+  const int lpp = k.lpp;
   long long pix_per_block = (long long)warps * (32 / lpp);
-  if (nvec == lpp * per_lane && (per_lane & (per_lane - 1)) == 0 && lpp >= 8 && npix > 0) {
-    // exact geometry: C == N * LPP * MAXV.  Two pixels per lane group while the row fits 2 vectors per lane.
+  if (k.kind == LN_GEO) {
 #define LN_GEO(MV, LP, PPX)                                                                                              \
   pdl_launch(layernorm_geo_kernel<T, MV, LP, PPX>, (unsigned)((npix + pix_per_block * PPX - 1) / (pix_per_block * PPX)),   \
              warps * 32, 0, st, x, x_pitch, g, res, res_pitch, out, out_pitch, npix, C, 1.0f / (float)C, mod)
-    if (lpp == 8 && per_lane == 1) { LN_GEO(1, 8, 2); return; }
-    if (lpp == 16 && per_lane == 1) { LN_GEO(1, 16, 2); return; }
-    if (lpp == 32 && per_lane == 1) { LN_GEO(1, 32, 2); return; }
-    if (lpp == 32 && per_lane == 2) { LN_GEO(2, 32, 2); return; }
-    if (lpp == 32 && per_lane == 4) { LN_GEO(4, 32, 1); return; }
-    if (lpp == 32 && per_lane == 8 && sizeof(T) == 4) { LN_GEO(8, 32, 1); return; }
+    if (lpp == 8) LN_GEO(1, 8, 2);
+    else if (lpp == 16) LN_GEO(1, 16, 2);
+    else if (k.maxv == 1) LN_GEO(1, 32, 2);
+    else if (k.maxv == 2) LN_GEO(2, 32, 2);
+    else if (k.maxv == 4) LN_GEO(4, 32, 1);
+    else if constexpr (sizeof(T) == 4) LN_GEO(8, 32, 1);
 #undef LN_GEO
+    return;
   }
   unsigned grid = (unsigned)((npix + pix_per_block - 1) / pix_per_block);
 #define LN_LAUNCH(MV) \
   pdl_launch(layernorm_vec_kernel<T, MV>, grid, warps * 32, 0, st, x, x_pitch, g, res, res_pitch, out, out_pitch, npix, C, lpp, mod)
-  if (per_lane <= 1) LN_LAUNCH(1);
-  else if (per_lane <= 2) LN_LAUNCH(2);
-  else if (per_lane <= 4) LN_LAUNCH(4);
-  else if (per_lane <= 8) LN_LAUNCH(8);
+  if (k.maxv == 1) LN_LAUNCH(1);
+  else if (k.maxv == 2) LN_LAUNCH(2);
+  else if (k.maxv == 4) LN_LAUNCH(4);
+  else if (k.maxv == 8) LN_LAUNCH(8);
   else LN_LAUNCH(16);
 #undef LN_LAUNCH
 }
@@ -321,7 +341,7 @@ static const int LA_REC = 4 * (64 + 1024);  // floats per partial record (4 head
 static const int LA_MAXBLK = 64;            // partial records per image
 
 static int la_blocks_per_image(int B, int N) {
-  int nchunks = (N + LA_PIX - 1) / LA_PIX;
+  const int nchunks = (N + LA_PIX - 1) / LA_PIX;
   // The partition must not depend on the batch size: a batch-sharded run has to reproduce the unsharded one bit for
   // bit (fp32 summation order).  37 blocks per image = one full wave of 2 resident blocks/SM at 8 images per GPU.
   (void)B;
@@ -331,6 +351,16 @@ static int la_blocks_per_image(int B, int N) {
   return nblk < 1 ? 1 : nblk;
 }
 size_t linattn_partial_floats(int B, int N) { return (size_t)B * LA_MAXBLK * LA_REC; }
+void linattn_partition(int B, int N, int* nblk, int* nchunks) {
+  *nchunks = (N + LA_PIX - 1) / LA_PIX;
+  *nblk = la_blocks_per_image(B, N);
+}
+// Every linear-attention kernel moves qkv and hidden in 16-byte vectors: both views must start on 16 bytes and their pitches
+// be multiples of 16 bytes.  hidden may be null (passes A + B only).
+bool linattn_views_ok(const void* qkv, int qkv_pitch, const void* hidden, int hid_pitch, size_t elem) {
+  const int vec = (int)(16 / elem);
+  return (uintptr_t)qkv % 16 == 0 && qkv_pitch % vec == 0 && (!hidden || ((uintptr_t)hidden % 16 == 0 && hid_pitch % vec == 0));
+}
 
 template <typename T>
 __global__ void __launch_bounds__(256) la_kv_kernel(const T* __restrict__ qkv, int pitch, float* __restrict__ part,
@@ -729,37 +759,37 @@ void launch_la_kv<float>(const float* qkv, int qkv_pitch, float* partial, int B,
 template <>
 void launch_la_kv<bf16>(const bf16* qkv, int qkv_pitch, float* partial, int B, int N, int nchunks, int nblk, size_t smem,
                         cudaStream_t st) {
-  if (qkv_pitch % 8 == 0 && ((uintptr_t)qkv % 16) == 0)
-    pdl_launch(la_kv_mma_kernel, dim3(nblk, B), 256, LAM_SMEM, st, qkv, qkv_pitch, partial, N, nchunks, nblk);
-  else
-    pdl_launch(la_kv_kernel<bf16>, dim3(nblk, B), 256, smem, st, qkv, qkv_pitch, partial, N, nchunks, nblk);
+  pdl_launch(la_kv_mma_kernel, dim3(nblk, B), 256, LAM_SMEM, st, qkv, qkv_pitch, partial, N, nchunks, nblk);
 }
 
 template <typename T>
-void launch_linattn_ctx(const T* qkv, int qkv_pitch, float* partial, float* ctx, int B, int N, cudaStream_t st) {
-  const int nchunks = (N + LA_PIX - 1) / LA_PIX;
-  const int nblk = la_blocks_per_image(B, N);
+bool launch_linattn_ctx(const T* qkv, int qkv_pitch, float* partial, float* ctx, int B, int N, cudaStream_t st) {
+  if (!linattn_views_ok(qkv, qkv_pitch, nullptr, 0, sizeof(T))) return false;
+  int nblk, nchunks;
+  linattn_partition(B, N, &nblk, &nchunks);
   const size_t smem = (size_t)(2 * LA_PIX * 128 + 128 * 5) * sizeof(float);
   if (!g_la_attr_done) {
     cudaFuncSetAttribute(la_kv_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    cudaFuncSetAttribute(la_kv_kernel<bf16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     cudaFuncSetAttribute(la_kv_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LAM_SMEM);
     g_la_attr_done = true;
   }
   launch_la_kv<T>(qkv, qkv_pitch, partial, B, N, nchunks, nblk, smem, st);
   pdl_launch(la_combine8_kernel, B * 4 * 8, 256, 0, st, partial, ctx, N, nblk);
+  return true;
 }
-template void launch_linattn_ctx<float>(const float*, int, float*, float*, int, int, cudaStream_t);
-template void launch_linattn_ctx<bf16>(const bf16*, int, float*, float*, int, int, cudaStream_t);
+template bool launch_linattn_ctx<float>(const float*, int, float*, float*, int, int, cudaStream_t);
+template bool launch_linattn_ctx<bf16>(const bf16*, int, float*, float*, int, int, cudaStream_t);
 
 template <typename T>
-void launch_linattn(const T* qkv, int qkv_pitch, float* partial, float* ctx, T* hidden, int hid_pitch, int B, int N,
+bool launch_linattn(const T* qkv, int qkv_pitch, float* partial, float* ctx, T* hidden, int hid_pitch, int B, int N,
                     cudaStream_t st) {
+  if (!linattn_views_ok(qkv, qkv_pitch, hidden, hid_pitch, sizeof(T))) return false;
   launch_linattn_ctx<T>(qkv, qkv_pitch, partial, ctx, B, N, st);
   pdl_launch(la_out_kernel<T>, dim3((N + 63) / 64, B), 256, 0, st, qkv, qkv_pitch, ctx, hidden, hid_pitch, N);
+  return true;
 }
-template void launch_linattn<float>(const float*, int, float*, float*, float*, int, int, int, cudaStream_t);
-template void launch_linattn<bf16>(const bf16*, int, float*, float*, bf16*, int, int, int, cudaStream_t);
+template bool launch_linattn<float>(const float*, int, float*, float*, float*, int, int, int, cudaStream_t);
+template bool launch_linattn<bf16>(const bf16*, int, float*, float*, bf16*, int, int, int, cudaStream_t);
 
 // Fold the per-image context into the to_out 1x1 weights so that pass C and the to_out conv become ONE
 // per-image-weight GEMM on the (head-softmaxed) q:  y[px][c] = sum_k qs[px][k] * Mb[b][c][k],
@@ -1037,13 +1067,24 @@ __global__ void __launch_bounds__(128) fullattn_mma_kernel(const bf16* __restric
   }
 }
 
+// fullattn_mma_kernel reads qkv in 16-byte vectors and writes hidden in bf16 pairs; fullattn_kernel moves single elements
+// and takes any view.
+template <typename T>
+FullAttnKernel fullattn_pick(const T* qkv, int qkv_pitch, const T* hidden, int hid_pitch) {
+  if (sizeof(T) == 2 && qkv_pitch % 8 == 0 && hid_pitch % 2 == 0 && ((uintptr_t)qkv % 16) == 0 && ((uintptr_t)hidden % 4) == 0)
+    return FA_MMA;
+  return FA_SCALAR;
+}
+template FullAttnKernel fullattn_pick<float>(const float*, int, const float*, int);
+template FullAttnKernel fullattn_pick<bf16>(const bf16*, int, const bf16*, int);
+
 template <typename T>
 void launch_fullattn(const T* qkv, int qkv_pitch, T* hidden, int hid_pitch, int B, int N, cudaStream_t st) {
   pdl_launch(fullattn_kernel<T>, dim3((N + 127) / 128, B * 4), 128, 0, st, qkv, qkv_pitch, hidden, hid_pitch, N);
 }
 template <>
 void launch_fullattn<bf16>(const bf16* qkv, int qkv_pitch, bf16* hidden, int hid_pitch, int B, int N, cudaStream_t st) {
-  if (qkv_pitch % 8 == 0 && hid_pitch % 2 == 0 && ((uintptr_t)qkv % 16) == 0 && ((uintptr_t)hidden % 4) == 0)
+  if (fullattn_pick<bf16>(qkv, qkv_pitch, hidden, hid_pitch) == FA_MMA)
     pdl_launch(fullattn_mma_kernel, dim3((N + FA_Q - 1) / FA_Q, B * 4), 128, 0, st, qkv, qkv_pitch, hidden, hid_pitch, N);
   else
     pdl_launch(fullattn_kernel<bf16>, dim3((N + 127) / 128, B * 4), 128, 0, st, qkv, qkv_pitch, hidden, hid_pitch, N);

@@ -115,6 +115,15 @@ struct LnMod {
 template <typename T>
 void launch_layernorm(const T* x, int x_pitch, const float* g, const T* res, int res_pitch, T* out, int out_pitch,
                       long long npix, int C, cudaStream_t st, const LnMod* mod = nullptr);
+// the kernel launch_layernorm runs: layernorm_scalar_kernel, layernorm_vec_kernel<MAXV> (lpp lanes per pixel) or
+// layernorm_geo_kernel<MAXV, LPP, PP>; res may be null
+enum { LN_SCALAR = 0, LN_VEC = 1, LN_GEO = 2 };
+struct LnPick {
+  int kind, maxv, lpp, pp;
+};
+template <typename T>
+LnPick ln_pick(int C, long long npix, int x_pitch, int res_pitch, int out_pitch, const void* x, const float* g, const void* res,
+               const void* out);
 // ---- NAFNet kernels (nafnet.cu)
 int dwgate_chunks(int H, int W);
 template <typename T>
@@ -136,17 +145,25 @@ void launch_naf_time_gate(const float* times, int rows, int width, const float* 
                           const float* b2, float* tgate, cudaStream_t st);
 // table[r][j] = dot(wall[j][0..td), tvec[r][0..td)) + ball[j]
 void launch_time_rows(const float* tvec, int rows, int td, const float* wall, const float* ball, int S, float* table, cudaStream_t st);
-// linear attention: qkv [B,N,384] -> ctx [B,4,32,32] (fp32) -> hidden [B,N,128]
+// linear attention: qkv [B,N,384] -> ctx [B,4,32,32] (fp32) -> hidden [B,N,128].  The launchers launch nothing and return
+// false when linattn_views_ok rejects the views (elem = sizeof(T); hidden may be null).
+bool linattn_views_ok(const void* qkv, int qkv_pitch, const void* hidden, int hid_pitch, size_t elem);
 template <typename T>
-void launch_linattn(const T* qkv, int qkv_pitch, float* partial, float* ctx, T* hidden, int hid_pitch, int B, int N,
+bool launch_linattn(const T* qkv, int qkv_pitch, float* partial, float* ctx, T* hidden, int hid_pitch, int B, int N,
                     cudaStream_t st);
 size_t linattn_partial_floats(int B, int N);
+// pass A's partition: nchunks chunks of 64 pixels per image, spread over nblk blocks per image (independent of B)
+void linattn_partition(int B, int N, int* nblk, int* nchunks);
 // passes A+B only (k,v -> ctx); and the fold of ctx into the to_out weights:
 //   Mb[b][c][h*32+d] = sum_e Wout[c][h*32+e] * ctx[b][h][d][e]   (bf16, K-major rows of 128)
 template <typename T>
-void launch_linattn_ctx(const T* qkv, int qkv_pitch, float* partial, float* ctx, int B, int N, cudaStream_t st);
+bool launch_linattn_ctx(const T* qkv, int qkv_pitch, float* partial, float* ctx, int B, int N, cudaStream_t st);
 void launch_la_fold(const float* ctx, const float* wout, bf16* Mb, int B, int C, cudaStream_t st);
-// full softmax attention (denoising-sde mid_attn): qkv [B,N,384] -> hidden [B,N,128]
+// full softmax attention (denoising-sde mid_attn): qkv [B,N,384] -> hidden [B,N,128]; fullattn_pick is the kernel
+// launch_fullattn runs (FA_MMA: bf16 only)
+enum FullAttnKernel { FA_SCALAR = 0, FA_MMA = 1 };
+template <typename T>
+FullAttnKernel fullattn_pick(const T* qkv, int qkv_pitch, const T* hidden, int hid_pitch);
 template <typename T>
 void launch_fullattn(const T* qkv, int qkv_pitch, T* hidden, int hid_pitch, int B, int N, cudaStream_t st);
 // time embedding: times[rows] -> table[rows][S]

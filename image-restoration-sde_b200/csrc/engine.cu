@@ -723,6 +723,7 @@ struct Builder {
         conv(pre + "fn.fn.to_qkv.weight", V{xn, C, C}, H, W, 1, 1, 0, 1, nullptr, "", 0, nullptr, V{qkv, 384, 384}, 384, nullptr,
              TC_FLAG_QSOFTMAX);
         release(xn);
+        if (!linattn_views_ok(qkv, 384, nullptr, 0, sizeof(T))) { ok = false; err = "linear attention: qkv view not 16-byte aligned"; }
         plan->ops.push_back(OpRec{CAT_ATTN, 0.0, [=](Plan*, cudaStream_t st) {
           launch_linattn_ctx<T>(qkv, 384, la_partial, la_ctx, B, N, st);
           c->launches += 2;
@@ -768,6 +769,7 @@ struct Builder {
       std::string bn = pre + "fn.fn.to_out.bias";
       conv(pre + "fn.fn.to_out.weight", V{hid, 128, 128}, H, W, 1, 1, 0, 1, bn.c_str(), "", 0, &in, out, C);
     } else {
+      if (!linattn_views_ok(qkv, 384, hid, 128, sizeof(T))) { ok = false; err = "linear attention: views not 16-byte aligned"; }
       plan->ops.push_back(OpRec{CAT_ATTN, 0.0, [=](Plan*, cudaStream_t st) {
         launch_linattn<T>(qkv, 384, la_partial, la_ctx, hid, 128, B, N, st);
         c->launches += 3;
@@ -2317,6 +2319,166 @@ int irsde_conv2d_fused(irsde_ctx* ctx, int32_t engine, const float* x, const flo
   }
   for (void* q : tmp) cudaFree(q);
   return rc;
+}
+
+// ---- one LayerNorm / attention op outside a plan ------------------------------------------------------------------
+static unsigned cast_blocks(long long n) { return (unsigned)std::min<long long>((n + 255) / 256, 65536); }
+
+// Waits for the stream, turns a launch error into the context's error and frees the scratch.
+static int finish_op(irsde_ctx* ctx, int rc, const char* what, cudaStream_t st, std::vector<void*>& tmp) {
+  cudaError_t ce = cudaStreamSynchronize(st);
+  if (ce == cudaSuccess) ce = cudaGetLastError();
+  if (!rc && ce != cudaSuccess) rc = fail(ctx, IRSDE_ERR_CUDA, std::string(what) + cudaGetErrorString(ce));
+  for (void* q : tmp) cudaFree(q);
+  return rc;
+}
+
+int irsde_layernorm(irsde_ctx* ctx, int32_t precision, const float* x, const irsde_ln_args* args, float* y, int32_t B, int32_t N,
+                    int32_t C, int32_t* info, void* stream) {
+  // ---- everything is validated here, before the first allocation or launch
+  if (!ctx || !x || !y || !args || !args->g) return fail(ctx, IRSDE_ERR_INVALID, "null argument");
+  const irsde_ln_args& a = *args;
+  if (precision < IRSDE_PREC_FP32 || precision > IRSDE_PREC_FP32X3) return fail(ctx, IRSDE_ERR_INVALID, "bad precision");
+  if (B < 1 || N < 1 || C < 1) return fail(ctx, IRSDE_ERR_INVALID, "bad shape");
+  auto view_ok = [&](int pitch, int off) { return off >= 0 && (long long)off + C <= pitch; };
+  if (!view_ok(a.in_pitch, a.in_off)) return fail(ctx, IRSDE_ERR_INVALID, "input view outside its pitch");
+  if (!view_ok(a.out_pitch, a.out_off)) return fail(ctx, IRSDE_ERR_INVALID, "output view outside its pitch");
+  if (a.res && !view_ok(a.res_pitch, a.res_off)) return fail(ctx, IRSDE_ERR_INVALID, "residual view outside its pitch");
+  if (a.ss) {
+    if (a.t_row < 0 || a.ss_img_stride < 0 || (long long)a.t_row + (long long)(B - 1) * a.ss_img_stride >= a.ss_rows)
+      return fail(ctx, IRSDE_ERR_INVALID, "time-modulation row outside the table");
+    if (a.off_scale < 0 || a.off_shift < 0 || (long long)a.off_scale + C > a.ss_S || (long long)a.off_shift + C > a.ss_S)
+      return fail(ctx, IRSDE_ERR_INVALID, "scale / shift columns outside the table row");
+  }
+  int32_t info_local[4];
+  if (!info) info = info_local;
+  info[0] = info[1] = info[2] = info[3] = 0;
+
+  cudaSetDevice(ctx->cfg.device);
+  cudaStream_t st = (cudaStream_t)stream;
+  const long long npix = (long long)B * N;
+  std::vector<void*> tmp;
+  int rc = IRSDE_OK;
+  int* t_dev = (int*)dev_alloc(ctx, sizeof(int), &tmp);
+  if (!t_dev) rc = fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
+  if (!rc) cudaMemcpyAsync(t_dev, &a.t_row, sizeof(int), cudaMemcpyHostToDevice, st);
+  LnMod m;
+  memset(&m, 0, sizeof m);
+  if (a.ss) {
+    m.ss = a.ss; m.t_ptr = t_dev; m.S = a.ss_S; m.off_scale = a.off_scale; m.off_shift = a.off_shift;
+    m.img_stride = a.ss_img_stride;
+  }
+  m.pix_per_img = N;
+  LnPick k{};
+  if (!rc && precision == IRSDE_PREC_BF16) {
+    const long long nx = npix * a.in_pitch, ny = npix * a.out_pitch, nr = a.res ? npix * a.res_pitch : 0;
+    bf16* xb = (bf16*)dev_alloc(ctx, nx * 2, &tmp);
+    bf16* yb = (bf16*)dev_alloc(ctx, ny * 2, &tmp);
+    bf16* rb = a.res ? (bf16*)dev_alloc(ctx, nr * 2, &tmp) : nullptr;
+    if (!xb || !yb || (a.res && !rb)) rc = fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
+    if (!rc) {
+      cast_f32_bf16_kernel<<<cast_blocks(nx), 256, 0, st>>>(x, xb, nx);
+      cast_f32_bf16_kernel<<<cast_blocks(ny), 256, 0, st>>>(y, yb, ny);
+      if (rb) cast_f32_bf16_kernel<<<cast_blocks(nr), 256, 0, st>>>(a.res, rb, nr);
+      const bf16 *xv = xb + a.in_off, *rv = rb ? rb + a.res_off : nullptr;
+      bf16* yv = yb + a.out_off;
+      k = ln_pick<bf16>(C, npix, a.in_pitch, a.res_pitch, a.out_pitch, xv, a.g, rv, yv);
+      launch_layernorm<bf16>(xv, a.in_pitch, a.g, rv, a.res_pitch, yv, a.out_pitch, npix, C, st, &m);
+      cast_bf16_f32_kernel<<<cast_blocks(ny), 256, 0, st>>>(yb, y, ny);
+    }
+  } else if (!rc) {
+    const float *xv = x + a.in_off, *rv = a.res ? a.res + a.res_off : nullptr;
+    float* yv = y + a.out_off;
+    k = ln_pick<float>(C, npix, a.in_pitch, a.res_pitch, a.out_pitch, xv, a.g, rv, yv);
+    launch_layernorm<float>(xv, a.in_pitch, a.g, rv, a.res_pitch, yv, a.out_pitch, npix, C, st, &m);
+  }
+  if (!rc) {
+    info[0] = k.kind; info[1] = k.maxv; info[2] = k.lpp; info[3] = k.pp;
+    ctx->launches++;
+  }
+  return finish_op(ctx, rc, "layernorm failed: ", st, tmp);
+}
+
+int irsde_attention(irsde_ctx* ctx, int32_t precision, int32_t kind, const float* qkv, int32_t qkv_pitch, int32_t qkv_off,
+                    float* out, int32_t out_pitch, int32_t out_off, const float* wout, int32_t Cout, float* ctx_out, int32_t B,
+                    int32_t N, int32_t* info, void* stream) {
+  // ---- everything is validated here, before the first allocation or launch
+  if (!ctx || !qkv || !out) return fail(ctx, IRSDE_ERR_INVALID, "null argument");
+  if (precision < IRSDE_PREC_FP32 || precision > IRSDE_PREC_FP32X3) return fail(ctx, IRSDE_ERR_INVALID, "bad precision");
+  if (kind < IRSDE_ATTN_LINEAR || kind > IRSDE_ATTN_FULL) return fail(ctx, IRSDE_ERR_INVALID, "unknown attention kind");
+  const bool bf = precision == IRSDE_PREC_BF16, lin = kind != IRSDE_ATTN_FULL, fold = kind == IRSDE_ATTN_LINEAR_FOLD;
+  if (fold && !bf) return fail(ctx, IRSDE_ERR_UNSUPPORTED, "the folded linear attention is the bf16 path");
+  if (B < 1 || B > 16383 || N < 1) return fail(ctx, IRSDE_ERR_INVALID, "bad shape");
+  if (lin && !ctx_out) return fail(ctx, IRSDE_ERR_INVALID, "linear attention needs ctx_out");
+  if (fold && (!wout || Cout < 1 || ((uintptr_t)wout & 15)))
+    return fail(ctx, IRSDE_ERR_INVALID, "the fold needs 16-byte aligned to_out weights [Cout][128], Cout >= 1");
+  if (qkv_off < 0 || (long long)qkv_off + 384 > qkv_pitch) return fail(ctx, IRSDE_ERR_INVALID, "qkv view outside its pitch");
+  if (!fold && (out_off < 0 || (long long)out_off + 128 > out_pitch))
+    return fail(ctx, IRSDE_ERR_INVALID, "hidden view outside its pitch");
+  // the views the launchers get: the caller's buffers (fp32), or bf16 copies that start on 256 bytes
+  const size_t elem = bf ? 2 : 4;
+  auto at = [&](const float* base, int off) { return (const void*)((bf ? 0 : (uintptr_t)base) + (uintptr_t)off * elem); };
+  if (lin && !linattn_views_ok(at(qkv, qkv_off), qkv_pitch, fold ? nullptr : at(out, out_off), out_pitch, elem))
+    return fail(ctx, IRSDE_ERR_INVALID, "linear attention: views must start on 16 bytes and pitches be multiples of 16 bytes");
+  int32_t info_local[4];
+  if (!info) info = info_local;
+  info[0] = info[1] = info[2] = info[3] = 0;
+
+  cudaSetDevice(ctx->cfg.device);
+  cudaStream_t st = (cudaStream_t)stream;
+  const long long npix = (long long)B * N;
+  std::vector<void*> tmp;
+  int rc = IRSDE_OK;
+  float* part = lin ? (float*)dev_alloc(ctx, linattn_partial_floats(B, N) * sizeof(float), &tmp) : nullptr;
+  float* cx = lin ? (float*)dev_alloc(ctx, (size_t)B * 4096 * sizeof(float), &tmp) : nullptr;
+  if (lin && (!part || !cx)) rc = fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
+  bool launched = false;
+  int kern = 0;
+  if (!rc && bf) {
+    const long long nq = npix * qkv_pitch, no = fold ? (long long)B * Cout * 128 : npix * out_pitch;
+    bf16* qb = (bf16*)dev_alloc(ctx, nq * 2, &tmp);
+    bf16* ob = (bf16*)dev_alloc(ctx, no * 2, &tmp);
+    if (!qb || !ob) rc = fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
+    if (!rc) {
+      cast_f32_bf16_kernel<<<cast_blocks(nq), 256, 0, st>>>(qkv, qb, nq);
+      if (!fold) cast_f32_bf16_kernel<<<cast_blocks(no), 256, 0, st>>>(out, ob, no);
+      const bf16* qv = qb + qkv_off;
+      if (kind == IRSDE_ATTN_LINEAR) {
+        kern = 2;
+        launched = launch_linattn<bf16>(qv, qkv_pitch, part, cx, ob + out_off, out_pitch, B, N, st);
+      } else if (fold) {
+        kern = 2;
+        launched = launch_linattn_ctx<bf16>(qv, qkv_pitch, part, cx, B, N, st);
+        if (launched) launch_la_fold(cx, wout, ob, B, Cout, st);
+      } else {
+        kern = fullattn_pick<bf16>(qv, qkv_pitch, ob + out_off, out_pitch) == FA_MMA ? 4 : 3;
+        launch_fullattn<bf16>(qv, qkv_pitch, ob + out_off, out_pitch, B, N, st);
+        launched = true;
+      }
+      if (launched) cast_bf16_f32_kernel<<<cast_blocks(no), 256, 0, st>>>(ob, out, no);
+    }
+  } else if (!rc) {
+    if (lin) {
+      kern = 1;
+      launched = launch_linattn<float>(qkv + qkv_off, qkv_pitch, part, cx, out + out_off, out_pitch, B, N, st);
+    } else {
+      kern = 3;
+      launch_fullattn<float>(qkv + qkv_off, qkv_pitch, out + out_off, out_pitch, B, N, st);
+      launched = true;
+    }
+  }
+  if (!rc && !launched) rc = fail(ctx, IRSDE_ERR_INVALID, "the linear-attention launcher refused the views");
+  if (!rc) {
+    if (lin) {
+      int nblk, nchunks;
+      linattn_partition(B, N, &nblk, &nchunks);
+      info[1] = nblk; info[2] = nchunks;
+      cudaMemcpyAsync(ctx_out, cx, (size_t)B * 4096 * sizeof(float), cudaMemcpyDeviceToDevice, st);
+    }
+    info[0] = kern;
+    ctx->launches += lin ? 3 : 1;
+  }
+  return finish_op(ctx, rc, "attention failed: ", st, tmp);
 }
 
 // ---- image conversion / metrics (stateless) ----------------------------------------------------------------

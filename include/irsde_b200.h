@@ -241,6 +241,51 @@ int irsde_conv2d_fused(irsde_ctx* ctx, int32_t engine, const float* x, const flo
                        int32_t B, int32_t Cin, int32_t H, int32_t W, int32_t Cout, int32_t KH, int32_t KW, int32_t stride,
                        int32_t pad, int32_t upsample, int32_t* info, void* stream);
 
+/* One channel LayerNorm of the network (module_util.py:70-79; biased variance, eps 1e-5), with the optional NAFBlock time
+ * modulation (DenoisingNAFNet_arch.py:62-63,75-76) and residual: y = ln(x) * g [* (scale + 1) + shift] [+ res].
+ * x, res and y are fp32 NHWC buffers of B*N pixels, each read or written through a (pitch, channel offset) view; views need
+ * not be 16-byte aligned. */
+typedef struct {
+  const float* g;          /* gain [C] */
+  const float* res;        /* residual buffer [B*N][res_pitch] read at channels res_off.., or NULL */
+  const float* ss;         /* time-modulation table [ss_rows][ss_S] or NULL: image b uses row t_row + b * ss_img_stride, */
+                           /* scale = row[off_scale + c], shift = row[off_shift + c] */
+  int32_t in_pitch, in_off;
+  int32_t res_pitch, res_off;
+  int32_t out_pitch, out_off;
+  int32_t ss_rows, ss_S, off_scale, off_shift, ss_img_stride, t_row;
+} irsde_ln_args;
+
+/* precision 0 (fp32; IRSDE_PREC_FP32X3 runs the same kernels) or 1 (bf16).  y is read and written: for bf16 the whole x, res
+ * and y buffers are converted to bf16, the kernel writes y's slice, and y is converted back, so an element outside the slice
+ * comes back unchanged when bf16 represents it.  Every view, table row and size is checked on the host before anything is
+ * allocated or launched.  info (or NULL) receives {kind, MAXV, LPP, PP} of the kernel that ran: kind 0 =
+ * layernorm_scalar_kernel (MAXV = LPP = PP = 0), 1 = layernorm_vec_kernel<MAXV> (LPP lanes per pixel, PP = 1),
+ * 2 = layernorm_geo_kernel<MAXV, LPP, PP>. */
+int irsde_layernorm(irsde_ctx* ctx, int32_t precision, const float* x, const irsde_ln_args* args, float* y, int32_t B, int32_t N,
+                    int32_t C, int32_t* info, void* stream);
+
+/* One attention core of the network on qkv = to_qkv's output, an fp32 NHWC buffer [B*N][qkv_pitch] whose channels
+ * qkv_off .. qkv_off+383 are q | k | v (4 heads of 32).
+ *   IRSDE_ATTN_LINEAR       LinearAttention (module_util.py:163-177): ctx_out = fp32 [B][4][32][32] context
+ *                           (ctx[b][h][d][e] = sum_n softmax_n(k)[d,n] v[e,n] / N), out = the 128 hidden channels, written
+ *                           through the view (out_pitch, out_off) of an fp32 [B*N][out_pitch] buffer;
+ *   IRSDE_ATTN_LINEAR_FOLD  (bf16 only) the same context, folded into the to_out weights wout fp32 [Cout][128]:
+ *                           out = fp32 [B][Cout][128], Mb[b][c][h*32+d] = sum_e wout[c][h*32+e] ctx[b][h][d][e]
+ *                           (module_util.py:176-178 re-associated); out_pitch / out_off are ignored;
+ *   IRSDE_ATTN_FULL         softmax Attention (module_util.py:192-204): out = hidden through (out_pitch, out_off); ctx_out
+ *                           is not used.
+ * Buffers are converted as in irsde_layernorm.  The linear kinds need views that start on 16 bytes of the storage type and
+ * pitches that are multiples of 16 bytes of it.  info (or NULL) receives {kernel, nblk, nchunks, 0}: kernel 1 =
+ * la_kv_kernel<float>, 2 = la_kv_mma_kernel, 3 = fullattn_kernel, 4 = fullattn_mma_kernel; nblk blocks per image
+ * share nchunks chunks of 64 pixels in the k,v pass (0 for IRSDE_ATTN_FULL). */
+#define IRSDE_ATTN_LINEAR 0
+#define IRSDE_ATTN_LINEAR_FOLD 1
+#define IRSDE_ATTN_FULL 2
+int irsde_attention(irsde_ctx* ctx, int32_t precision, int32_t kind, const float* qkv, int32_t qkv_pitch, int32_t qkv_off,
+                    float* out, int32_t out_pitch, int32_t out_off, const float* wout, int32_t Cout, float* ctx_out, int32_t B,
+                    int32_t N, int32_t* info, void* stream);
+
 /* ---- launch-plan introspection (parity instrumentation: per-layer comparison with the oracle) ----
  * The network forward for a (B,H,W) input is a fixed list of ops.  irsde_plan_num_ops returns its length (or a negative
  * irsde_status); irsde_plan_op_info gives op `op`'s label (the state-dict name of the weight it applies, e.g.
