@@ -25,8 +25,9 @@ SYMBOLS = ["irsde_create", "irsde_create_ch_mult", "irsde_create_nafnet", "irsde
            "irsde_reverse", "irsde_noise_state", "irsde_noise_state_images", "irsde_set_image_base", "irsde_set_image_uids", "irsde_comm_unique_id", "irsde_comm_init", "irsde_broadcast_weights", "irsde_gather", "irsde_launch_count", "irsde_device_bytes", "irsde_conv2d", "irsde_profile_begin",
            "irsde_profile_end", "irsde_profile_end_bytes", "irsde_conv2d_ex", "irsde_conv2d_fused", "irsde_layernorm",
            "irsde_attention", "irsde_plan_num_ops", "irsde_plan_op_info", "irsde_trace_forward", "irsde_trim",
-           "irsde_random_states"]
+           "irsde_random_states", "irsde_nafnet_op", "irsde_time_embedding", "irsde_step_philox", "irsde_prep_input"]
 ATTN_LINEAR, ATTN_LINEAR_FOLD, ATTN_FULL = 0, 1, 2  # irsde_attention kinds
+NAF_DWGATE_SCA, NAF_SIMPLE_GATE, NAF_PIXEL_SHUFFLE_ADD, NAF_ADD = 0, 1, 2, 3  # irsde_nafnet_op kinds
 
 
 class Config(ctypes.Structure):
@@ -55,6 +56,14 @@ class LnArgs(ctypes.Structure):
                 ("out_pitch", ctypes.c_int32), ("out_off", ctypes.c_int32),
                 ("ss_rows", ctypes.c_int32), ("ss_S", ctypes.c_int32), ("off_scale", ctypes.c_int32),
                 ("off_shift", ctypes.c_int32), ("ss_img_stride", ctypes.c_int32), ("t_row", ctypes.c_int32)]
+
+
+class NafArgs(ctypes.Structure):
+    """irsde_nafnet_args: operands and views of one irsde_nafnet_op call (device pointers as ints)."""
+    _fields_ = [("x", ctypes.c_void_p), ("y", ctypes.c_void_p), ("out", ctypes.c_void_p), ("w", ctypes.c_void_p),
+                ("bias", ctypes.c_void_p), ("sca_w", ctypes.c_void_p), ("sca_b", ctypes.c_void_p), ("sca", ctypes.c_void_p),
+                ("x_pitch", ctypes.c_int32), ("x_off", ctypes.c_int32), ("y_pitch", ctypes.c_int32), ("y_off", ctypes.c_int32),
+                ("out_pitch", ctypes.c_int32), ("out_off", ctypes.c_int32)]
 
 
 _lib = None
@@ -116,6 +125,14 @@ def load():
     L.irsde_layernorm.restype = ctypes.c_int
     L.irsde_attention.argtypes = [vp, i32, i32, vp, i32, i32, vp, i32, i32, vp, i32, vp, i32, i32, ctypes.POINTER(i32), vp]
     L.irsde_attention.restype = ctypes.c_int
+    L.irsde_nafnet_op.argtypes = [vp, i32, i32, ctypes.POINTER(NafArgs), i32, i32, i32, i32, ctypes.POINTER(i32), vp]
+    L.irsde_nafnet_op.restype = ctypes.c_int
+    L.irsde_time_embedding.argtypes = [i32, vp, i32, i32, vp, vp, vp, vp, vp, vp, i32, vp, vp, vp]
+    L.irsde_time_embedding.restype = ctypes.c_int
+    L.irsde_step_philox.argtypes = [vp, i32, vp, vp, vp, i32, vp, i32, i64, u64, vp]
+    L.irsde_step_philox.restype = ctypes.c_int
+    L.irsde_prep_input.argtypes = [i32, vp, vp, vp] + [i32] * 13 + [vp]
+    L.irsde_prep_input.restype = ctypes.c_int
     L.irsde_plan_num_ops.argtypes = [vp, i32, i32, i32]
     L.irsde_plan_num_ops.restype = i32
     L.irsde_plan_op_info.argtypes = [vp, i32, i32, i32, i32, ctypes.c_char_p, i32, ctypes.POINTER(i32)]

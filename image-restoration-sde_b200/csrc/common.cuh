@@ -125,10 +125,14 @@ template <typename T>
 LnPick ln_pick(int C, long long npix, int x_pitch, int res_pitch, int out_pitch, const void* x, const float* g, const void* res,
                const void* out);
 // ---- NAFNet kernels (nafnet.cu)
+// pixels per pooling chunk of an N-pixel image, and the chunks of an H x W image
+int dw_pix(int N);
 int dwgate_chunks(int H, int W);
 template <typename T>
 void launch_dwgate(const T* x, int x_pitch, const float* w, const float* bias, T* gate, int g_pitch, float* partial, int B,
                    int H, int W, int c, cudaStream_t st);
+// true: sca_kernel scales the gate in place (one launch); false: a scale_channels_kernel pass follows (two launches)
+bool sca_fused(int N);
 template <typename T>
 void launch_sca_scale(const float* partial, const float* w, const float* bias, float* sca, T* g, int g_pitch, int B, int c,
                       int nchunks, int N, int* launches, cudaStream_t st);
@@ -141,6 +145,9 @@ void launch_pixel_shuffle_add(const T* in, int in_pitch, const T* skip, int s_pi
                               cudaStream_t st);
 template <typename T>
 void launch_add(const T* a, int a_pitch, const T* b, int b_pitch, T* out, int o_pitch, long long npix, int c, cudaStream_t st);
+// dynamic shared memory of naf_time_mlp_kernel / time_mlp_kernel (bytes)
+size_t naf_time_mlp_smem(int width);
+size_t time_mlp_smem(int nf);
 void launch_naf_time_gate(const float* times, int rows, int width, const float* w1, const float* b1, const float* w2,
                           const float* b2, float* tgate, cudaStream_t st);
 // table[r][j] = dot(wall[j][0..td), tvec[r][0..td)) + ball[j]
@@ -170,7 +177,8 @@ void launch_fullattn(const T* qkv, int qkv_pitch, T* hidden, int hid_pitch, int 
 void launch_time_table(const float* times, int rows, int nf, const float* w1, const float* b1, const float* w2,
                        const float* b2, const float* wall, const float* ball, int S, float* temb_ws, float* table,
                        cudaStream_t st);
-// sampler update
+// sampler update.  z == null draws z in-kernel, keyed by seed, uid_base / uids and t: from *st_dev in the chain, from the
+// arguments (t_host) otherwise
 struct StepState {
   int t;               // current timestep (table row)
   int i;               // executed-step index (z slice)
@@ -181,7 +189,7 @@ struct StepState {
 };
 void launch_sde_update(int mode, const float* x, const float* mu, const float* noise, const float* z, long long z_stride,
                        const float* coef, const StepState* st_dev, int t_host, float* out, long long n, uint64_t seed,
-                       long long img_elems, uint64_t uid_base, cudaStream_t st);
+                       long long img_elems, uint64_t uid_base, const unsigned long long* uids, cudaStream_t st);
 void launch_advance_step(StepState* st_dev, cudaStream_t st);
 void launch_set_step(StepState* st_dev, int t, int i, const float* z, unsigned long long seed, unsigned long long uid_base,
                      const unsigned long long* uids, cudaStream_t st);

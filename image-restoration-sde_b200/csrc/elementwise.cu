@@ -151,11 +151,14 @@ void launch_time_rows(const float* tvec, int rows, int td, const float* wall, co
   time_table_kernel<<<dim3((S + 7) / 8, rows), 256, 0, st>>>(tvec, td, wall, ball, S, table);
 }
 
+// emb [nf] + h1 [4nf] floats
+size_t time_mlp_smem(int nf) { return (size_t)nf * 5 * sizeof(float); }
+
 void launch_time_table(const float* times, int rows, int nf, const float* w1, const float* b1, const float* w2,
                        const float* b2, const float* wall, const float* ball, int S, float* temb_ws, float* table,
                        cudaStream_t st) {
   int td = nf * 4;
-  time_mlp_kernel<<<rows, 256, (nf + td) * sizeof(float), st>>>(times, nf, w1, b1, w2, b2, temb_ws);
+  time_mlp_kernel<<<rows, 256, time_mlp_smem(nf), st>>>(times, nf, w1, b1, w2, b2, temb_ws);
   time_table_kernel<<<dim3((S + 7) / 8, rows), 256, 0, st>>>(temb_ws, td, wall, ball, S, table);
 }
 
@@ -269,9 +272,8 @@ __global__ void sde_update_kernel(int mode, const float* __restrict__ x, const f
                                   const float* __restrict__ noise, const float* __restrict__ z, long long z_stride,
                                   const float* __restrict__ coef, const StepState* __restrict__ stp, int t_host,
                                   float* __restrict__ out, long long n, uint64_t seed, long long img_elems,
-                                  uint64_t uid_base) {
+                                  uint64_t uid_base, const unsigned long long* __restrict__ uids) {
   PDL_ENTRY();
-  const unsigned long long* uids = nullptr;
   int t = stp ? stp->t : t_host;
   int si = stp ? stp->i : 0;
   float c[8];
@@ -315,11 +317,11 @@ __global__ void sde_update_kernel(int mode, const float* __restrict__ x, const f
 
 void launch_sde_update(int mode, const float* x, const float* mu, const float* noise, const float* z, long long z_stride,
                        const float* coef, const StepState* st_dev, int t_host, float* out, long long n, uint64_t seed,
-                       long long img_elems, uint64_t uid_base, cudaStream_t st) {
+                       long long img_elems, uint64_t uid_base, const unsigned long long* uids, cudaStream_t st) {
   long long groups = (n + 3) / 4;
   pdl_launch(sde_update_kernel, (unsigned)((groups + 255) / 256), 256, 0, st, mode, x, mu, noise, z, z_stride, coef, st_dev,
                                                                       t_host, out, n, seed, img_elems > 0 ? img_elems : n,
-                                                                      uid_base);
+                                                                      uid_base, uids);
 }
 
 __global__ void advance_step_kernel(StepState* s) {

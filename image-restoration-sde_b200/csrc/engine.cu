@@ -155,6 +155,11 @@ int fail(const irsde_ctx* ctx, int code, const std::string& msg) {
   return code;
 }
 
+// the time MLPs run with the default dynamic shared memory limit (no cudaFuncSetAttribute opt-in)
+constexpr size_t kTimeMlpSmemMax = 48 * 1024;
+// sca_kernel keeps the c channel means in dynamic shared memory, under the same limit
+constexpr int kScaMaxC = 48 * 1024 / 4;
+
 void* dev_alloc(irsde_ctx* ctx, size_t bytes, std::vector<void*>* owner) {
   void* p = nullptr;
   if (bytes == 0) bytes = 16;
@@ -1446,6 +1451,8 @@ int irsde_create(const irsde_config* cfg, irsde_ctx** out) {
     return fail(nullptr, IRSDE_ERR_INVALID, "bad network configuration");
   if (cfg->variant != IRSDE_NET_CONDITIONAL && cfg->variant != IRSDE_NET_DENOISING)
     return fail(nullptr, IRSDE_ERR_INVALID, "bad variant");
+  if (time_mlp_smem(cfg->nf) > kTimeMlpSmemMax)
+    return fail(nullptr, IRSDE_ERR_UNSUPPORTED, "nf > 2457: the time MLP needs more than 48 KB of shared memory");
   if (cfg->precision != IRSDE_PREC_FP32 && cfg->precision != IRSDE_PREC_BF16 && cfg->precision != IRSDE_PREC_FP32X3)
     return fail(nullptr, IRSDE_ERR_INVALID, "bad precision");
   int ndev = 0;
@@ -1543,6 +1550,10 @@ int irsde_create_nafnet(const irsde_nafnet_config* ncfg, irsde_ctx** out) {
   if (ncfg->width < 4 || ncfg->width % 2 || ncfg->img_channel < 1 || ncfg->n_levels < 0 || ncfg->n_levels > 8 ||
       ncfg->middle_blk_num < 0)
     return fail(nullptr, IRSDE_ERR_INVALID, "bad NAFNet configuration");
+  if (naf_time_mlp_smem(ncfg->width) > kTimeMlpSmemMax)
+    return fail(nullptr, IRSDE_ERR_UNSUPPORTED, "width > 945: the time MLP needs more than 48 KB of shared memory");
+  if (((long long)ncfg->width << ncfg->n_levels) > kScaMaxC)
+    return fail(nullptr, IRSDE_ERR_UNSUPPORTED, "width << n_levels > 12288: the SCA mat-vec needs more than 48 KB of shared memory");
   irsde_config cfg;
   memset(&cfg, 0, sizeof cfg);
   cfg.in_nc = cfg.out_nc = ncfg->img_channel;
@@ -1829,7 +1840,7 @@ int irsde_step(irsde_ctx* ctx, int32_t mode, const float* x, const float* mu, co
   if (need_z && !z) return fail(ctx, IRSDE_ERR_INVALID, "z required for stochastic modes");
   if (mode <= IRSDE_MODE_POSTERIOR && !mu) return fail(ctx, IRSDE_ERR_INVALID, "mu required for IRSDE modes");
   cudaSetDevice(ctx->cfg.device);
-  launch_sde_update(mode, x, mu, noise, z, 0, ctx->coef_dev[mode], nullptr, t, out, n, 0, 0, 0, (cudaStream_t)stream);
+  launch_sde_update(mode, x, mu, noise, z, 0, ctx->coef_dev[mode], nullptr, t, out, n, 0, 0, 0, nullptr, (cudaStream_t)stream);
   ctx->launches++;
   CUDA_TRY(ctx, cudaGetLastError());
   return IRSDE_OK;
@@ -1870,7 +1881,7 @@ int irsde_reverse(irsde_ctx* ctx, int32_t mode, const float* xT, const float* mu
   auto one_step = [&](cudaStream_t s) {
     run_forward(ctx, p, s);
     launch_sde_update(mode, p->x_state, mu_arg, p->eps_buf, nullptr, n, ctx->coef_dev[mode], p->d_step, 0, p->x_state, n, 0,
-                      n / B, 0, s);
+                      n / B, 0, nullptr, s);
     launch_advance_step(p->d_step, s);
     ctx->launches += 2;
   };
@@ -2479,6 +2490,155 @@ int irsde_attention(irsde_ctx* ctx, int32_t precision, int32_t kind, const float
     ctx->launches += lin ? 3 : 1;
   }
   return finish_op(ctx, rc, "attention failed: ", st, tmp);
+}
+
+// ---- one NAFNet op, time embedding, sampler step or input packing outside a plan ----------------------------------
+int irsde_nafnet_op(irsde_ctx* ctx, int32_t precision, int32_t kind, const irsde_nafnet_args* args, int32_t B, int32_t H,
+                    int32_t W, int32_t c, int32_t* info, void* stream) {
+  // ---- everything is validated here, before the first allocation or launch
+  if (!ctx || !args || !args->x || !args->out) return fail(ctx, IRSDE_ERR_INVALID, "null argument");
+  const irsde_nafnet_args& a = *args;
+  if (precision < IRSDE_PREC_FP32 || precision > IRSDE_PREC_FP32X3) return fail(ctx, IRSDE_ERR_INVALID, "bad precision");
+  if (kind < IRSDE_NAF_DWGATE_SCA || kind > IRSDE_NAF_ADD) return fail(ctx, IRSDE_ERR_INVALID, "unknown NAFNet op");
+  const bool dw = kind == IRSDE_NAF_DWGATE_SCA, ps = kind == IRSDE_NAF_PIXEL_SHUFFLE_ADD;
+  if (B < 1 || B > 65535 || H < 1 || W < 1 || c < 1 || (long long)H * W > (1LL << 30))
+    return fail(ctx, IRSDE_ERR_INVALID, "bad shape");
+  if (dw && c > kScaMaxC) return fail(ctx, IRSDE_ERR_UNSUPPORTED, "c > 12288: the SCA mat-vec needs more than 48 KB of shared memory");
+  if (dw && (!a.w || !a.bias || !a.sca_w || !a.sca_b || !a.sca)) return fail(ctx, IRSDE_ERR_INVALID, "DWGATE_SCA needs w, bias, sca_w, sca_b and sca");
+  if ((ps || kind == IRSDE_NAF_ADD) && !a.y) return fail(ctx, IRSDE_ERR_INVALID, "PIXEL_SHUFFLE_ADD and ADD need y");
+  auto view_ok = [](int pitch, int off, long long width) { return off >= 0 && (long long)off + width <= pitch; };
+  const long long xw = ps ? 4LL * c : kind == IRSDE_NAF_ADD ? c : 2LL * c;
+  if (!view_ok(a.x_pitch, a.x_off, xw)) return fail(ctx, IRSDE_ERR_INVALID, "x view outside its pitch");
+  if (a.y && (ps || kind == IRSDE_NAF_ADD) && !view_ok(a.y_pitch, a.y_off, c)) return fail(ctx, IRSDE_ERR_INVALID, "y view outside its pitch");
+  if (!view_ok(a.out_pitch, a.out_off, c)) return fail(ctx, IRSDE_ERR_INVALID, "out view outside its pitch");
+  int32_t info_local[4];
+  if (!info) info = info_local;
+  info[0] = info[1] = info[2] = info[3] = 0;
+
+  cudaSetDevice(ctx->cfg.device);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int N = H * W;
+  const long long npix_in = (long long)B * N, npix_out = ps ? 4 * npix_in : npix_in;  // PIXEL_SHUFFLE_ADD: H x W is the input
+  const int nchunks = dw ? dwgate_chunks(H, W) : 0;
+  std::vector<void*> tmp;
+  int rc = IRSDE_OK;
+  float* partial = dw ? (float*)dev_alloc(ctx, (size_t)B * nchunks * c * sizeof(float), &tmp) : nullptr;
+  if (dw && !partial) rc = fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
+  int sca_launches = 0;
+  // one launch path for both storage types: S = float views of the caller's buffers, or bf16 copies of them
+  auto run = [&](auto* xs, auto* ys, auto* os) {
+    using S = std::remove_const_t<std::remove_pointer_t<decltype(xs)>>;
+    const S* xv = xs + a.x_off;
+    const S* yv = ys ? ys + a.y_off : nullptr;
+    S* ov = os + a.out_off;
+    if (dw) {
+      launch_dwgate<S>(xv, a.x_pitch, a.w, a.bias, ov, a.out_pitch, partial, B, H, W, c, st);
+      launch_sca_scale<S>(partial, a.sca_w, a.sca_b, a.sca, ov, a.out_pitch, B, c, nchunks, N, &sca_launches, st);
+    } else if (kind == IRSDE_NAF_SIMPLE_GATE) {
+      launch_simple_gate<S>(xv, a.x_pitch, ov, a.out_pitch, npix_in, c, st);
+    } else if (ps) {
+      launch_pixel_shuffle_add<S>(xv, a.x_pitch, yv, a.y_pitch, ov, a.out_pitch, B, H, W, c, st);
+    } else {
+      launch_add<S>(xv, a.x_pitch, yv, a.y_pitch, ov, a.out_pitch, npix_in, c, st);
+    }
+  };
+  const bool has_y = ps || kind == IRSDE_NAF_ADD;
+  if (!rc && precision == IRSDE_PREC_BF16) {
+    const long long nx = npix_in * a.x_pitch, ny = has_y ? npix_out * a.y_pitch : 0, no = npix_out * a.out_pitch;
+    bf16* xb = (bf16*)dev_alloc(ctx, nx * 2, &tmp);
+    bf16* yb = has_y ? (bf16*)dev_alloc(ctx, ny * 2, &tmp) : nullptr;
+    bf16* ob = (bf16*)dev_alloc(ctx, no * 2, &tmp);
+    if (!xb || !ob || (has_y && !yb)) rc = fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
+    if (!rc) {
+      cast_f32_bf16_kernel<<<cast_blocks(nx), 256, 0, st>>>(a.x, xb, nx);
+      if (yb) cast_f32_bf16_kernel<<<cast_blocks(ny), 256, 0, st>>>(a.y, yb, ny);
+      cast_f32_bf16_kernel<<<cast_blocks(no), 256, 0, st>>>(a.out, ob, no);
+      run((const bf16*)xb, (const bf16*)yb, ob);
+      cast_bf16_f32_kernel<<<cast_blocks(no), 256, 0, st>>>(ob, a.out, no);
+    }
+  } else if (!rc) {
+    run(a.x, has_y ? a.y : (const float*)nullptr, a.out);
+  }
+  if (!rc) {
+    if (dw) {
+      info[0] = dw_pix(N); info[1] = nchunks; info[2] = sca_launches;
+      ctx->launches += 1 + sca_launches;
+    } else {
+      ctx->launches++;
+    }
+  }
+  return finish_op(ctx, rc, "NAFNet op failed: ", st, tmp);
+}
+
+int irsde_step_philox(irsde_ctx* ctx, int32_t mode, const float* x, const float* mu, const float* noise, int32_t t, float* out,
+                      int32_t B, int64_t image_elems, uint64_t seed, void* stream) {
+  if (!ctx || !x || !noise || !out || mode < 0 || mode >= IRSDE_NUM_MODES) return fail(ctx, IRSDE_ERR_INVALID, "bad argument");
+  if (mode != IRSDE_MODE_SDE && mode != IRSDE_MODE_POSTERIOR && mode != IRSDE_MODE_DSDE_SDE)
+    return fail(ctx, IRSDE_ERR_INVALID, "the ODE modes draw no noise");
+  if (!ctx->have_sched) return fail(ctx, IRSDE_ERR_STATE, "schedule not set");
+  if (t < 1 || t > ctx->T) return fail(ctx, IRSDE_ERR_INVALID, "t out of range [1,T]");
+  if (mode <= IRSDE_MODE_POSTERIOR && !mu) return fail(ctx, IRSDE_ERR_INVALID, "mu required for IRSDE modes");
+  if (B < 1 || image_elems < 1) return fail(ctx, IRSDE_ERR_INVALID, "bad shape");
+  if (ctx->n_uids && ctx->n_uids != B) return fail(ctx, IRSDE_ERR_INVALID, "irsde_set_image_uids count does not match the batch");
+  cudaSetDevice(ctx->cfg.device);
+  launch_sde_update(mode, x, mu, noise, nullptr, 0, ctx->coef_dev[mode], nullptr, t, out, (long long)B * image_elems, seed,
+                    image_elems, ctx->image_base, ctx->n_uids ? ctx->d_uids : nullptr, (cudaStream_t)stream);
+  ctx->launches++;
+  CUDA_TRY(ctx, cudaGetLastError());
+  return IRSDE_OK;
+}
+
+int irsde_time_embedding(int32_t family, const float* times, int32_t rows, int32_t width, const float* w1, const float* b1,
+                         const float* w2, const float* b2, const float* wall, const float* ball, int32_t S, float* temb,
+                         float* table, void* stream) {
+  if (!times || !w1 || !b1 || !w2 || !b2 || !wall || !ball || !temb || !table) return fail(nullptr, IRSDE_ERR_INVALID, "null argument");
+  if (family != 0 && family != 1) return fail(nullptr, IRSDE_ERR_INVALID, "family must be 0 (ConditionalUNet) or 1 (NAFNet)");
+  if (rows < 1 || rows > 65535 || S < 1 || width < 4 || width % 2) return fail(nullptr, IRSDE_ERR_INVALID, "bad shape");
+  if ((family == 0 ? time_mlp_smem(width) : naf_time_mlp_smem(width)) > kTimeMlpSmemMax)
+    return fail(nullptr, IRSDE_ERR_UNSUPPORTED, "the time MLP of this width needs more than 48 KB of shared memory");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (family == 0) {
+    launch_time_table(times, rows, width, w1, b1, w2, b2, wall, ball, S, temb, table, st);
+  } else {
+    launch_naf_time_gate(times, rows, width, w1, b1, w2, b2, temb, st);
+    launch_time_rows(temb, rows, 2 * width, wall, ball, S, table, st);
+  }
+  cudaError_t ce = cudaStreamSynchronize(st);
+  if (ce == cudaSuccess) ce = cudaGetLastError();
+  if (ce != cudaSuccess) return fail(nullptr, IRSDE_ERR_CUDA, std::string("time embedding failed: ") + cudaGetErrorString(ce));
+  return IRSDE_OK;
+}
+
+int irsde_prep_input(int32_t precision, const float* xt, const float* cond, float* out, int32_t B, int32_t C, int32_t H, int32_t W,
+                     int32_t Hp, int32_t Wp, int32_t pitch, int32_t conditional, int32_t zero_pad, int32_t pad_top, int32_t pad_left,
+                     int32_t row_pix, int32_t img_rows, void* stream) {
+  if (!xt || !out || (conditional && !cond)) return fail(nullptr, IRSDE_ERR_INVALID, "null argument");
+  if (precision < IRSDE_PREC_FP32 || precision > IRSDE_PREC_FP32X3) return fail(nullptr, IRSDE_ERR_INVALID, "bad precision");
+  if (B < 1 || C < 1 || H < 1 || W < 1 || Hp < H || Wp < W) return fail(nullptr, IRSDE_ERR_INVALID, "bad shape");
+  if (!zero_pad && (Hp - H >= H || Wp - W >= W))
+    return fail(nullptr, IRSDE_ERR_INVALID, "reflect padding of H - 1 or more rows / columns would read outside the image");
+  if (pitch < C * (conditional ? 2 : 1)) return fail(nullptr, IRSDE_ERR_INVALID, "pitch below the packed channels");
+  if (row_pix == 0 && (img_rows || pad_top || pad_left)) return fail(nullptr, IRSDE_ERR_INVALID, "a border needs row_pix and img_rows");
+  if (row_pix != 0 && (pad_top < 0 || pad_left < 0 || (long long)pad_top + Hp > img_rows || (long long)pad_left + Wp > row_pix))
+    return fail(nullptr, IRSDE_ERR_INVALID, "the padded image does not fit inside its border");
+  const long long n = (long long)B * (row_pix ? (long long)img_rows * row_pix : (long long)Hp * Wp) * pitch;
+  cudaStream_t st = (cudaStream_t)stream;
+  bf16* ob = nullptr;
+  if (precision == IRSDE_PREC_BF16) {
+    if (cudaMalloc(&ob, n * 2) != cudaSuccess) return fail(nullptr, IRSDE_ERR_CUDA, "cudaMalloc failed");
+    cast_f32_bf16_kernel<<<cast_blocks(n), 256, 0, st>>>(out, ob, n);
+    launch_prep_input<bf16>(xt, cond, ob, B, C, H, W, Hp, Wp, pitch, conditional ? 1 : 0, st, pad_top, pad_left, row_pix, img_rows,
+                            zero_pad ? 1 : 0);
+    cast_bf16_f32_kernel<<<cast_blocks(n), 256, 0, st>>>(ob, out, n);
+  } else {
+    launch_prep_input<float>(xt, cond, out, B, C, H, W, Hp, Wp, pitch, conditional ? 1 : 0, st, pad_top, pad_left, row_pix, img_rows,
+                             zero_pad ? 1 : 0);
+  }
+  cudaError_t ce = cudaStreamSynchronize(st);
+  if (ce == cudaSuccess) ce = cudaGetLastError();
+  if (ob) cudaFree(ob);
+  if (ce != cudaSuccess) return fail(nullptr, IRSDE_ERR_CUDA, std::string("prep_input failed: ") + cudaGetErrorString(ce));
+  return IRSDE_OK;
 }
 
 // ---- image conversion / metrics (stateless) ----------------------------------------------------------------

@@ -3,6 +3,8 @@
 // All are HBM-bound NHWC kernels (fp32 math; float or bf16 storage).
 #include <math.h>
 
+#include <algorithm>
+
 #include "common.cuh"
 
 namespace irsde {
@@ -13,8 +15,10 @@ namespace irsde {
 //   partial[b][chunk][ch] = sum over the chunk's pixels of gate (AdaptiveAvgPool2d numerator, :29-30)
 // block = 64 channels x 4 pixel lanes, chunk = 64 pixels of one image - 16 for images of <= 1024 pixels, where 64-pixel
 // chunks leave a handful of blocks each walking 16 pixels x 9 taps serially (c=512, 16x16) - (deterministic reduction order, fixed by the image shape)
+// grid (ceil(c/64), min(nchunks, 65535), B): a block walks chunks blockIdx.y, blockIdx.y + gridDim.y, ..., so images of
+// more than 65535 chunks (a 2048x2048 level has 65536) launch too; below that every block owns one chunk.
 // =============================================================================================
-static inline int dw_pix(int N) { return N <= 1024 ? 16 : 64; }
+int dw_pix(int N) { return N <= 1024 ? 16 : 64; }
 
 template <typename T>
 __global__ void __launch_bounds__(256) dwgate_kernel(const T* __restrict__ x, int x_pitch, const float* __restrict__ w,
@@ -25,42 +29,45 @@ __global__ void __launch_bounds__(256) dwgate_kernel(const T* __restrict__ x, in
   __shared__ float red[4][64];
   const int cl = threadIdx.x & 63, pl = threadIdx.x >> 6;
   const int ch = blockIdx.x * 64 + cl;
-  const int chunk = blockIdx.y, b = blockIdx.z;
+  const int b = blockIdx.z;
   const int N = H * W;
-  float acc_sum = 0.f;
-  if (ch < c) {
-    float w1[9], w2[9];
+  for (int chunk = blockIdx.y; chunk < nchunks; chunk += (int)gridDim.y) {
+    float acc_sum = 0.f;
+    if (ch < c) {
+      float w1[9], w2[9];
 #pragma unroll
-    for (int k = 0; k < 9; ++k) { w1[k] = w[ch * 9 + k]; w2[k] = w[(ch + c) * 9 + k]; }
-    const float b1 = bias[ch], b2 = bias[ch + c];
-    for (int i = pl; i < DW_PIX; i += 4) {
-      const int p = chunk * DW_PIX + i;
-      if (p >= N) break;
-      const int h = p / W, wq = p - h * W;
-      float a1 = b1, a2 = b2;
+      for (int k = 0; k < 9; ++k) { w1[k] = w[ch * 9 + k]; w2[k] = w[(ch + c) * 9 + k]; }
+      const float b1 = bias[ch], b2 = bias[ch + c];
+      for (int i = pl; i < DW_PIX; i += 4) {
+        const int p = chunk * DW_PIX + i;
+        if (p >= N) break;
+        const int h = p / W, wq = p - h * W;
+        float a1 = b1, a2 = b2;
 #pragma unroll
-      for (int r = 0; r < 3; ++r) {
-        const int hh = h + r - 1;
-        if (hh < 0 || hh >= H) continue;
+        for (int r = 0; r < 3; ++r) {
+          const int hh = h + r - 1;
+          if (hh < 0 || hh >= H) continue;
 #pragma unroll
-        for (int s = 0; s < 3; ++s) {
-          const int ww = wq + s - 1;
-          if (ww < 0 || ww >= W) continue;
-          const T* row = x + (((long long)b * H + hh) * W + ww) * x_pitch;
-          a1 = fmaf(w1[r * 3 + s], to_f(row[ch]), a1);
-          a2 = fmaf(w2[r * 3 + s], to_f(row[ch + c]), a2);
+          for (int s = 0; s < 3; ++s) {
+            const int ww = wq + s - 1;
+            if (ww < 0 || ww >= W) continue;
+            const T* row = x + (((long long)b * H + hh) * W + ww) * x_pitch;
+            a1 = fmaf(w1[r * 3 + s], to_f(row[ch]), a1);
+            a2 = fmaf(w2[r * 3 + s], to_f(row[ch + c]), a2);
+          }
         }
+        const float gv = a1 * a2;
+        const T gq = from_f<T>(gv);
+        gate[((long long)b * N + p) * g_pitch + ch] = gq;
+        acc_sum += to_f(gq);  // pool the stored (rounded) value: what conv3 will actually read
       }
-      const float gv = a1 * a2;
-      const T gq = from_f<T>(gv);
-      gate[((long long)b * N + p) * g_pitch + ch] = gq;
-      acc_sum += to_f(gq);  // pool the stored (rounded) value: what conv3 will actually read
     }
+    red[pl][cl] = acc_sum;
+    __syncthreads();
+    if (pl == 0 && ch < c)
+      partial[((long long)b * nchunks + chunk) * c + ch] = (red[0][cl] + red[1][cl]) + (red[2][cl] + red[3][cl]);
+    if (chunk + (int)gridDim.y < nchunks) __syncthreads();  // red is refilled for the next chunk
   }
-  red[pl][cl] = acc_sum;
-  __syncthreads();
-  if (pl == 0 && ch < c)
-    partial[((long long)b * nchunks + chunk) * c + ch] = (red[0][cl] + red[1][cl]) + (red[2][cl] + red[3][cl]);
 }
 
 // mean over pixels -> 1x1 conv (c x c mat-vec + bias): sca[b][o]            (DenoisingNAFNet_arch.py:29-33)
@@ -168,7 +175,7 @@ template <typename T>
 void launch_dwgate(const T* x, int x_pitch, const float* w, const float* bias, T* gate, int g_pitch, float* partial, int B,
                    int H, int W, int c, cudaStream_t st) {
   const int nchunks = dwgate_chunks(H, W);
-  pdl_launch(dwgate_kernel<T>, dim3((c + 63) / 64, nchunks, B), 256, 0, st, x, x_pitch, w, bias, gate, g_pitch, partial, H, W, c, nchunks,
+  pdl_launch(dwgate_kernel<T>, dim3((c + 63) / 64, std::min(nchunks, 65535), B), 256, 0, st, x, x_pitch, w, bias, gate, g_pitch, partial, H, W, c, nchunks,
              dw_pix(H * W));
 }
 template void launch_dwgate<float>(const float*, int, const float*, const float*, float*, int, float*, int, int, int, int, cudaStream_t);
@@ -179,10 +186,12 @@ void launch_scale_channels(T* x, int pitch, const float* sca, int B, int N, int 
 
 // sca[b][:] and g *= sca in place.  N <= 1024 pixels: one launch does both; larger images use a second, fully
 // parallel pass (8 channels per block would not cover the pixels fast enough).
+bool sca_fused(int N) { return N <= 1024; }
+
 template <typename T>
 void launch_sca_scale(const float* partial, const float* w, const float* bias, float* sca, T* g, int g_pitch, int B, int c,
                       int nchunks, int N, int* launches, cudaStream_t st) {
-  const bool fused = N <= 1024;
+  const bool fused = sca_fused(N);
   pdl_launch(sca_kernel<T>, dim3((c + 7) / 8, B), 256, c * sizeof(float), st, partial, w, bias, sca, c, nchunks, N, fused ? g : (T*)nullptr, g_pitch);
   *launches = 1;
   if (!fused) { launch_scale_channels<T>(g, g_pitch, sca, B, N, c, st); *launches = 2; }
@@ -260,10 +269,12 @@ __global__ void naf_time_mlp_kernel(const float* __restrict__ times, int width, 
   for (int o = threadIdx.x; o < td / 2; o += blockDim.x) tgate[(long long)row * (td / 2) + o] = tt[o] * tt[o + td / 2];
 }
 
+// emb [w] + h1 [8w] + t [4w] floats
+size_t naf_time_mlp_smem(int width) { return (size_t)width * 13 * sizeof(float); }
+
 void launch_naf_time_gate(const float* times, int rows, int width, const float* w1, const float* b1, const float* w2,
                           const float* b2, float* tgate, cudaStream_t st) {
-  const int td = width * 4;
-  naf_time_mlp_kernel<<<rows, 256, (width + 2 * td + td) * sizeof(float), st>>>(times, width, w1, b1, w2, b2, tgate);
+  naf_time_mlp_kernel<<<rows, 256, naf_time_mlp_smem(width), st>>>(times, width, w1, b1, w2, b2, tgate);
 }
 
 }  // namespace irsde

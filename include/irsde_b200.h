@@ -98,14 +98,16 @@ typedef struct {
 } irsde_latent_unet_config;
 
 /* Replaces `ConditionalUNet(in_nc,out_nc,nf,depth)` + `.to(device)`
- * (DenoisingUNet_arch.py:20, models/denoising_model.py:36). */
+ * (DenoisingUNet_arch.py:20, models/denoising_model.py:36).  nf <= 2456: the time MLP keeps 20 nf bytes in shared memory. */
 int irsde_create(const irsde_config* cfg, irsde_ctx** out);
 /* The latent-task variant `ConditionalUNet(in_nc, out_nc, nf, ch_mult=[1,2,4,4])`
  * (codes/config/latent-dehazing/models/modules/DenoisingUNet_arch.py:17-20,51-56,70): level i has nf*[1,ch_mult...][i]
  * channels and depth = len(ch_mult) (cfg->depth is ignored). */
 int irsde_create_ch_mult(const irsde_config* cfg, const int32_t* ch_mult, int32_t n_levels, irsde_ctx** out);
 /* Same context type, ConditionalNAFNet architecture; every other entry point (load_tensor, noise_fn, reverse, ...)
- * is shared.  Replaces `ConditionalNAFNet(...)` + `.to(device)` (DenoisingNAFNet_arch.py:89). */
+ * is shared.  Replaces `ConditionalNAFNet(...)` + `.to(device)` (DenoisingNAFNet_arch.py:89).  width <= 944 and
+ * width << n_levels <= 12288: the time MLP (52 width bytes) and the SCA mat-vec (4 bytes per channel) fit in 48 KB of
+ * shared memory. */
 int irsde_create_nafnet(const irsde_nafnet_config* cfg, irsde_ctx** out);
 void irsde_destroy(irsde_ctx* ctx);
 const char* irsde_last_error(const irsde_ctx* ctx);
@@ -285,6 +287,66 @@ int irsde_layernorm(irsde_ctx* ctx, int32_t precision, const float* x, const irs
 int irsde_attention(irsde_ctx* ctx, int32_t precision, int32_t kind, const float* qkv, int32_t qkv_pitch, int32_t qkv_off,
                     float* out, int32_t out_pitch, int32_t out_off, const float* wout, int32_t Cout, float* ctx_out, int32_t B,
                     int32_t N, int32_t* info, void* stream);
+
+/* One NAFBlock op of the launch plan (DenoisingNAFNet_arch.py:9-12,29-33,65-67; the decoder's PixelShuffle + skip, :172-174;
+ * the latent variant's x + intro(x)).  x, y and out are fp32 NHWC buffers read or written through (pitch, channel offset)
+ * views; views need not be aligned.  Pixel counts: x and (for ADD) y hold B*H*W pixels; for PIXEL_SHUFFLE_ADD, H x W is the
+ * input's size and y (the skip) and out hold B*2H*2W pixels.
+ *   IRSDE_NAF_DWGATE_SCA      gate = dw3x3(x)[0..c) * dw3x3(x)[c..2c) (depthwise, zero padding 1, bias), then
+ *                             sca[b] = sca_w @ mean_HW(gate[b]) + sca_b and out = gate * sca: x holds 2c channels, w is
+ *                             [2c][9], bias [2c], sca_w [c][c], sca_b [c], sca fp32 [B][c] (written);
+ *   IRSDE_NAF_SIMPLE_GATE     out = x[0..c) * x[c..2c);
+ *   IRSDE_NAF_PIXEL_SHUFFLE_ADD  out[b, 2h+i, 2w+j, q] = x[b, h, w, 4q + 2i + j] + y[b, 2h+i, 2w+j, q] (c = q);
+ *   IRSDE_NAF_ADD             out = x + y (c channels each). */
+#define IRSDE_NAF_DWGATE_SCA 0
+#define IRSDE_NAF_SIMPLE_GATE 1
+#define IRSDE_NAF_PIXEL_SHUFFLE_ADD 2
+#define IRSDE_NAF_ADD 3
+typedef struct {
+  const float* x;
+  const float* y;         /* PIXEL_SHUFFLE_ADD, ADD; else ignored */
+  float* out;
+  const float* w;         /* DWGATE_SCA only: conv2 weight [2c][9] and bias [2c] */
+  const float* bias;
+  const float* sca_w;     /* DWGATE_SCA only: sca.1 weight [c][c] and bias [c] */
+  const float* sca_b;
+  float* sca;             /* DWGATE_SCA only: fp32 [B][c] output */
+  int32_t x_pitch, x_off;
+  int32_t y_pitch, y_off;
+  int32_t out_pitch, out_off;
+} irsde_nafnet_args;
+
+/* Buffers are converted as in irsde_layernorm (sca stays fp32).  Every view and size is checked on the host before anything is
+ * allocated or launched.  info (or NULL) receives, for DWGATE_SCA, {pixels per pooling chunk, chunks per image, launches of
+ * the SCA stage (1: sca_kernel scales the gate in place, 2: a scale_channels_kernel pass follows), 0}; zeros otherwise. */
+int irsde_nafnet_op(irsde_ctx* ctx, int32_t precision, int32_t kind, const irsde_nafnet_args* args, int32_t B, int32_t H,
+                    int32_t W, int32_t c, int32_t* info, void* stream);
+
+/* The time-embedding MLP and the per-block (scale, shift) table the plan builds (stateless: no ctx; device pointers).
+ *   family 0 (ConditionalUNet, DenoisingUNet_arch.py:42-47, module_util.py:29-41,128-141): temb [rows][4 width] =
+ *            SiLU(Linear(GELU(Linear(pos(t))))), w1 [4w][w], w2 [4w][4w], wall [S][4w];
+ *   family 1 (NAFNet, DenoisingNAFNet_arch.py:18-20,51-54,96-101): temb [rows][2 width] = SimpleGate(Linear(SimpleGate(
+ *            Linear(pos(t))))), w1 [8w][w], w2 [4w][4w], wall [S][2w];
+ * table [rows][S] = temb @ wall^T + ball.  times: [rows] device floats.  width must be even and >= 4, and the MLP's shared
+ * memory (20 width or 52 width bytes) must fit in 48 KB. */
+int irsde_time_embedding(int32_t family, const float* times, int32_t rows, int32_t width, const float* w1, const float* b1,
+                         const float* w2, const float* b2, const float* wall, const float* ball, int32_t S, float* temb,
+                         float* table, void* stream);
+
+/* irsde_step for the stochastic modes with z drawn in-kernel, as irsde_reverse(z = NULL) draws it at step t: keyed by (seed,
+ * image uid, t, element index inside the image) with the uids of irsde_set_image_base / irsde_set_image_uids; x, mu, noise and
+ * out hold B images of image_elems floats. */
+int irsde_step_philox(irsde_ctx* ctx, int32_t mode, const float* x, const float* mu, const float* noise, int32_t t, float* out,
+                      int32_t B, int64_t image_elems, uint64_t seed, void* stream);
+
+/* The network's input packing (stateless): out [B][img_rows][row_pix][pitch] (row_pix = img_rows = 0: [B][Hp][Wp][pitch]) gets,
+ * at pixel (pad_top + hp, pad_left + wp), cat(xt - cond, cond) (conditional) or xt, of the image padded at the bottom / right
+ * to Hp x Wp by reflection (zero_pad = 0; Hp - H < H and Wp - W < W) or with zeros; channels 2C (C) .. pitch-1 are set to zero.
+ * Pixels outside the padded image (the border) are not written.  xt, cond: fp32 NCHW [B][C][H][W].  out is converted as in
+ * irsde_layernorm for precision 1. */
+int irsde_prep_input(int32_t precision, const float* xt, const float* cond, float* out, int32_t B, int32_t C, int32_t H, int32_t W,
+                     int32_t Hp, int32_t Wp, int32_t pitch, int32_t conditional, int32_t zero_pad, int32_t pad_top, int32_t pad_left,
+                     int32_t row_pix, int32_t img_rows, void* stream);
 
 /* ---- launch-plan introspection (parity instrumentation: per-layer comparison with the oracle) ----
  * The network forward for a (B,H,W) input is a fixed list of ops.  irsde_plan_num_ops returns its length (or a negative
