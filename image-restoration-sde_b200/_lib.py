@@ -24,7 +24,7 @@ SYMBOLS = ["irsde_create", "irsde_create_ch_mult", "irsde_create_nafnet", "irsde
            "irsde_finalize_weights", "irsde_set_schedule", "irsde_set_coeffs", "irsde_noise_fn", "irsde_step",
            "irsde_reverse", "irsde_noise_state", "irsde_noise_state_images", "irsde_set_image_base", "irsde_set_image_uids", "irsde_comm_unique_id", "irsde_comm_init", "irsde_broadcast_weights", "irsde_gather", "irsde_launch_count", "irsde_device_bytes", "irsde_conv2d", "irsde_profile_begin",
            "irsde_profile_end", "irsde_profile_end_bytes", "irsde_conv2d_ex", "irsde_conv2d_fused", "irsde_layernorm",
-           "irsde_attention", "irsde_plan_num_ops", "irsde_plan_op_info", "irsde_trace_forward", "irsde_trim",
+           "irsde_attention", "irsde_linattn_block", "irsde_plan_num_ops", "irsde_plan_op_info", "irsde_trace_forward", "irsde_trim",
            "irsde_random_states", "irsde_nafnet_op", "irsde_time_embedding", "irsde_step_philox", "irsde_prep_input"]
 ATTN_LINEAR, ATTN_LINEAR_FOLD, ATTN_FULL = 0, 1, 2  # irsde_attention kinds
 NAF_DWGATE_SCA, NAF_SIMPLE_GATE, NAF_PIXEL_SHUFFLE_ADD, NAF_ADD = 0, 1, 2, 3  # irsde_nafnet_op kinds
@@ -125,6 +125,8 @@ def load():
     L.irsde_layernorm.restype = ctypes.c_int
     L.irsde_attention.argtypes = [vp, i32, i32, vp, i32, i32, vp, i32, i32, vp, i32, vp, i32, i32, ctypes.POINTER(i32), vp]
     L.irsde_attention.restype = ctypes.c_int
+    L.irsde_linattn_block.argtypes = [vp, vp, i32, i32, vp, i32, i32, vp, vp, vp, vp, vp, vp, i32, i32, i32, vp]
+    L.irsde_linattn_block.restype = ctypes.c_int
     L.irsde_nafnet_op.argtypes = [vp, i32, i32, ctypes.POINTER(NafArgs), i32, i32, i32, i32, ctypes.POINTER(i32), vp]
     L.irsde_nafnet_op.restype = ctypes.c_int
     L.irsde_time_embedding.argtypes = [i32, vp, i32, i32, vp, vp, vp, vp, vp, vp, i32, vp, vp, vp]

@@ -6,7 +6,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libirsde_b200.so")
-SOURCES = ["engine.cu", "conv_simt.cu", "conv_tc.cu", "elementwise.cu", "attention.cu", "nafnet.cu", "imaging.cu"]
+SOURCES = ["engine.cu", "conv_simt.cu", "conv_tc.cu", "elementwise.cu", "attention.cu", "linattn_fused.cu", "nafnet.cu", "imaging.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
          "-cudart", "static"]

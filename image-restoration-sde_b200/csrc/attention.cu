@@ -7,6 +7,7 @@
 #include <string.h>
 
 #include "common.cuh"
+#include "la_mma.cuh"
 
 namespace irsde {
 
@@ -336,9 +337,7 @@ template void launch_layernorm<bf16>(const bf16*, int, const float*, const bf16*
 //   pass B (la_combine8): merge the per-block partials: ctx[d][e] = sum_n softmax_n(k)[d,n] v[e,n] / N
 //   pass C (la_out): per pixel/head: q = softmax_d(q) * 32^-.5 ; out[e] = sum_d ctx[d][e] q[d]
 // =============================================================================================
-static const int LA_PIX = 64;               // pixels per chunk
-static const int LA_REC = 4 * (64 + 1024);  // floats per partial record (4 heads x (m[32], s[32], ctx[32][32]))
-static const int LA_MAXBLK = 64;            // partial records per image
+// LA_PIX, LA_REC, LA_MAXBLK: la_mma.cuh
 
 static int la_blocks_per_image(int B, int N) {
   const int nchunks = (N + LA_PIX - 1) / LA_PIX;
@@ -570,32 +569,10 @@ __global__ void __launch_bounds__(256) la_out_kernel(const T* __restrict__ qkv, 
 // Both operands are pixel-major in shared memory, so fragments come from ldmatrix.trans.
 // Warp w owns head w/2 and d-rows 16*(w%2)..+15 (4 n-tiles of 8 e's => 16 fp32 accumulators / thread).
 // ---------------------------------------------------------------------------------------------
-static const int LAM_TP = 264;  // tile row pitch (bf16): 256 + 8 pad -> conflict-free ldmatrix
-static const int LAM_PP = 136;  // P row pitch (bf16): 128 + 8 pad
 static const size_t LAM_SMEM = (size_t)2 * LA_PIX * LAM_TP * 2 + (size_t)LA_PIX * LAM_PP * 2 + 128 * 4;
 
-__device__ __forceinline__ void ldsm_x4_trans(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3)
-               : "r"(addr));
-}
-__device__ __forceinline__ float ex2_approx(float x) {  // 2^x, one MUFU (rel. error 2^-22; -inf -> +0)
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-__device__ __forceinline__ void mma_bf16_16816(float* c, uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0,
-                                               uint32_t b1) {
-  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-               : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
-}
-
-// The softmax statistics of a chunk stay inside a warp.  Lane (qtr = lane / 4, cpl = lane % 4) of warp w owns channel
-// pairs w*4+cpl and 32+w*4+cpl on the 8 pixels px == qtr (mod 8): the running max / sum live in registers (replicated over
-// the 8 qtr lanes), the cross-pixel max and sum are three xor-shuffles each, and the bf16x2 accesses
-// (word = 4*px + pair mod 32) are bank-conflict free.  One chunk needs two block barriers: tile landed, and P and alpha
-// visible to the MMA warps.
+// The chunk step (softmax statistics in registers, P^T V on the tensor cores) is la_chunk_softmax_pv (la_mma.cuh); one
+// chunk needs two block barriers: tile landed, and P and alpha visible to the MMA warps.
 __global__ void __launch_bounds__(256) la_kv_mma_kernel(const bf16* __restrict__ qkv, int pitch, float* __restrict__ part,
                                                         int N, int nchunks, int nblk) {
   PDL_ENTRY();
@@ -603,10 +580,9 @@ __global__ void __launch_bounds__(256) la_kv_mma_kernel(const bf16* __restrict__
   bf16* tile = reinterpret_cast<bf16*>(lam_sm);                          // [2][64][LAM_TP]  (k | v)
   bf16* Ps = tile + 2 * LA_PIX * LAM_TP;                                 // [64][LAM_PP]
   float* alpha_s = reinterpret_cast<float*>(Ps + LA_PIX * LAM_PP);       // [128]
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int tid = threadIdx.x;
   const int b = blockIdx.y, blk = blockIdx.x;
   const int c0 = (int)(((long long)nchunks * blk) / nblk), c1 = (int)(((long long)nchunks * (blk + 1)) / nblk);
-  const int h = warp >> 1, dbase = h * 32 + (warp & 1) * 16;
   float acc[4][4];
 #pragma unroll
   for (int i = 0; i < 4; ++i)
@@ -645,105 +621,16 @@ __global__ void __launch_bounds__(256) la_kv_mma_kernel(const bf16* __restrict__
   };
 
   if (c0 < c1) issue_load(c0, 0);
-  const float LOG2E = 1.4426950408889634f;
-  // statistics mapping and register-resident running statistics: [0,1] = pair A (lo, hi channel), [2,3] = pair B
-  const int sq = lane >> 2, pA = warp * 4 + (lane & 3), pB = 32 + pA;
   float mr[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY}, sr[4] = {0.f, 0.f, 0.f, 0.f};
   for (int ch = c0; ch < c1; ++ch) {
     const int buf = (ch - c0) & 1;
-    const bf16* T0 = tile + buf * LA_PIX * LAM_TP;
     asm volatile("cp.async.wait_group 0;" ::: "memory");
     __syncthreads();  // tile[buf] landed; everyone is done with tile[buf^1] and Ps of the previous chunk
     if (ch + 1 < c1) issue_load(ch + 1, buf ^ 1);
-    // ---- softmax statistics, branch-free: rows past the image hold k = -1e30 (see issue_load); ~13 instructions per bf16 pair
-    float k[16][2];
-    float mx[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const bf16* row = T0 + (i * 8 + sq) * LAM_TP;
-      const __nv_bfloat162 a = *reinterpret_cast<const __nv_bfloat162*>(row + 2 * pA);
-      const __nv_bfloat162 c = *reinterpret_cast<const __nv_bfloat162*>(row + 2 * pB);
-      k[i][0] = __low2float(a); k[i][1] = __high2float(a);
-      k[8 + i][0] = __low2float(c); k[8 + i][1] = __high2float(c);
-      mx[0] = fmaxf(mx[0], k[i][0]); mx[1] = fmaxf(mx[1], k[i][1]);
-      mx[2] = fmaxf(mx[2], k[8 + i][0]); mx[3] = fmaxf(mx[3], k[8 + i][1]);
-    }
-    float mn[4], mnl[4], ps[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-#pragma unroll
-      for (int o = 4; o < 32; o <<= 1) mx[c] = fmaxf(mx[c], __shfl_xor_sync(0xffffffffu, mx[c], o));
-      mn[c] = fmaxf(mr[c], mx[c]);
-      mnl[c] = mn[c] * LOG2E;
-    }
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      bf16* prow = Ps + (i * 8 + sq) * LAM_PP;
-      const __nv_bfloat162 qa = __floats2bfloat162_rn(ex2_approx(fmaf(k[i][0], LOG2E, -mnl[0])), ex2_approx(fmaf(k[i][1], LOG2E, -mnl[1])));
-      const __nv_bfloat162 qb = __floats2bfloat162_rn(ex2_approx(fmaf(k[8 + i][0], LOG2E, -mnl[2])), ex2_approx(fmaf(k[8 + i][1], LOG2E, -mnl[3])));
-      ps[0] += __low2float(qa);   // sum the rounded values the MMA will actually use
-      ps[1] += __high2float(qa);
-      ps[2] += __low2float(qb);
-      ps[3] += __high2float(qb);
-      *reinterpret_cast<__nv_bfloat162*>(prow + 2 * pA) = qa;
-      *reinterpret_cast<__nv_bfloat162*>(prow + 2 * pB) = qb;
-    }
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-#pragma unroll
-      for (int o = 4; o < 32; o <<= 1) ps[c] += __shfl_xor_sync(0xffffffffu, ps[c], o);
-      const float a = ex2_approx((mr[c] - mn[c]) * LOG2E);  // 0 on the first chunk (mr = -inf)
-      sr[c] = sr[c] * a + ps[c];
-      mr[c] = mn[c];
-      if (sq == 0) alpha_s[2 * (c < 2 ? pA : pB) + (c & 1)] = a;
-    }
-    __syncthreads();  // P and alpha visible to the MMA warps
-    // ---- rescale and accumulate: rows g / g+8 of this warp's 16 d-rows
-    {
-      const float al_lo = alpha_s[dbase + (lane >> 2)], al_hi = alpha_s[dbase + (lane >> 2) + 8];
-#pragma unroll
-      for (int nt = 0; nt < 4; ++nt) { acc[nt][0] *= al_lo; acc[nt][1] *= al_lo; acc[nt][2] *= al_hi; acc[nt][3] *= al_hi; }
-    }
-    const uint32_t Pbase = (uint32_t)__cvta_generic_to_shared(Ps);
-    const uint32_t Vbase = (uint32_t)__cvta_generic_to_shared(T0);
-    const int mi = lane >> 3, r8 = lane & 7;  // ldmatrix: lane supplies row r8 of matrix mi
-#pragma unroll
-    for (int ks = 0; ks < 4; ++ks) {
-      const int k0 = ks * 16;
-      uint32_t a0, a1, a2, a3;
-      // A = P^T: matrices (k0-7,m0-7) (k0-7,m8-15) (k8-15,m0-7) (k8-15,m8-15) -> a0,a1,a2,a3 after transpose
-      ldsm_x4_trans(Pbase + (uint32_t)(((k0 + (mi >> 1) * 8 + r8) * LAM_PP + dbase + (mi & 1) * 8) * 2), a0, a1, a2, a3);
-#pragma unroll
-      for (int np = 0; np < 2; ++np) {  // two pairs of n-tiles (16 e's each)
-        uint32_t b0, b1, b2, b3;
-        // B = V: matrices (k0-7,n0-7) (k8-15,n0-7) (k0-7,n8-15) (k8-15,n8-15)
-        ldsm_x4_trans(Vbase + (uint32_t)(((k0 + (mi & 1) * 8 + r8) * LAM_TP + 128 + h * 32 + np * 16 + (mi >> 1) * 8) * 2), b0,
-                      b1, b2, b3);
-        mma_bf16_16816(acc[np * 2], a0, a1, a2, a3, b0, b1);
-        mma_bf16_16816(acc[np * 2 + 1], a0, a1, a2, a3, b2, b3);
-      }
-    }
+    la_chunk_softmax_pv(tile + buf * LA_PIX * LAM_TP, Ps, alpha_s, mr, sr, acc);
   }
   __syncthreads();
-  float* rec = part + ((long long)b * LA_MAXBLK + blk) * LA_REC;
-  if (sq == 0) {
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-      const int chn = 2 * (c < 2 ? pA : pB) + (c & 1);
-      rec[(chn >> 5) * 1088 + (chn & 31)] = mr[c];
-      rec[(chn >> 5) * 1088 + 32 + (chn & 31)] = sr[c];
-    }
-  }
-  {
-    const int g = lane >> 2, t4 = lane & 3, drow = (warp & 1) * 16 + g;
-    float* cp = rec + h * 1088 + 64;
-#pragma unroll
-    for (int nt = 0; nt < 4; ++nt) {
-      const int e = nt * 8 + t4 * 2;
-      *reinterpret_cast<float2*>(cp + drow * 32 + e) = make_float2(acc[nt][0], acc[nt][1]);
-      *reinterpret_cast<float2*>(cp + (drow + 8) * 32 + e) = make_float2(acc[nt][2], acc[nt][3]);
-    }
-  }
+  la_store_record(part + ((long long)b * LA_MAXBLK + blk) * LA_REC, mr, sr, acc);
 }
 
 static bool g_la_attr_done = false;
@@ -762,6 +649,12 @@ void launch_la_kv<bf16>(const bf16* qkv, int qkv_pitch, float* partial, int B, i
   pdl_launch(la_kv_mma_kernel, dim3(nblk, B), 256, LAM_SMEM, st, qkv, qkv_pitch, partial, N, nchunks, nblk);
 }
 
+void launch_la_combine(const float* partial, float* ctx, int B, int N, cudaStream_t st) {
+  int nblk, nchunks;
+  linattn_partition(B, N, &nblk, &nchunks);
+  pdl_launch(la_combine8_kernel, B * 4 * 8, 256, 0, st, partial, ctx, N, nblk);
+}
+
 template <typename T>
 bool launch_linattn_ctx(const T* qkv, int qkv_pitch, float* partial, float* ctx, int B, int N, cudaStream_t st) {
   if (!linattn_views_ok(qkv, qkv_pitch, nullptr, 0, sizeof(T))) return false;
@@ -774,7 +667,7 @@ bool launch_linattn_ctx(const T* qkv, int qkv_pitch, float* partial, float* ctx,
     g_la_attr_done = true;
   }
   launch_la_kv<T>(qkv, qkv_pitch, partial, B, N, nchunks, nblk, smem, st);
-  pdl_launch(la_combine8_kernel, B * 4 * 8, 256, 0, st, partial, ctx, N, nblk);
+  launch_la_combine(partial, ctx, B, N, st);
   return true;
 }
 template bool launch_linattn_ctx<float>(const float*, int, float*, float*, int, int, cudaStream_t);
@@ -913,15 +806,6 @@ __global__ void __launch_bounds__(128) fullattn_kernel(const T* __restrict__ qkv
 // pipe does.  It stays on mma.sync, whose operands come straight from registers.
 // ---------------------------------------------------------------------------------------------
 static const int FA_Q = 64, FA_K = 64, FA_P = 40;  // queries / keys per block; smem row pitch (32 + 8 pad, bf16)
-__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3)
-               : "r"(addr));
-}
-__device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
-  __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
-  return *reinterpret_cast<uint32_t*>(&v);
-}
 __global__ void __launch_bounds__(128) fullattn_mma_kernel(const bf16* __restrict__ qkv, int pitch, bf16* __restrict__ hidden,
                                                            int hid_pitch, int N) {
   PDL_ENTRY();

@@ -166,6 +166,18 @@ void linattn_partition(int B, int N, int* nblk, int* nchunks);
 template <typename T>
 bool launch_linattn_ctx(const T* qkv, int qkv_pitch, float* partial, float* ctx, int B, int N, cudaStream_t st);
 void launch_la_fold(const float* ctx, const float* wout, bf16* Mb, int B, int C, cudaStream_t st);
+// pass B alone: merge pass A's partial records into ctx [B][4][32][32]
+void launch_la_combine(const float* partial, float* ctx, int B, int N, cudaStream_t st);
+// Residual(PreNorm(LinearAttention)) in two fused passes over x (linattn_fused.cu, bf16, C = 64 or 128):
+//   launch_la_kv_ln: LayerNorm(x; g1), k|v = W_kv xn (W_kv = rows 128..383 of the packed to_qkv weight, [256][C]), pass A's
+//                    partial records (then launch_la_combine, launch_la_fold); xn_dump (tests; null in the plan) gets xn
+//   launch_la_out_ln: out = LayerNorm(Mb[b] softmax_h(W_q xn) + bias; g2) + x  (W_q = rows 0..127, [128][C])
+// linattn_fused_ok: C and the views the fused passes take (x: 16-byte vectors, out: bf16 pairs)
+bool linattn_fused_ok(int C, const void* x, int x_pitch, const void* out, int out_pitch);
+void launch_la_kv_ln(const bf16* x, int x_pitch, const float* g1, const bf16* wkv, float* partial, int B, int N, int C,
+                     bf16* xn_dump, cudaStream_t st);
+void launch_la_out_ln(const bf16* x, int x_pitch, const float* g1, const bf16* wq, const bf16* Mb, const float* bias,
+                      const float* g2, bf16* out, int out_pitch, int B, int N, int C, cudaStream_t st);
 // full softmax attention (denoising-sde mid_attn): qkv [B,N,384] -> hidden [B,N,128]; fullattn_pick is the kernel
 // launch_fullattn runs (FA_MMA: bf16 only)
 enum FullAttnKernel { FA_SCALAR = 0, FA_MMA = 1 };

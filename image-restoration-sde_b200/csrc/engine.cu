@@ -709,6 +709,12 @@ struct Builder {
   void attention(const std::string& pre, V in, V out, int H, int W, bool full, float* la_partial, float* la_ctx) {
     int C = in.C, B = plan->B, N = H * W;
     long long npix = (long long)B * N;
+    if constexpr (std::is_same<T, bf16>::value) {
+      if (!full && ctx->use_tc && linattn_fused_ok(C, in.p, in.pitch, out.p, out.pitch)) {
+        linattn_fused(pre, in, out, H, W, la_partial, la_ctx);
+        return;
+      }
+    }
     T* xn = tmp(npix * C);
     float* g1 = fw(pre + "fn.norm.g");
     irsde_ctx* c = ctx;
@@ -796,6 +802,46 @@ struct Builder {
     }
     release(qkv);
     release(hid);
+  }
+
+  // Residual(PreNorm(LinearAttention)) for C = 64 / 128 (bf16): two fused passes over x (linattn_fused.cu) around the combine
+  // and the fold, four launches instead of seven, and none of the xn, qkv and y tensors.  W_q and W_kv are rows 0..127 and
+  // 128..383 of the packed to_qkv weight ([384][C], irsde_finalize_weights).
+  void linattn_fused(const std::string& pre, V in, V out, int H, int W, float* la_partial, float* la_ctx) {
+    const int C = in.C, B = plan->B, N = H * W;
+    const long long npix = (long long)B * N;
+    irsde_ctx* c = ctx;
+    const bf16* wqkv = ctx->w_tc[pre + "fn.fn.to_qkv.weight"];
+    if (!wqkv) { ok = false; err = "unpacked tc weight " + pre + "fn.fn.to_qkv.weight"; return; }
+    float* g1 = fw(pre + "fn.norm.g");
+    plan->ops.push_back(OpRec{CAT_ATTN, 0.0, [=](Plan*, cudaStream_t st) {
+      launch_la_kv_ln(in.p, in.pitch, g1, wqkv + 128 * C, la_partial, B, N, C, nullptr, st);
+      c->launches++;
+    }});
+    plan->ops.back().label = pre + "norm+to_qkv k,v+linattn kv (fused)";
+    plan->ops.back().bytes = (double)npix * C * sizeof(T);
+    plan->ops.push_back(OpRec{CAT_ATTN, 0.0, [=](Plan*, cudaStream_t st) {
+      launch_la_combine(la_partial, la_ctx, B, N, st);
+      c->launches++;
+    }});
+    plan->ops.back().label = pre + "linattn combine";
+    bf16* Mb = tmp((long long)B * C * 128);
+    float* wout = fw(pre + "fn.fn.to_out.0.weight");
+    plan->ops.push_back(OpRec{CAT_ATTN, 0.0, [=](Plan*, cudaStream_t st) {
+      launch_la_fold(la_ctx, wout, Mb, B, C, st);
+      c->launches++;
+    }});
+    plan->ops.back().label = pre + "fold ctx into to_out";
+    float* bout = fw(pre + "fn.fn.to_out.0.bias");
+    float* g2 = fw(pre + "fn.fn.to_out.1.g");
+    plan->ops.push_back(OpRec{CAT_ATTN, 0.0, [=](Plan*, cudaStream_t st) {
+      launch_la_out_ln(in.p, in.pitch, g1, wqkv, Mb, bout, g2, out.p, out.pitch, B, N, C, st);
+      c->launches++;
+    }});
+    plan->ops.back().label = pre + "to_out.norm+res";
+    plan->ops.back().bytes = 2.0 * npix * C * sizeof(T);
+    mark_out(out, H, W);
+    release(Mb);
   }
 
   // ---- latent autoencoder UNet.encode / UNet.decode (UNet_arch.py:59-91) --------------------------------------
@@ -2490,6 +2536,49 @@ int irsde_attention(irsde_ctx* ctx, int32_t precision, int32_t kind, const float
     ctx->launches += lin ? 3 : 1;
   }
   return finish_op(ctx, rc, "attention failed: ", st, tmp);
+}
+
+int irsde_linattn_block(irsde_ctx* ctx, const float* x, int32_t x_pitch, int32_t x_off, float* out, int32_t out_pitch,
+                        int32_t out_off, const float* g1, const float* wqkv, const float* wout, const float* bout, const float* g2,
+                        float* xn_out, int32_t B, int32_t N, int32_t C, void* stream) {
+  // ---- everything is validated here, before the first allocation or launch
+  if (!ctx || !x || !out || !g1 || !wqkv || !wout || !bout || !g2) return fail(ctx, IRSDE_ERR_INVALID, "null argument");
+  if (B < 1 || B > 16383 || N < 1) return fail(ctx, IRSDE_ERR_INVALID, "bad shape");
+  if (C != 64 && C != 128) return fail(ctx, IRSDE_ERR_UNSUPPORTED, "the fused linear-attention block takes C = 64 or 128");
+  if (x_off < 0 || (long long)x_off + C > x_pitch) return fail(ctx, IRSDE_ERR_INVALID, "input view outside its pitch");
+  if (out_off < 0 || (long long)out_off + C > out_pitch) return fail(ctx, IRSDE_ERR_INVALID, "output view outside its pitch");
+  if (x_pitch % 8 || x_off % 8 || out_pitch % 2 || out_off % 2)
+    return fail(ctx, IRSDE_ERR_INVALID, "input view: pitch and offset multiples of 8; output view: multiples of 2");
+  if (((uintptr_t)g1 | (uintptr_t)g2 | (uintptr_t)bout | (uintptr_t)wout) & 15)
+    return fail(ctx, IRSDE_ERR_INVALID, "g1, g2, bout and wout must start on 16 bytes");
+  cudaSetDevice(ctx->cfg.device);
+  cudaStream_t st = (cudaStream_t)stream;
+  const long long npix = (long long)B * N, nx = npix * x_pitch, no = npix * out_pitch;
+  std::vector<void*> tmp;
+  int rc = IRSDE_OK;
+  float* part = (float*)dev_alloc(ctx, linattn_partial_floats(B, N) * sizeof(float), &tmp);
+  float* cx = (float*)dev_alloc(ctx, (size_t)B * 4096 * sizeof(float), &tmp);
+  bf16* xb = (bf16*)dev_alloc(ctx, nx * 2, &tmp);
+  bf16* ob = (bf16*)dev_alloc(ctx, no * 2, &tmp);
+  bf16* wp = (bf16*)dev_alloc(ctx, (size_t)384 * C * 2, &tmp);
+  bf16* Mb = (bf16*)dev_alloc(ctx, (size_t)B * C * 128 * 2, &tmp);
+  bf16* xnb = xn_out ? (bf16*)dev_alloc(ctx, npix * C * 2, &tmp) : nullptr;
+  if (!part || !cx || !xb || !ob || !wp || !Mb || (xn_out && !xnb)) rc = fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
+  if (!rc && !linattn_fused_ok(C, xb + x_off, x_pitch, ob + out_off, out_pitch))
+    rc = fail(ctx, IRSDE_ERR_INVALID, "the fused linear-attention passes refused the views");
+  if (!rc) {
+    cast_f32_bf16_kernel<<<cast_blocks(nx), 256, 0, st>>>(x, xb, nx);
+    cast_f32_bf16_kernel<<<cast_blocks(no), 256, 0, st>>>(out, ob, no);
+    pack_weight<bf16>(WL_TAPS, wqkv, wp, 384, C, 1, 1, 1, st);  // the layout irsde_finalize_weights gives to_qkv
+    launch_la_kv_ln(xb + x_off, x_pitch, g1, wp + 128 * C, part, B, N, C, xnb, st);
+    launch_la_combine(part, cx, B, N, st);
+    launch_la_fold(cx, wout, Mb, B, C, st);
+    launch_la_out_ln(xb + x_off, x_pitch, g1, wp, Mb, bout, g2, ob + out_off, out_pitch, B, N, C, st);
+    cast_bf16_f32_kernel<<<cast_blocks(no), 256, 0, st>>>(ob, out, no);
+    if (xnb) cast_bf16_f32_kernel<<<cast_blocks(npix * C), 256, 0, st>>>(xnb, xn_out, npix * C);
+    ctx->launches += 4;
+  }
+  return finish_op(ctx, rc, "linear-attention block failed: ", st, tmp);
 }
 
 // ---- one NAFNet op, time embedding, sampler step or input packing outside a plan ----------------------------------

@@ -288,6 +288,19 @@ int irsde_attention(irsde_ctx* ctx, int32_t precision, int32_t kind, const float
                     float* out, int32_t out_pitch, int32_t out_off, const float* wout, int32_t Cout, float* ctx_out, int32_t B,
                     int32_t N, int32_t* info, void* stream);
 
+/* One whole Residual(PreNorm(LinearAttention)) block (module_util.py:150-178) on the bf16 path, C = 64 or 128, as the
+ * launch plan runs it: two fused passes over x (LayerNorm + k,v projection + the context partials; LayerNorm + q projection
+ * + q softmax + to_out with the folded context + LayerNorm + residual) around the combine and the fold.
+ *   x     fp32 [B*N][x_pitch], the block input at channels x_off .. x_off+C-1 (x_pitch, x_off multiples of 8);
+ *   out   fp32 [B*N][out_pitch], the block output written at channels out_off .. out_off+C-1 (even pitch and offset);
+ *   g1    fn.norm.g [C]; wqkv fn.fn.to_qkv.weight [384][C]; wout fn.fn.to_out.0.weight [C][128]; bout its bias [C];
+ *   g2    fn.fn.to_out.1.g [C] (g1, g2, bout and wout start on 16 bytes);
+ *   xn_out NULL, or fp32 [B*N][C]: the bf16 LayerNorm(x) the first pass computes.
+ * Buffers are converted as in irsde_layernorm. */
+int irsde_linattn_block(irsde_ctx* ctx, const float* x, int32_t x_pitch, int32_t x_off, float* out, int32_t out_pitch,
+                        int32_t out_off, const float* g1, const float* wqkv, const float* wout, const float* bout, const float* g2,
+                        float* xn_out, int32_t B, int32_t N, int32_t C, void* stream);
+
 /* One NAFBlock op of the launch plan (DenoisingNAFNet_arch.py:9-12,29-33,65-67; the decoder's PixelShuffle + skip, :172-174;
  * the latent variant's x + intro(x)).  x, y and out are fp32 NHWC buffers read or written through (pitch, channel offset)
  * views; views need not be aligned.  Pixel counts: x and (for ADD) y hold B*H*W pixels; for PIXEL_SHUFFLE_ADD, H x W is the
