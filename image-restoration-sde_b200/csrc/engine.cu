@@ -133,6 +133,8 @@ struct irsde_ctx {
   std::vector<ProfEv> prof_events;
   bool use_tc = false;  // bf16 mode: route eligible convs through the wgmma tap-GEMM engine
   std::vector<int> udim;  // UNet channels per level: nf * [1, ch_mult...] (DenoisingUNet_arch.py:51-56)
+  cudaEvent_t order_ev = nullptr;    // end of the work the last stream-ordered call enqueued (StreamOrder)
+  cudaStream_t order_st = nullptr;   // the stream that call ran on
 };
 
 namespace {
@@ -159,6 +161,24 @@ int fail(const irsde_ctx* ctx, int code, const std::string& msg) {
 constexpr size_t kTimeMlpSmemMax = 48 * 1024;
 // sca_kernel keeps the c channel means in dynamic shared memory, under the same limit
 constexpr int kScaMaxC = 48 * 1024 / 4;
+
+// The calls that use a context's plans, time tables or uid buffer (noise_fn, reverse, trace_forward, latent encode /
+// decode, set_image_uids, noise_state_images, step_philox) share those buffers whatever stream they run on.  One event
+// per context serializes them: every such call records it on its stream when it returns, and a call on another stream
+// than the previous one first makes its stream wait for it.  No launch is added.
+struct StreamOrder {
+  irsde_ctx* ctx;
+  cudaStream_t st;
+  StreamOrder(irsde_ctx* c, cudaStream_t s) : ctx(c), st(s) {
+    if (!ctx->order_ev) cudaEventCreateWithFlags(&ctx->order_ev, cudaEventDisableTiming);
+    else if (ctx->order_st != st) cudaStreamWaitEvent(st, ctx->order_ev, 0);
+  }
+  ~StreamOrder() {
+    if (!ctx->order_ev) return;
+    cudaEventRecord(ctx->order_ev, st);
+    ctx->order_st = st;
+  }
+};
 
 void* dev_alloc(irsde_ctx* ctx, size_t bytes, std::vector<void*>* owner) {
   void* p = nullptr;
@@ -1297,6 +1317,13 @@ int build_plan(irsde_ctx* ctx, int B, int H, int W, Plan** out) {
   p->fwd_times = (float*)dev_alloc(ctx, (size_t)B * 4, &p->allocs);
   p->fwd_temb = (float*)dev_alloc(ctx, (size_t)B * td * 4, &p->allocs);
   p->fwd_table = (float*)dev_alloc(ctx, (size_t)B * ctx->S * 4, &p->allocs);
+  if (ok && p->x_state && p->mu_buf && p->eps_buf && p->d_step && p->d_zero && p->fwd_table) {
+    cudaMemset(p->d_zero, 0, sizeof(int));
+    // The stem's zero border and d_zero are set on the legacy stream, which non-blocking streams do not wait for: the
+    // plan is complete on the device before any of its work is enqueued, whatever stream runs it.
+    cudaError_t se = cudaDeviceSynchronize();
+    if (se != cudaSuccess) { ok = false; err = std::string("plan setup failed: ") + cudaGetErrorString(se); }
+  }
   if (!ok || !p->x_state || !p->mu_buf || !p->eps_buf || !p->d_step || !p->d_zero || !p->fwd_table) {
     for (auto* d : p->tc_descs) tc_conv_destroy(d);
     for (void* q : p->allocs) cudaFree(q);
@@ -1304,7 +1331,6 @@ int build_plan(irsde_ctx* ctx, int B, int H, int W, Plan** out) {
     delete p;
     return fail(ctx, IRSDE_ERR_CUDA, err.empty() ? "plan allocation failed" : err);
   }
-  cudaMemset(p->d_zero, 0, sizeof(int));
   p->bytes = ctx->dev_bytes - bytes_before;
   p->last_use = ++ctx->use_clock;
   ctx->plan_bytes += p->bytes;
@@ -1381,6 +1407,8 @@ int upload_coeffs(irsde_ctx* ctx, int mode, const float* tab, int T) {
   if (T > 4096) return fail(ctx, IRSDE_ERR_UNSUPPORTED, "T > 4096 not supported");
   CUDA_TRY(ctx, cudaDeviceSynchronize());  // chains in flight on non-blocking streams still read the old table
   CUDA_TRY(ctx, cudaMemcpy(ctx->coef_dev[mode], tab, bytes, cudaMemcpyHostToDevice));
+  // a pageable copy returns once staged; its DMA runs on the legacy stream, which later chains do not wait for
+  CUDA_TRY(ctx, cudaDeviceSynchronize());
   return IRSDE_OK;
 }
 
@@ -1410,7 +1438,8 @@ int ensure_chain_table(irsde_ctx* ctx, Plan* p, int T, cudaStream_t st) {
     { const long long add = ((long long)cap * 4 + (long long)cap * td * 4 + (long long)cap * ctx->S * 4); p->bytes += add; ctx->plan_bytes += add; }
     std::vector<float> tv(cap);
     for (int i = 0; i < cap; ++i) tv[i] = (float)i;
-    CUDA_TRY(ctx, cudaMemcpy(p->chain_times, tv.data(), (size_t)cap * 4, cudaMemcpyHostToDevice));
+    // pageable source: staged before the call returns, copied in the caller's stream order ahead of time_rows below
+    CUDA_TRY(ctx, cudaMemcpyAsync(p->chain_times, tv.data(), (size_t)cap * 4, cudaMemcpyHostToDevice, st));
     p->chain_cap = cap;
     for (int m = 0; m < IRSDE_NUM_MODES; ++m)
       if (p->graph[m]) { cudaGraphExecDestroy(p->graph[m]); p->graph[m] = nullptr; }
@@ -1563,6 +1592,7 @@ static int latent_run(irsde_ctx* ctx, bool decode, const float* in, float* out, 
   if (!ctx->finalized) return fail(ctx, IRSDE_ERR_STATE, "weights not finalized");
   cudaSetDevice(ctx->cfg.device);
   cudaStream_t st = (cudaStream_t)stream;
+  StreamOrder order(ctx, st);
   Plan* p;
   auto key = std::make_tuple(B, H, W);
   bool existed = ctx->plans.find(key) != ctx->plans.end();
@@ -1736,6 +1766,7 @@ void irsde_destroy(irsde_ctx* ctx) {
   if (ctx->nccl_comm && g_nccl.CommDestroy) g_nccl.CommDestroy(ctx->nccl_comm);
   cudaSetDevice(ctx->cfg.device);
   cudaDeviceSynchronize();
+  if (ctx->order_ev) cudaEventDestroy(ctx->order_ev);
   for (auto& kv : ctx->plans) free_plan(ctx, kv.second);
   ctx->plans.clear();
   for (void* q : ctx->allocs) cudaFree(q);
@@ -1746,9 +1777,11 @@ int irsde_load_tensor(irsde_ctx* ctx, const char* name, const void* data, int32_
   if (!ctx || !name || !data || ndim < 0 || ndim > 4) return fail(ctx, IRSDE_ERR_INVALID, "bad argument to irsde_load_tensor");
   cudaSetDevice(ctx->cfg.device);
   // Weights are pointer-stable buffers that captured step graphs read: a re-upload (load_state_dict, broadcast) must not
-  // overtake chains still in flight on the caller's (possibly non-blocking) streams.  The first tensor of an upload
-  // round drains the device; the copies below are synchronous, so later launches see the new values.
-  if (ctx->finalized || ctx->raw.empty()) CUDA_TRY(ctx, cudaDeviceSynchronize());
+  // overtake chains still in flight on the caller's (possibly non-blocking) streams, and `data` may be a device tensor
+  // that such a stream is still writing.  A device-to-device cudaMemcpy orders itself against neither, so every copy
+  // waits for all earlier device work, and the call returns only once its copy is complete (the caller may free or
+  // reuse `data` at once).
+  CUDA_TRY(ctx, cudaDeviceSynchronize());
   long long n = 1;
   std::vector<int64_t> sh(shape, shape + ndim);
   for (auto d : sh) n *= d;
@@ -1761,6 +1794,7 @@ int irsde_load_tensor(irsde_ctx* ctx, const char* name, const void* data, int32_
   t.shape = sh;
   t.numel = n;
   CUDA_TRY(ctx, cudaMemcpy(t.dev, data, (size_t)n * 4, cudaMemcpyDefault));
+  CUDA_TRY(ctx, cudaDeviceSynchronize());
   ctx->finalized = false;
   return IRSDE_OK;
 }
@@ -1865,6 +1899,7 @@ int irsde_noise_fn(irsde_ctx* ctx, const float* x, const float* mu, const float*
   if (n_times != 1 && n_times != B) return fail(ctx, IRSDE_ERR_INVALID, "n_times must be 1 or B");
   cudaSetDevice(ctx->cfg.device);
   cudaStream_t st = (cudaStream_t)stream;
+  StreamOrder order(ctx, st);
   Plan* p;
   int rc = build_plan(ctx, B, H, W, &p);
   if (rc) return rc;
@@ -1906,6 +1941,7 @@ int irsde_reverse(irsde_ctx* ctx, int32_t mode, const float* xT, const float* mu
   if (ctx->cfg.in_nc != ctx->cfg.out_nc) return fail(ctx, IRSDE_ERR_INVALID, "chain needs in_nc == out_nc");
   cudaSetDevice(ctx->cfg.device);
   cudaStream_t st = (cudaStream_t)stream;
+  StreamOrder order(ctx, st);
   Plan* p;
   int rc = build_plan(ctx, B, H, W, &p);
   if (rc) return rc;
@@ -1979,6 +2015,7 @@ int irsde_noise_state_images(irsde_ctx* ctx, const float* mu, float* out, int32_
   if (!ctx->have_sched) return fail(ctx, IRSDE_ERR_STATE, "schedule not set");
   cudaSetDevice(ctx->cfg.device);
   if (ctx->n_uids && ctx->n_uids != B) return fail(ctx, IRSDE_ERR_INVALID, "irsde_set_image_uids count does not match the batch");
+  StreamOrder order(ctx, (cudaStream_t)stream);
   launch_noise_state(mu, out, (long long)B * image_elems, ctx->max_sigma, seed, image_elems, ctx->image_base,
                      ctx->n_uids ? ctx->d_uids : nullptr, (cudaStream_t)stream);
   ctx->launches++;
@@ -2011,6 +2048,7 @@ int irsde_set_image_uids(irsde_ctx* ctx, const uint64_t* uids, int32_t n, void* 
     ctx->d_uids = (unsigned long long*)dev_alloc(ctx, sizeof(unsigned long long) * MAX_UIDS, &ctx->allocs);
     if (!ctx->d_uids) return fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
   }
+  StreamOrder order(ctx, (cudaStream_t)stream);
   // pageable host source: the copy is staged before the call returns, so the caller may reuse `uids` at once
   CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_uids, uids, sizeof(uint64_t) * n, cudaMemcpyHostToDevice, (cudaStream_t)stream));
   ctx->n_uids = n;
@@ -2092,6 +2130,7 @@ int irsde_trace_forward(irsde_ctx* ctx, const float* x, const float* mu, const f
   if (n_times != 1 && n_times != B) return fail(ctx, IRSDE_ERR_INVALID, "n_times must be 1 or B");
   cudaSetDevice(ctx->cfg.device);
   cudaStream_t st = (cudaStream_t)stream;
+  StreamOrder order(ctx, st);
   Plan* p;
   int rc = build_plan(ctx, B, H, W, &p);
   if (rc) return rc;
@@ -2670,6 +2709,7 @@ int irsde_step_philox(irsde_ctx* ctx, int32_t mode, const float* x, const float*
   if (B < 1 || image_elems < 1) return fail(ctx, IRSDE_ERR_INVALID, "bad shape");
   if (ctx->n_uids && ctx->n_uids != B) return fail(ctx, IRSDE_ERR_INVALID, "irsde_set_image_uids count does not match the batch");
   cudaSetDevice(ctx->cfg.device);
+  StreamOrder order(ctx, (cudaStream_t)stream);
   launch_sde_update(mode, x, mu, noise, nullptr, 0, ctx->coef_dev[mode], nullptr, t, out, (long long)B * image_elems, seed,
                     image_elems, ctx->image_base, ctx->n_uids ? ctx->d_uids : nullptr, (cudaStream_t)stream);
   ctx->launches++;

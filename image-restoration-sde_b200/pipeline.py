@@ -106,6 +106,7 @@ class Restorer:
             for k, (shape, idx) in enumerate(batches):
                 dev, ev = staged
                 main.wait_event(ev)
+                dev.record_stream(main)   # allocated on the copy stream: its block must outlive the main stream's reads
                 res = self.restore_batch(dev, [first_uid + i for i in idx])
                 done = torch.cuda.Event()
                 done.record(main)

@@ -13,6 +13,24 @@
  *     the reference's torch tensors have); `stream` is a cudaStream_t passed as void*
  *     (torch.cuda.current_stream().cuda_stream);
  *   - weights are copied/repacked by the library; the caller keeps ownership of its buffers.
+ *
+ * Streams
+ *   - every entry with a `stream` argument reads its device inputs and writes its outputs in that stream's order (work
+ *     enqueued on the stream before the call is seen, work enqueued after it sees the outputs), on blocking and
+ *     non-blocking streams alike, and never uses the legacy default stream for it;
+ *   - these synchronize the device: irsde_set_schedule, irsde_set_coeffs, irsde_load_tensor (it waits for all earlier
+ *     device work before its copy and returns once the copy is complete, so `data` may come from any stream and may be
+ *     reused at once), irsde_finalize_weights, irsde_broadcast_weights, irsde_trim, irsde_destroy, irsde_profile_end*;
+ *     the standalone operator entries (irsde_conv2d*, irsde_layernorm, irsde_attention, irsde_linattn_block,
+ *     irsde_nafnet_op, irsde_time_embedding, irsde_prep_input) synchronize their stream and free their scratch memory,
+ *     which waits for the device;
+ *   - the first use of a (B, H, W) by a context (building its launch plan, including irsde_plan_num_ops /
+ *     irsde_plan_op_info) synchronizes the device, and the first graph capture of a mode may block the host; every
+ *     later call only enqueues work;
+ *   - calls on one context from different streams are serialized: a call that uses the context's plans, tables or uid
+ *     buffer (irsde_noise_fn, irsde_reverse, irsde_trace_forward, irsde_latent_encode / _decode, irsde_set_image_uids,
+ *     irsde_noise_state_images, irsde_step_philox) on another stream than the previous such call first makes its stream
+ *     wait for the work that call enqueued.
  */
 #ifndef IRSDE_B200_H
 #define IRSDE_B200_H
