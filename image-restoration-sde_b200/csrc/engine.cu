@@ -384,14 +384,16 @@ std::vector<NafBlockInfo> naf_blocks(const NafCfg& n) {
   }
   return v;
 }
-std::vector<ParamSpec> naf_param_specs(const NafCfg& n) {
+// variant: IRSDE_NET_CONDITIONAL reads cat(x - cond, cond); the denoising-sde task's network reads x alone
+// (codes/config/denoising-sde/models/modules/DenoisingNAFNet_arch.py:103)
+std::vector<ParamSpec> naf_param_specs(const NafCfg& n, int variant) {
   std::vector<ParamSpec> v;
   int64_t w = n.width, td = 4 * w, ic = n.img_channel;
   v.push_back({"time_mlp.1.weight", {2 * td, w}});
   v.push_back({"time_mlp.1.bias", {2 * td}});
   v.push_back({"time_mlp.3.weight", {td, td}});
   v.push_back({"time_mlp.3.bias", {td}});
-  v.push_back({"intro.weight", {w, 2 * ic, 3, 3}});
+  v.push_back({"intro.weight", {w, variant == IRSDE_NET_CONDITIONAL ? 2 * ic : ic, 3, 3}});
   v.push_back({"intro.bias", {w}});
   v.push_back({"ending.weight", {ic, w, 3, 3}});
   v.push_back({"ending.bias", {ic}});
@@ -1072,13 +1074,15 @@ struct Builder {
     naf_partial = (float*)dev_alloc(ctx, pmax * sizeof(float), &plan->allocs);
     naf_sca = (float*)dev_alloc(ctx, (size_t)B * cmax * sizeof(float), &plan->allocs);
     if (!naf_partial || !naf_sca) { ok = false; err = "cudaMalloc failed"; return; }
-    const int C0 = 2 * ic, pitch0 = (C0 + 7) / 8 * 8;
+    // conditional: intro reads cat(x - cond, cond); denoising-sde: x alone (DenoisingNAFNet_arch.py:103,147-150)
+    const int cond = ctx->cfg.variant == IRSDE_NET_CONDITIONAL ? 1 : 0;
+    const int C0 = cond ? 2 * ic : ic, pitch0 = (C0 + 7) / 8 * 8;
     const long long np0 = (long long)B * hs[0] * ws[0];
     T* X0 = alloc(np0 * pitch0);
     int Hh = plan->H, Ww = plan->W, Hp = plan->Hp, Wp = plan->Wp;
     irsde_ctx* cx = ctx;
     plan->ops.push_back(OpRec{CAT_MISC, 0.0, [=](Plan* p, cudaStream_t st) {
-      launch_prep_input<T>(p->cur.x, p->cur.mu, X0, B, ic, Hh, Ww, Hp, Wp, pitch0, 1, st, 0, 0, 0, 0, 1);  // zero pad
+      launch_prep_input<T>(p->cur.x, p->cur.mu, X0, B, ic, Hh, Ww, Hp, Wp, pitch0, cond, st, 0, 0, 0, 0, 1);  // zero pad
       cx->launches++;
     }});
     T* xin = alloc(np0 * w);
@@ -1622,7 +1626,14 @@ int irsde_latent_shape(irsde_ctx* ctx, int32_t H, int32_t W, int32_t* lat_h, int
 }
 
 int irsde_create_nafnet(const irsde_nafnet_config* ncfg, irsde_ctx** out) {
+  return irsde_create_nafnet_variant(ncfg, IRSDE_NET_CONDITIONAL, out);
+}
+
+int irsde_create_nafnet_variant(const irsde_nafnet_config* ncfg, int32_t variant, irsde_ctx** out) {
   if (!ncfg || !out) return fail(nullptr, IRSDE_ERR_INVALID, "null argument");
+  if (variant != IRSDE_NET_CONDITIONAL && variant != IRSDE_NET_DENOISING) return fail(nullptr, IRSDE_ERR_INVALID, "bad variant");
+  if (variant == IRSDE_NET_DENOISING && ncfg->latent)
+    return fail(nullptr, IRSDE_ERR_INVALID, "the latent NAFNet has no denoising variant");
   if (ncfg->width < 4 || ncfg->width % 2 || ncfg->img_channel < 1 || ncfg->n_levels < 0 || ncfg->n_levels > 8 ||
       ncfg->middle_blk_num < 0)
     return fail(nullptr, IRSDE_ERR_INVALID, "bad NAFNet configuration");
@@ -1635,7 +1646,8 @@ int irsde_create_nafnet(const irsde_nafnet_config* ncfg, irsde_ctx** out) {
   cfg.in_nc = cfg.out_nc = ncfg->img_channel;
   cfg.nf = ncfg->width;
   cfg.depth = ncfg->n_levels > 0 ? ncfg->n_levels : 1;
-  cfg.variant = IRSDE_NET_CONDITIONAL;
+  // the entry points that take mu (noise_fn, reverse, trace_forward) check it against this variant
+  cfg.variant = variant;
   cfg.precision = ncfg->precision;
   cfg.device = ncfg->device;
   cfg.flags = ncfg->flags;
@@ -1802,7 +1814,8 @@ int irsde_load_tensor(irsde_ctx* ctx, const char* name, const void* data, int32_
 int irsde_finalize_weights(irsde_ctx* ctx) {
   if (!ctx) return fail(nullptr, IRSDE_ERR_INVALID, "null ctx");
   cudaSetDevice(ctx->cfg.device);
-  auto specs = ctx->lat.on ? lat_param_specs(ctx->lat) : (ctx->naf.on ? naf_param_specs(ctx->naf) : param_specs(ctx->cfg, ctx->udim));
+  auto specs = ctx->lat.on ? lat_param_specs(ctx->lat)
+                           : (ctx->naf.on ? naf_param_specs(ctx->naf, ctx->cfg.variant) : param_specs(ctx->cfg, ctx->udim));
   for (auto& s : specs) {
     auto it = ctx->raw.find(s.name);
     if (it == ctx->raw.end()) return fail(ctx, IRSDE_ERR_STATE, "missing state-dict entry " + s.name);

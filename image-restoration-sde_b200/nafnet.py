@@ -1,6 +1,8 @@
 """``ConditionalNAFNet`` (Refusion's score network) with the reference's constructor, ``forward(inp, cond, time)``
 signature and state-dict names/shapes (codes/config/deraining/models/modules/DenoisingNAFNet_arch.py:87-188; latent
 variant codes/config/latent-dehazing/models/modules/DenoisingNAFNet_arch.py:147-181), executed by the native library.
+``DenoisingNAFNet`` is the denoising-sde task's class of the same name, ``forward(x, time)``
+(codes/config/denoising-sde/models/modules/DenoisingNAFNet_arch.py:103,147-150).
 """
 import ctypes
 
@@ -11,15 +13,16 @@ from . import _lib
 from .unet import ConditionalUNet, _Node
 
 
-def nafnet_param_shapes(img_channel, width, middle_blk_num, enc_blk_nums, dec_blk_nums):
-    """State-dict entries in the reference's registration order (DenoisingNAFNet_arch.py:15-49,89-143)."""
+def nafnet_param_shapes(img_channel, width, middle_blk_num, enc_blk_nums, dec_blk_nums, variant="conditional"):
+    """State-dict entries in the reference's registration order (DenoisingNAFNet_arch.py:15-49,89-143).  The
+    ``"denoising"`` variant's intro conv reads img_channel channels instead of 2 * img_channel."""
     S = {}
     td = width * 4
     S["time_mlp.1.weight"] = (td * 2, width)
     S["time_mlp.1.bias"] = (td * 2,)
     S["time_mlp.3.weight"] = (td, td)
     S["time_mlp.3.bias"] = (td,)
-    S["intro.weight"] = (width, img_channel * 2, 3, 3)
+    S["intro.weight"] = (width, img_channel * 2 if variant == "conditional" else img_channel, 3, 3)
     S["intro.bias"] = (width,)
     S["ending.weight"] = (img_channel, width, 3, 3)
     S["ending.bias"] = (img_channel,)
@@ -68,14 +71,15 @@ class _NafConfig(ctypes.Structure):
 
 
 class _NafContext(_lib.Context):
-    def __init__(self, img_channel, width, middle, enc, dec, latent, precision, device_index, force_simt=False):
+    def __init__(self, img_channel, width, middle, enc, dec, latent, precision, device_index, force_simt=False,
+                 variant=_lib.NET_CONDITIONAL):
         L = _lib.load()
-        L.irsde_create_nafnet.argtypes = [ctypes.POINTER(_NafConfig), ctypes.POINTER(ctypes.c_void_p)]
-        L.irsde_create_nafnet.restype = ctypes.c_int
+        L.irsde_create_nafnet_variant.argtypes = [ctypes.POINTER(_NafConfig), ctypes.c_int32, ctypes.POINTER(ctypes.c_void_p)]
+        L.irsde_create_nafnet_variant.restype = ctypes.c_int
         cfg = _NafConfig(img_channel, width, middle, len(enc), (ctypes.c_int32 * 8)(*enc), (ctypes.c_int32 * 8)(*dec),
                          1 if latent else 0, precision, device_index, 1 if force_simt else 0)
         h = ctypes.c_void_p()
-        _lib.check(L.irsde_create_nafnet(ctypes.byref(cfg), ctypes.byref(h)))
+        _lib.check(L.irsde_create_nafnet_variant(ctypes.byref(cfg), variant, ctypes.byref(h)))
         self.h = h
         self.L = L
 
@@ -100,7 +104,7 @@ class ConditionalNAFNet(ConditionalUNet):
         if self.precision not in _lib.PRECISIONS:
             raise ValueError("precision must be one of %s" % (sorted(_lib.PRECISIONS),))
         self._force_simt = force_simt
-        self._shapes = nafnet_param_shapes(img_channel, width, middle_blk_num, enc_blk_nums, dec_blk_nums)
+        self._shapes = nafnet_param_shapes(img_channel, width, middle_blk_num, enc_blk_nums, dec_blk_nums, self.variant)
         for name, shp in self._shapes.items():
             parts = name.split(".")
             node = self
@@ -125,8 +129,8 @@ class ConditionalNAFNet(ConditionalUNet):
             if self._ctx is not None:
                 self._ctx.close()
             self._ctx = _NafContext(self.img_channel, self.width, self.middle_blk_num, self.enc_blk_nums, self.dec_blk_nums,
-                                    self.latent, _lib.PRECISIONS[self.precision], idx,
-                                    force_simt=self._force_simt)
+                                    self.latent, _lib.PRECISIONS[self.precision], idx, force_simt=self._force_simt,
+                                    variant=_lib.NET_CONDITIONAL if self.variant == "conditional" else _lib.NET_DENOISING)
             self._ctx_dev = idx
             self._sig = None
         return self._ctx
@@ -134,3 +138,19 @@ class ConditionalNAFNet(ConditionalUNet):
     @torch.no_grad()
     def forward(self, inp, cond, time):
         return self._run(inp, cond, time)
+
+
+class DenoisingNAFNet(ConditionalNAFNet):
+    """The denoising-sde task's ``ConditionalNAFNet``: no condition input, intro conv over the img_channel channels of x
+    (codes/config/denoising-sde/models/modules/DenoisingNAFNet_arch.py:87-150).  Drives ``DenoisingSDE``."""
+
+    variant = "denoising"
+
+    def __init__(self, img_channel=3, width=16, middle_blk_num=1, enc_blk_nums=[], dec_blk_nums=[], upscale=1,
+                 precision=None, force_simt=False):
+        super().__init__(img_channel, width, middle_blk_num, enc_blk_nums, dec_blk_nums, upscale, False, precision,
+                         force_simt)
+
+    @torch.no_grad()
+    def forward(self, x, time):
+        return self._run(x, None, time)

@@ -8,7 +8,7 @@ What it does before handing control to the script (nothing in the reference tree
     cwd-local ``models``/``options`` and does ``sys.path.insert(0, "../../"); import utils``);
   * import the reference's ``utils`` package and swap ``IRSDE`` / ``DenoisingSDE`` for ours
     (codes/utils/sde_utils.py:80,373) - every other helper (img/file/deg utils) stays the reference's;
-  * import the task's ``models.modules`` and swap ``ConditionalUNet`` for ours (the factory is
+  * import the task's ``models.modules`` and swap ``ConditionalUNet`` and ``ConditionalNAFNet`` for ours (the factory is
     ``getattr(M, which_model_G)(**setting)``, models/networks.py:10-15), choosing the variant by the
     reference class's own ``forward`` signature (``(x, time)`` => denoising-sde variant);
   * provide tiny stand-ins for optional third-party modules the scripts import but this image lacks
@@ -89,17 +89,21 @@ def install(script_dir):
         utils.sde_utils.IRSDE = irsde_b200.IRSDE
         utils.sde_utils.DenoisingSDE = irsde_b200.DenoisingSDE
     mods = importlib.import_module("models.modules")
-    ref_cls = getattr(mods, "ConditionalUNet", None)
-    ours = irsde_b200.ConditionalUNet
-    if ref_cls is not None:
-        params = list(inspect.signature(ref_cls.forward).parameters)
-        if len(params) == 3:  # (self, x, time): denoising-sde variant
-            ours = irsde_b200.DenoisingUNet
-    mods.ConditionalUNet = ours
+
+    def denoising(name):  # (self, x, time): the denoising-sde variant of the reference class
+        ref_cls = getattr(mods, name, None)
+        return ref_cls is not None and len(inspect.signature(ref_cls.forward).parameters) == 3
+
+    mods.ConditionalUNet = irsde_b200.DenoisingUNet if denoising("ConditionalUNet") else irsde_b200.ConditionalUNet
     if hasattr(mods, "ConditionalNAFNet"):
         latent = "latent" in os.path.basename(os.path.abspath(script_dir))
         import functools
-        mods.ConditionalNAFNet = functools.partial(irsde_b200.ConditionalNAFNet, latent=latent) if latent else irsde_b200.ConditionalNAFNet
+        if latent:
+            mods.ConditionalNAFNet = functools.partial(irsde_b200.ConditionalNAFNet, latent=latent)
+        elif denoising("ConditionalNAFNet"):
+            mods.ConditionalNAFNet = irsde_b200.DenoisingNAFNet
+        else:
+            mods.ConditionalNAFNet = irsde_b200.ConditionalNAFNet
     if hasattr(mods, "UNet"):
         mods.UNet = irsde_b200.UNet
     return utils, mods

@@ -127,6 +127,11 @@ int irsde_create_ch_mult(const irsde_config* cfg, const int32_t* ch_mult, int32_
  * width << n_levels <= 12288: the time MLP (52 width bytes) and the SCA mat-vec (4 bytes per channel) fit in 48 KB of
  * shared memory. */
 int irsde_create_nafnet(const irsde_nafnet_config* cfg, irsde_ctx** out);
+/* irsde_create_nafnet with the network variant: IRSDE_NET_CONDITIONAL is irsde_create_nafnet; IRSDE_NET_DENOISING is the
+ * denoising-sde task's ConditionalNAFNet, whose intro conv reads the img_channel channels of x and whose forward takes
+ * no condition (codes/config/denoising-sde/models/modules/DenoisingNAFNet_arch.py:89-103,147).  That context drives the
+ * DenoisingSDE modes and takes mu == NULL; cfg->latent must be 0 with it. */
+int irsde_create_nafnet_variant(const irsde_nafnet_config* cfg, int32_t variant, irsde_ctx** out);
 void irsde_destroy(irsde_ctx* ctx);
 const char* irsde_last_error(const irsde_ctx* ctx);
 /* "irsde_b200 <version> sm_90a" */
