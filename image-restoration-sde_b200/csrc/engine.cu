@@ -162,6 +162,27 @@ constexpr size_t kTimeMlpSmemMax = 48 * 1024;
 // sca_kernel keeps the c channel means in dynamic shared memory, under the same limit
 constexpr int kScaMaxC = 48 * 1024 / 4;
 
+// The shape limits of the kernels' launches and index arithmetic (include/irsde_b200.h "Shape limits"), checked on the host
+// before anything is allocated or launched, by the plan builder and by every standalone entry:
+//   - a grid's y and z dimensions take at most 65535: the kernels put B there (the LinearAttention passes, dwgate / sca,
+//     the time table's rows, tensor2img / img2tensor / sqerr / ssim) and 4 B for full attention (one row per image and head);
+//   - the network kernels (dwgate / sca, LinearAttention, full attention, the tap-GEMM conv) hold the pixel count of one image
+//     (N = H * W, a pixel index inside it) in int: H * W <= 2^30.  The image entries index in long long and pass 1 x 1.
+// grid_rows is the largest value the caller's launches put in y or z, named by `what`; H, W is the largest image they see.
+constexpr long long kMaxGridYZ = 65535, kMaxImagePixels = 1LL << 30;
+int check_shape_limits(const irsde_ctx* ctx, long long grid_rows, const char* what, long long H, long long W) {
+  char b[256];
+  if (grid_rows > kMaxGridYZ) {
+    snprintf(b, sizeof b, "%s = %lld exceeds 65535, the CUDA grid y / z limit of the launches that index it", what, grid_rows);
+    return fail(ctx, IRSDE_ERR_INVALID, b);
+  }
+  if (H * W > kMaxImagePixels) {
+    snprintf(b, sizeof b, "an image of %lld x %lld pixels exceeds 2^30 pixels, the int pixel count of the kernels", H, W);
+    return fail(ctx, IRSDE_ERR_INVALID, b);
+  }
+  return IRSDE_OK;
+}
+
 // The calls that use a context's plans, time tables or uid buffer (noise_fn, reverse, trace_forward, latent encode /
 // decode, set_image_uids, noise_state_images, step_philox) share those buffers whatever stream they run on.  One event
 // per context serializes them: every such call records it on its stream when it returns, and a call on another stream
@@ -1292,6 +1313,14 @@ int build_plan(irsde_ctx* ctx, int B, int H, int W, Plan** out) {
   auto it = ctx->plans.find(key);
   if (it != ctx->plans.end()) { it->second->last_use = ++ctx->use_clock; *out = it->second; return IRSDE_OK; }
   if (B <= 0 || H <= 0 || W <= 0) return fail(ctx, IRSDE_ERR_INVALID, "bad image shape");
+  {
+    // every level runs on the image padded to a multiple of 2^levels; the denoising UNet's mid_attn is full attention
+    const long long sp = 1LL << (ctx->lat.on ? ctx->lat.depth : ctx->naf.on ? ctx->naf.n_enc : ctx->cfg.depth);
+    const bool full = !ctx->lat.on && !ctx->naf.on && ctx->cfg.variant == IRSDE_NET_DENOISING;
+    if (int rc = check_shape_limits(ctx, full ? 4LL * B : B, full ? "4 B (full-attention grid rows)" : "B",
+                                    (H + sp - 1) / sp * sp, (W + sp - 1) / sp * sp))
+      return rc;
+  }
   const long long bytes_before = ctx->dev_bytes;
   int s = 1 << ctx->cfg.depth;
   // reflect pad needs pad < size (F.pad 'reflect' raises otherwise, DenoisingUNet_arch.py:82)
@@ -2517,7 +2546,8 @@ int irsde_attention(irsde_ctx* ctx, int32_t precision, int32_t kind, const float
   if (kind < IRSDE_ATTN_LINEAR || kind > IRSDE_ATTN_FULL) return fail(ctx, IRSDE_ERR_INVALID, "unknown attention kind");
   const bool bf = precision == IRSDE_PREC_BF16, lin = kind != IRSDE_ATTN_FULL, fold = kind == IRSDE_ATTN_LINEAR_FOLD;
   if (fold && !bf) return fail(ctx, IRSDE_ERR_UNSUPPORTED, "the folded linear attention is the bf16 path");
-  if (B < 1 || B > 16383 || N < 1) return fail(ctx, IRSDE_ERR_INVALID, "bad shape");
+  if (B < 1 || N < 1) return fail(ctx, IRSDE_ERR_INVALID, "bad shape");
+  if (int rc = check_shape_limits(ctx, lin ? B : 4LL * B, lin ? "B" : "4 B (full-attention grid rows)", N, 1)) return rc;
   if (lin && !ctx_out) return fail(ctx, IRSDE_ERR_INVALID, "linear attention needs ctx_out");
   if (fold && (!wout || Cout < 1 || ((uintptr_t)wout & 15)))
     return fail(ctx, IRSDE_ERR_INVALID, "the fold needs 16-byte aligned to_out weights [Cout][128], Cout >= 1");
@@ -2595,7 +2625,8 @@ int irsde_linattn_block(irsde_ctx* ctx, const float* x, int32_t x_pitch, int32_t
                         float* xn_out, int32_t B, int32_t N, int32_t C, void* stream) {
   // ---- everything is validated here, before the first allocation or launch
   if (!ctx || !x || !out || !g1 || !wqkv || !wout || !bout || !g2) return fail(ctx, IRSDE_ERR_INVALID, "null argument");
-  if (B < 1 || B > 16383 || N < 1) return fail(ctx, IRSDE_ERR_INVALID, "bad shape");
+  if (B < 1 || N < 1) return fail(ctx, IRSDE_ERR_INVALID, "bad shape");
+  if (int rc = check_shape_limits(ctx, B, "B", N, 1)) return rc;
   if (C != 64 && C != 128) return fail(ctx, IRSDE_ERR_UNSUPPORTED, "the fused linear-attention block takes C = 64 or 128");
   if (x_off < 0 || (long long)x_off + C > x_pitch) return fail(ctx, IRSDE_ERR_INVALID, "input view outside its pitch");
   if (out_off < 0 || (long long)out_off + C > out_pitch) return fail(ctx, IRSDE_ERR_INVALID, "output view outside its pitch");
@@ -2642,8 +2673,8 @@ int irsde_nafnet_op(irsde_ctx* ctx, int32_t precision, int32_t kind, const irsde
   if (precision < IRSDE_PREC_FP32 || precision > IRSDE_PREC_FP32X3) return fail(ctx, IRSDE_ERR_INVALID, "bad precision");
   if (kind < IRSDE_NAF_DWGATE_SCA || kind > IRSDE_NAF_ADD) return fail(ctx, IRSDE_ERR_INVALID, "unknown NAFNet op");
   const bool dw = kind == IRSDE_NAF_DWGATE_SCA, ps = kind == IRSDE_NAF_PIXEL_SHUFFLE_ADD;
-  if (B < 1 || B > 65535 || H < 1 || W < 1 || c < 1 || (long long)H * W > (1LL << 30))
-    return fail(ctx, IRSDE_ERR_INVALID, "bad shape");
+  if (B < 1 || H < 1 || W < 1 || c < 1) return fail(ctx, IRSDE_ERR_INVALID, "bad shape");
+  if (int rc = check_shape_limits(ctx, B, "B", ps ? 2LL * H : H, ps ? 2LL * W : W)) return rc;
   if (dw && c > kScaMaxC) return fail(ctx, IRSDE_ERR_UNSUPPORTED, "c > 12288: the SCA mat-vec needs more than 48 KB of shared memory");
   if (dw && (!a.w || !a.bias || !a.sca_w || !a.sca_b || !a.sca)) return fail(ctx, IRSDE_ERR_INVALID, "DWGATE_SCA needs w, bias, sca_w, sca_b and sca");
   if ((ps || kind == IRSDE_NAF_ADD) && !a.y) return fail(ctx, IRSDE_ERR_INVALID, "PIXEL_SHUFFLE_ADD and ADD need y");
@@ -2735,7 +2766,8 @@ int irsde_time_embedding(int32_t family, const float* times, int32_t rows, int32
                          float* table, void* stream) {
   if (!times || !w1 || !b1 || !w2 || !b2 || !wall || !ball || !temb || !table) return fail(nullptr, IRSDE_ERR_INVALID, "null argument");
   if (family != 0 && family != 1) return fail(nullptr, IRSDE_ERR_INVALID, "family must be 0 (ConditionalUNet) or 1 (NAFNet)");
-  if (rows < 1 || rows > 65535 || S < 1 || width < 4 || width % 2) return fail(nullptr, IRSDE_ERR_INVALID, "bad shape");
+  if (rows < 1 || S < 1 || width < 4 || width % 2) return fail(nullptr, IRSDE_ERR_INVALID, "bad shape");
+  if (int rc = check_shape_limits(nullptr, rows, "rows", 1, 1)) return rc;
   if ((family == 0 ? time_mlp_smem(width) : naf_time_mlp_smem(width)) > kTimeMlpSmemMax)
     return fail(nullptr, IRSDE_ERR_UNSUPPORTED, "the time MLP of this width needs more than 48 KB of shared memory");
   cudaStream_t st = (cudaStream_t)stream;
@@ -2786,7 +2818,7 @@ int irsde_prep_input(int32_t precision, const float* xt, const float* cond, floa
 // ---- image conversion / metrics (stateless) ----------------------------------------------------------------
 static int img_args_ok(const void* a, const void* b, int B, int C, int H, int W) {
   if (!a || !b || B < 1 || H < 1 || W < 1 || (C != 1 && C != 3)) return fail(nullptr, IRSDE_ERR_INVALID, "bad image argument");
-  return IRSDE_OK;
+  return check_shape_limits(nullptr, B, "B", 1, 1);  // the image kernels index pixels in long long: only B is limited
 }
 static int img_launch_status(const char* what) {
   cudaError_t e = cudaGetLastError();

@@ -31,6 +31,18 @@
  *     buffer (irsde_noise_fn, irsde_reverse, irsde_trace_forward, irsde_latent_encode / _decode, irsde_set_image_uids,
  *     irsde_noise_state_images, irsde_step_philox) on another stream than the previous such call first makes its stream
  *     wait for the work that call enqueued.
+ *
+ * Shape limits
+ *   - the kernels put the batch in a CUDA grid's y or z dimension, which takes at most 65535: B <= 65535 for every network
+ *     and entry, and B <= 16383 where full softmax attention runs (IRSDE_NET_DENOISING UNets, IRSDE_ATTN_FULL), whose grid
+ *     has one row per image and head; likewise rows <= 65535 for irsde_time_embedding;
+ *   - the network kernels count the pixels of one image in int: H * W <= 2^30, where H x W is the image a network's first
+ *     level runs on (padded to a multiple of 2^levels), the attention's N, or the larger image of an irsde_nafnet_op (the
+ *     image entries index in 64 bits and limit only B);
+ *   - these are checked on the host before anything is allocated or launched, by the plan builder (irsde_noise_fn,
+ *     irsde_reverse, irsde_trace_forward, irsde_plan_num_ops / _op_info, irsde_latent_encode / _decode) and by the
+ *     standalone entries (irsde_attention, irsde_linattn_block, irsde_nafnet_op, irsde_time_embedding and the image entries);
+ *     a shape past a limit fails with IRSDE_ERR_INVALID and a message naming the limit.
  */
 #ifndef IRSDE_B200_H
 #define IRSDE_B200_H

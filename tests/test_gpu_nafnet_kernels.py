@@ -187,13 +187,15 @@ def test_philox_known_answers():
         assert got == want, ["%08x" % v for v in got]
 
 
-def philox_normals(seed, uids, image_elems, stream, swap_uid=False, swap_seed=False, swap_cs=False, blk_add=0):
+def philox_normals(seed, uids, image_elems, stream, swap_uid=False, swap_seed=False, swap_cs=False, blk_add=0, blocks=None):
     """z [len(uids), image_elems] (fp64) as the kernel draws it: element j of the image with uid u is lane j % 4 of Philox
     block j // 4 with counter (block, uid lo, stream, 0x1234567 ^ uid hi) and key (seed lo, seed hi); the uniforms are
-    formed in fp32 like normal4 forms them, Box-Muller in fp64 on them.  The keywords build the wrong generators."""
-    nb = (image_elems + 3) // 4
+    formed in fp32 like normal4 forms them, Box-Muller in fp64 on them.  The keywords build the wrong generators.
+    blocks = (b0, b1): only the elements 4 b0 .. 4 b1 - 1 of each image, [len(uids), 4 (b1 - b0)]."""
+    b0, b1 = blocks if blocks is not None else (0, (image_elems + 3) // 4)
+    nb = b1 - b0
     u = np.repeat(np.asarray([int(v) for v in uids], dtype=np.uint64), nb)
-    blk = (np.tile(np.arange(nb, dtype=np.int64), len(uids)) + blk_add) & 0xFFFFFFFF
+    blk = (np.tile(np.arange(b0, b1, dtype=np.int64), len(uids)) + blk_add) & 0xFFFFFFFF
     lo, hi = u & M32, u >> np.uint64(32)
     if swap_uid:
         lo, hi = hi, lo
