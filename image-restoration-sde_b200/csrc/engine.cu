@@ -201,11 +201,12 @@ struct StreamOrder {
   }
 };
 
+// ctx may be null (the entries that take no context): nothing is counted
 void* dev_alloc(irsde_ctx* ctx, size_t bytes, std::vector<void*>* owner) {
   void* p = nullptr;
   if (bytes == 0) bytes = 16;
   if (cudaMalloc(&p, bytes) != cudaSuccess) return nullptr;
-  ctx->dev_bytes += (long long)bytes;
+  if (ctx) ctx->dev_bytes += (long long)bytes;
   owner->push_back(p);
   return p;
 }
@@ -1481,7 +1482,7 @@ int ensure_chain_table(irsde_ctx* ctx, Plan* p, int T, cudaStream_t st) {
   return IRSDE_OK;
 }
 
-// ---- one tap-GEMM conv outside a plan (irsde_conv2d_ex, irsde_conv2d_fused) ------------------------------------------
+// ---- the standalone entries' scratch and conv body (irsde_conv2d_ex ... irsde_prep_input) ---------------------------------
 __global__ void cast_f32_bf16_kernel(const float* __restrict__ in, bf16* __restrict__ out, long long n) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
     out[i] = __float2bfloat16_rn(in[i]);
@@ -1491,55 +1492,151 @@ __global__ void cast_bf16_f32_kernel(const bf16* __restrict__ in, float* __restr
     out[i] = __bfloat162float(in[i]);
 }
 
-// Runs the conv the plan builder would make of this shape: `in` is an NHWC view in the engine's storage type S (bf16, or
-// fp32 for the fp32x3 engine; the stem's padded layout for K == 7), `w` is packed by pack_weight<S>.  Output: the NHWC view
-// (out, out_pitch), or with out == nullptr fp32 NCHW at out_nchw cropped to crop_h x crop_w.  As in a plan, the time table
-// of `ep` (ss, t_ptr, ss_img_stride) is attached after the descriptor is created.  info (may be null) receives
-// tc_conv_query.  Waits for the stream before it frees its scratch; `what` prefixes the error of a failed launch.
-template <typename S>
-int run_tc_conv(irsde_ctx* ctx, const char* what, const S* in, int in_pitch, int B, int H, int W, int Cin, int K, int up,
-                const S* w, int Cout, int Ho, int Wo, const Epilogue& ep, S* out, int out_pitch, float* out_nchw, int crop_h,
-                int crop_w, int flags, int32_t* info, cudaStream_t st) {
-  constexpr bool f32 = std::is_same<S, float>::value;
-  const TapTable t = tap_table(K, up);
-  const int Ha = t.s2d() ? H / 2 : H, Wa = t.s2d() ? W / 2 : W;
-  const long long npix = (long long)B * H * W;  // A pixels, also after the space-to-depth pass (4 planes of Ha x Wa)
-  std::vector<void*> scratch;
-  S* s2d = t.s2d() ? (S*)dev_alloc(ctx, npix * Cin * sizeof(S), &scratch) : nullptr;
-  float* split = f32 ? (float*)dev_alloc(ctx, 2 * npix * Cin * 4, &scratch) : nullptr;
-  if ((t.s2d() && !s2d) || (f32 && !split)) {
-    for (void* q : scratch) cudaFree(q);
-    return fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
+// The device scratch of one standalone entry call.  The bf16 paths run on bf16 copies of the caller's fp32 buffers: a
+// staged buffer is converted whole, the kernels work on views into the copy, and finish() converts the outputs back.
+// Memory comes from dev_alloc (counted in the context's bytes, for the entries that take a context), and every launch goes
+// to the entry's stream.  Nothing is freed before that stream has drained: finish() waits for it, and so
+// does the destructor when an early return skipped finish().
+class Scratch {
+ public:
+  irsde_ctx* const ctx;
+  const cudaStream_t st;
+
+  Scratch(irsde_ctx* c, cudaStream_t s) : ctx(c), st(s) {}
+  ~Scratch() {
+    if (!bufs_.empty()) release();
   }
+  template <typename T>
+  T* alloc(long long n) {
+    return (T*)dev_alloc(ctx, n * sizeof(T), &bufs_);
+  }
+  // bf16 copies of the caller's buffers: of one the call reads, of one it only writes (converted back by finish()), and of
+  // one it updates or writes a view of (both)
+  const bf16* in(const float* src, long long n) { return stage(src, nullptr, n); }
+  bf16* out(float* dst, long long n) { return stage(nullptr, dst, n); }
+  bf16* inout(float* buf, long long n) { return stage(buf, buf, n); }
+  // a device copy of v (the time-table row of a modulated epilogue)
+  const int* upload(int v) {
+    int* p = alloc<int>(1);
+    if (p) cudaMemcpyAsync(p, &v, sizeof v, cudaMemcpyHostToDevice, st);
+    return p;
+  }
+  int oom() const { return fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed"); }
+  // With rc == IRSDE_OK, converts the staged outputs back.  Then waits for the stream, turns a launch error into
+  // IRSDE_ERR_CUDA ("what: <CUDA error>") and frees the scratch.
+  int finish(int rc, const char* what) {
+    if (!rc)
+      for (const Back& b : back_) cast_bf16_f32_kernel<<<blocks(b.n), 256, 0, st>>>(b.src, b.dst, b.n);
+    const cudaError_t ce = release();
+    if (!rc && ce != cudaSuccess) rc = fail(ctx, IRSDE_ERR_CUDA, std::string(what) + ": " + cudaGetErrorString(ce));
+    return rc;
+  }
+
+ private:
+  struct Back { const bf16* src; float* dst; long long n; };
+  std::vector<void*> bufs_;
+  std::vector<Back> back_;
+  static unsigned blocks(long long n) { return (unsigned)std::min<long long>((n + 255) / 256, 65536); }
+  bf16* stage(const float* from, float* to, long long n) {
+    bf16* b = alloc<bf16>(n);
+    if (!b) return nullptr;
+    if (from) cast_f32_bf16_kernel<<<blocks(n), 256, 0, st>>>(from, b, n);
+    if (to) back_.push_back({b, to, n});
+    return b;
+  }
+  cudaError_t release() {
+    cudaError_t ce = cudaStreamSynchronize(st);
+    if (ce == cudaSuccess) ce = cudaGetLastError();
+    for (void* p : bufs_) cudaFree(p);
+    bufs_.clear();
+    back_.clear();
+    return ce;
+  }
+};
+
+// A channel view [off, off + width) of rows `pitch` elements apart; off and pitch also multiples of `align`.
+bool view_ok(int pitch, int off, long long width, int align = 1) {
+  return off >= 0 && off + width <= pitch && off % align == 0 && pitch % align == 0;
+}
+
+// An entry's info[4]: the caller's, or `local` when it passes none; zeroed.
+int32_t* zeroed_info(int32_t* info, int32_t* local) {
+  if (!info) info = local;
+  info[0] = info[1] = info[2] = info[3] = 0;
+  return info;
+}
+
+// Which of the tap-GEMM's conv shapes (tap_table) a standalone conv is: 3x3/1 pad 1 (also after nearest x2), 1x1, 4x4/2
+// pad 1 over an even H x W, or the 7x7/1 pad 3 stem.  Each entry applies its own engine rules on top.
+struct ConvShape {
+  bool k3, k1, k4, k7;
+};
+ConvShape conv_shape(int KH, int KW, int stride, int pad, int up, int H, int W) {
+  return ConvShape{KH == 3 && KW == 3 && stride == 1 && pad == 1, KH == 1 && KW == 1 && stride == 1 && pad == 0 && up == 1,
+                   KH == 4 && KW == 4 && stride == 2 && pad == 1 && up == 1 && H % 2 == 0 && W % 2 == 0,
+                   KH == 7 && KW == 7 && stride == 1 && pad == 3 && up == 1};
+}
+ConvGeom conv_geom(int B, int Cin, int H, int W, int Cout, int KH, int KW, int stride, int pad, int up) {
+  return ConvGeom{B, H, W, Cin, up, KH, KW, stride, pad, (H * up + 2 * pad - KH) / stride + 1, (W * up + 2 * pad - KW) / stride + 1,
+                  Cout};
+}
+
+// Runs the conv the plan builder would make of this shape on the tap-GEMM (S = bf16, or fp32 for the fp32x3 engine), with
+// the operands of run_conv.  As in a plan, the time table of `ep` (ss, t_ptr, ss_img_stride) is attached after the
+// descriptor is created.
+template <typename S>
+int run_tc_conv(Scratch& sc, const ConvGeom& g, const S* in, int in_pitch, const S* w, const Epilogue& ep, S* out, int out_pitch,
+                float* out_nchw, int crop_h, int crop_w, int flags, int32_t* info) {
+  constexpr bool f32 = std::is_same<S, float>::value;
+  const TapTable t = tap_table(g.KH, g.up);
+  const int Ha = t.s2d() ? g.Hin / 2 : g.Hin, Wa = t.s2d() ? g.Win / 2 : g.Win;
+  const long long npix = (long long)g.B * g.Hin * g.Win;  // A pixels, also after the space-to-depth pass (4 planes of Ha x Wa)
+  S* s2d = t.s2d() ? sc.alloc<S>(npix * g.Cin) : nullptr;
+  float* split = f32 ? sc.alloc<float>(2 * npix * g.Cin) : nullptr;
+  if ((t.s2d() && !s2d) || (f32 && !split)) return sc.oom();
   if (s2d) {
-    launch_space_to_depth<S>(in, in_pitch, s2d, B, H, W, Cin, st);
+    launch_space_to_depth<S>(in, in_pitch, s2d, g.B, g.Hin, g.Win, g.Cin, sc.st);
     in = s2d;
-    in_pitch = Cin;
+    in_pitch = g.Cin;
   }
   Epilogue e0 = ep;
   e0.ss = nullptr; e0.t_ptr = nullptr; e0.ss_img_stride = 0;
   std::string terr;
   TcConvDesc* d;
   if constexpr (f32) {
-    launch_split_tf32(in, in_pitch, split, npix, Cin, st);
-    d = tc_conv_create_f32x3(split, B, Ha, Wa, Cin, t.planes, w, Cout, t.ntaps, t.taps, t.nph, e0, out, out_pitch, Ho, Wo, &terr);
+    launch_split_tf32(in, in_pitch, split, npix, g.Cin, sc.st);
+    d = tc_conv_create_f32x3(split, g.B, Ha, Wa, g.Cin, t.planes, w, g.Cout, t.ntaps, t.taps, t.nph, e0, out, out_pitch, g.Hout,
+                             g.Wout, &terr);
   } else {
-    d = tc_conv_create(in, in_pitch, B, Ha, Wa, t.planes < 0 ? 64 : Cin, t.planes, w, Cout, t.ntaps, t.taps, t.nph, e0, out,
-                       out_pitch, Ho, Wo, &terr, flags);
+    d = tc_conv_create(in, in_pitch, g.B, Ha, Wa, t.planes < 0 ? 64 : g.Cin, t.planes, w, g.Cout, t.ntaps, t.taps, t.nph, e0, out,
+                       out_pitch, g.Hout, g.Wout, &terr, flags);
   }
-  int rc = d ? IRSDE_OK : fail(ctx, IRSDE_ERR_INVALID, std::string(f32 ? "tc_conv_create_f32x3: " : "tc_conv_create: ") + terr);
-  if (d) {
-    if (ep.ss) tc_conv_set_runtime(d, ep.ss, ep.t_ptr, ep.ss_img_stride);
-    if (!out) tc_conv_set_out_nchw(d, out_nchw, crop_h, crop_w);
-    if (info) tc_conv_query(d, info);
-    tc_conv_launch(d, st);
-    tc_conv_destroy(d);
+  if (!d) return fail(sc.ctx, IRSDE_ERR_INVALID, std::string(f32 ? "tc_conv_create_f32x3: " : "tc_conv_create: ") + terr);
+  if (ep.ss) tc_conv_set_runtime(d, ep.ss, ep.t_ptr, ep.ss_img_stride);
+  if (!out) tc_conv_set_out_nchw(d, out_nchw, crop_h, crop_w);
+  if (info) tc_conv_query(d, info);
+  tc_conv_launch(d, sc.st);
+  tc_conv_destroy(d);
+  return IRSDE_OK;
+}
+
+// One conv outside a plan, on engine 0 (SIMT, fp32), 1 (bf16 tap-GEMM) or 2 (fp32x3 tap-GEMM): packs w into the scratch in
+// layout wl and runs it.  in and ep.res are NHWC views in the engine's storage type S (the stem's padded layout for K = 7).
+// The output is the NHWC view (out, out_pitch), or with out == nullptr fp32 NCHW at out_nchw cropped to crop_h x crop_w.
+// flags are the tap-GEMM's TC_FLAG_*; info (may be null) receives its tc_conv_query.
+template <typename S>
+int run_conv(Scratch& sc, int engine, const ConvGeom& g, const S* in, int in_pitch, WLayout wl, const float* w, const Epilogue& ep,
+             S* out, int out_pitch, float* out_nchw, int crop_h, int crop_w, int flags, int32_t* info) {
+  S* wp = sc.alloc<S>(packed_weight_elems<S>(wl, g.Cout, g.Cin, g.KH, g.KW, g.B));
+  if (!wp) return sc.oom();
+  pack_weight<S>(wl, w, wp, g.Cout, g.Cin, g.KH, g.KW, g.B, sc.st);
+  if constexpr (std::is_same<S, float>::value) {
+    if (engine == 0) {
+      launch_conv_simt<float>(g, in, in_pitch, wp, ep, out, out_pitch, out_nchw, crop_h, crop_w, sc.st);
+      return IRSDE_OK;
+    }
   }
-  cudaError_t ce = cudaStreamSynchronize(st);
-  if (!rc && ce == cudaSuccess) ce = cudaGetLastError();
-  if (!rc && ce != cudaSuccess) rc = fail(ctx, IRSDE_ERR_CUDA, std::string(what) + cudaGetErrorString(ce));
-  for (void* q : scratch) cudaFree(q);
-  return rc;
+  return run_tc_conv<S>(sc, g, in, in_pitch, wp, ep, out, out_pitch, out_nchw, crop_h, crop_w, flags, info);
 }
 
 }  // namespace
@@ -2212,131 +2309,58 @@ int irsde_conv2d_ex(irsde_ctx* ctx, int32_t engine, const float* x, const float*
     return fail(ctx, IRSDE_ERR_INVALID, "q-softmax / per-image weights need a 1x1 conv with Cout % 8 == 0");
   if (f_qsm && Cout < 128) return fail(ctx, IRSDE_ERR_INVALID, "q-softmax needs Cout >= 128 (4 heads x 32)");
   cudaSetDevice(ctx->cfg.device);
-  cudaStream_t st = (cudaStream_t)stream;
-  int up = upsample ? 2 : 1;
-  if (engine == 1) {
-    // tensor-core engine: same taps/weight packing as the plan builder
-    std::string terr;
-    if (!tc_init(&terr)) return fail(ctx, IRSDE_ERR_CUDA, "tc_init: " + terr);
-    bool k3 = KH == 3 && KW == 3 && stride == 1 && pad == 1, k1 = KH == 1 && KW == 1 && stride == 1 && pad == 0 && up == 1,
-         k4 = KH == 4 && KW == 4 && stride == 2 && pad == 1 && up == 1 && H % 2 == 0 && W % 2 == 0,
-         k7 = KH == 7 && KW == 7 && stride == 1 && pad == 3 && up == 1 && Cin <= 8 && Cout % 8 == 0;
-    bool nchw = Cout % 8 != 0;  // head-style output: fp32 NCHW straight from the epilogue
-    if (!(k3 || k1 || k4 || k7) || (!k7 && Cin % 8) || (nchw && !(k3 && up == 1)))
+  if (engine < 0 || engine > 2) return fail(ctx, IRSDE_ERR_INVALID, "unknown engine");
+  std::string terr;
+  if (engine != 0 && !tc_init(&terr)) return fail(ctx, IRSDE_ERR_CUDA, "tc_init: " + terr);
+  const int up = upsample ? 2 : 1;
+  const ConvShape s = conv_shape(KH, KW, stride, pad, up, H, W);
+  bool k7 = false, nchw = false;  // nchw: head-style output, fp32 NCHW straight from the epilogue
+  if (engine == 1) {  // bf16 tap-GEMM: the plan builder's shapes, the stem included
+    k7 = s.k7 && Cin <= 8 && Cout % 8 == 0;
+    nchw = Cout % 8 != 0;
+    if (!(s.k3 || s.k1 || s.k4 || k7) || (!k7 && Cin % 8) || (nchw && !(s.k3 && up == 1)))
       return fail(ctx, IRSDE_ERR_UNSUPPORTED, "shape not supported by the tensor-core engine");
-    int Ho = (H * up + 2 * pad - KH) / stride + 1, Wo = (W * up + 2 * pad - KW) / stride + 1;
-    int Cout_pad = (Cout + 7) / 8 * 8;
-    std::vector<void*> tmp;
-    long long nin = k7 ? (long long)B * (H + 6) * (W + 8) * 8 + 64 : (long long)B * H * W * Cin;
-    long long nout = (long long)B * Ho * Wo * Cout_pad;
-    const WLayout wl = k7 ? WL_STEM : f_wimg ? WL_PER_IMAGE : (k3 && up == 2) ? WL_UP : WL_TAPS;  // per-image: w is [B][Cout][Cin]
-    bf16* resb = nullptr;
-    if (residual) {
-      if (nchw) return fail(ctx, IRSDE_ERR_UNSUPPORTED, "residual needs Cout % 8 == 0");
-      resb = (bf16*)dev_alloc(ctx, nout * 2, &tmp);
-      if (!resb) { for (void* q : tmp) cudaFree(q); return fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed"); }
-      launch_nchw_to_nhwc<bf16>(residual, resb, B, Cout, Ho, Wo, Cout, st);
-    }
-    bf16* xin = (bf16*)dev_alloc(ctx, nin * 2, &tmp);
-    bf16* wp = (bf16*)dev_alloc(ctx, packed_weight_elems<bf16>(wl, Cout, Cin, KH, KW, B) * 2, &tmp);
-    bf16* yo = (bf16*)dev_alloc(ctx, nout * 2, &tmp);
-    int rc = IRSDE_OK;
-    if (!xin || !wp || !yo) rc = fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
-    if (!rc) {
-      if (k7) {
-        cudaMemsetAsync(xin, 0, nin * 2, st);
-        launch_prep_input<bf16>(x, nullptr, xin, B, Cin, H, W, H, W, 8, 0, st, 3, 3, W + 8, H + 6);
-      } else {
-        launch_nchw_to_nhwc<bf16>(x, xin, B, Cin, H, W, Cin, st);
-      }
-      pack_weight<bf16>(wl, w, wp, Cout, Cin, KH, KW, B, st);
-      Epilogue ep;
-      memset(&ep, 0, sizeof ep);
-      ep.bias = bias;
-      ep.silu = silu;
-      if (resb) { ep.res = resb; ep.res_pitch = Cout; }
-      rc = run_tc_conv<bf16>(ctx, "tensor-core conv2d failed: ", xin, k7 ? 8 : Cin, B, H, W, Cin, KH, up, wp, Cout, Ho, Wo, ep,
-                             nchw ? nullptr : yo, Cout, y, Ho, Wo,
-                             (f_qsm ? TC_FLAG_QSOFTMAX : 0) | (f_wimg ? TC_FLAG_W_PER_IMAGE : 0), nullptr, st);
-    }
-    if (!rc) {
-      if (!nchw) launch_nhwc_to_nchw<bf16>(yo, Cout, y, B, Cout, Ho, Wo, st);
-      ctx->launches += 4;
-      cudaError_t e = cudaStreamSynchronize(st);
-      if (e == cudaSuccess) e = cudaGetLastError();
-      if (e != cudaSuccess) rc = fail(ctx, IRSDE_ERR_CUDA, std::string("tensor-core conv2d failed: ") + cudaGetErrorString(e));
-    }
-    for (void* q : tmp) cudaFree(q);
-    return rc;
-  }
-  if (engine == 2) {
-    // fp32x3 engine: fp32 NHWC, hi/lo split, 3 x tf32 wgmma (conv_tc.cu MODE 3)
-    std::string terr;
-    if (!tc_init(&terr)) return fail(ctx, IRSDE_ERR_CUDA, "tc_init: " + terr);
-    bool k3 = KH == 3 && KW == 3 && stride == 1 && pad == 1, k1 = KH == 1 && KW == 1 && stride == 1 && pad == 0 && up == 1,
-         k4 = KH == 4 && KW == 4 && stride == 2 && pad == 1 && up == 1 && H % 2 == 0 && W % 2 == 0;
-    bool nchw = Cout % 4 != 0;
-    if (!(k3 || k1 || k4) || Cin % 4 || (nchw && !(k3 && up == 1)) || residual && nchw)
+    if (residual && nchw) return fail(ctx, IRSDE_ERR_UNSUPPORTED, "residual needs Cout % 8 == 0");
+  } else if (engine == 2) {  // fp32x3: fp32 NHWC, hi/lo split, 3 x tf32 wgmma (conv_tc.cu MODE 3)
+    nchw = Cout % 4 != 0;
+    if (!(s.k3 || s.k1 || s.k4) || Cin % 4 || (nchw && !(s.k3 && up == 1)) || residual && nchw)
       return fail(ctx, IRSDE_ERR_UNSUPPORTED, "shape not supported by the fp32x3 engine");
-    int Ho = (H * up + 2 * pad - KH) / stride + 1, Wo = (W * up + 2 * pad - KW) / stride + 1;
-    std::vector<void*> tmp;
-    long long nin = (long long)B * H * W * Cin, nout = (long long)B * Ho * Wo * Cout;
-    const WLayout wl = (k3 && up == 2) ? WL_UP : WL_TAPS;
-    float* xin = (float*)dev_alloc(ctx, nin * 4, &tmp);
-    float* wp = (float*)dev_alloc(ctx, packed_weight_elems<float>(wl, Cout, Cin, KH, KW) * 4, &tmp);
-    float* yo = (float*)dev_alloc(ctx, (nout + 16) * 4, &tmp);
-    float* resb = residual ? (float*)dev_alloc(ctx, nout * 4, &tmp) : nullptr;
-    int rc = IRSDE_OK;
-    if (!xin || !wp || !yo || (residual && !resb)) rc = fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
-    if (!rc) {
-      launch_nchw_to_nhwc<float>(x, xin, B, Cin, H, W, Cin, st);
-      if (resb) launch_nchw_to_nhwc<float>(residual, resb, B, Cout, Ho, Wo, Cout, st);
-      pack_weight<float>(wl, w, wp, Cout, Cin, KH, KW, 1, st);
-      Epilogue ep;
-      memset(&ep, 0, sizeof ep);
-      ep.bias = bias;
-      ep.silu = silu;
-      if (resb) { ep.res = resb; ep.res_pitch = Cout; }
-      rc = run_tc_conv<float>(ctx, "fp32x3 conv2d failed: ", xin, Cin, B, H, W, Cin, KH, up, wp, Cout, Ho, Wo, ep,
-                              nchw ? nullptr : yo, Cout, y, Ho, Wo, 0, nullptr, st);
-    }
-    if (!rc) {
-      if (!nchw) launch_nhwc_to_nchw<float>(yo, Cout, y, B, Cout, Ho, Wo, st);
-      ctx->launches += 5;
-      cudaError_t e = cudaStreamSynchronize(st);
-      if (e == cudaSuccess) e = cudaGetLastError();
-      if (e != cudaSuccess) rc = fail(ctx, IRSDE_ERR_CUDA, std::string("fp32x3 conv2d failed: ") + cudaGetErrorString(e));
-    }
-    for (void* q : tmp) cudaFree(q);
-    return rc;
   }
-  if (engine != 0) return fail(ctx, IRSDE_ERR_INVALID, "unknown engine");
-  ConvGeom g;
-  g.B = B; g.Hin = H; g.Win = W; g.Cin = Cin; g.up = up; g.KH = KH; g.KW = KW; g.stride = stride; g.pad = pad;
-  g.Hout = (H * up + 2 * pad - KH) / stride + 1;
-  g.Wout = (W * up + 2 * pad - KW) / stride + 1;
-  g.Cout = Cout;
-  std::vector<void*> tmp;
-  long long nin = (long long)B * H * W * Cin, nout = (long long)B * g.Hout * g.Wout * Cout;
-  float* xin = (float*)dev_alloc(ctx, nin * 4, &tmp);
-  float* wp = (float*)dev_alloc(ctx, packed_weight_elems<float>(WL_SIMT, Cout, Cin, KH, KW) * 4, &tmp);
-  float* yo = (float*)dev_alloc(ctx, nout * 4, &tmp);
-  int rc = IRSDE_OK;
-  if (!xin || !wp || !yo) rc = fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
-  if (!rc) {
-    launch_nchw_to_nhwc<float>(x, xin, B, Cin, H, W, Cin, st);
-    pack_weight<float>(WL_SIMT, w, wp, Cout, Cin, KH, KW, 1, st);
+  const ConvGeom g = conv_geom(B, Cin, H, W, Cout, KH, KW, stride, pad, up);
+  const int Ho = g.Hout, Wo = g.Wout;
+  // per-image: w is [B][Cout][Cin]
+  const WLayout wl = engine == 0 ? WL_SIMT : k7 ? WL_STEM : f_wimg ? WL_PER_IMAGE : (s.k3 && up == 2) ? WL_UP : WL_TAPS;
+  const int tc_flags = (f_qsm ? TC_FLAG_QSOFTMAX : 0) | (f_wimg ? TC_FLAG_W_PER_IMAGE : 0);
+  Scratch sc(ctx, (cudaStream_t)stream);
+  // NCHW -> NHWC staging in the engine's storage type; bf16 output rows padded to 8 channels, the fp32x3 output with slack
+  auto run = [&](auto* type) {
+    using S = std::remove_pointer_t<decltype(type)>;
+    const long long nin = k7 ? (long long)B * (H + 6) * (W + 8) * 8 + 64 : (long long)B * H * W * Cin;
+    const long long nout = (long long)B * Ho * Wo * (engine == 1 ? (Cout + 7) / 8 * 8 : Cout);
+    S* res = residual ? sc.alloc<S>(nout) : nullptr;
+    S* xin = sc.alloc<S>(nin);
+    S* yo = sc.alloc<S>(engine == 2 ? nout + 16 : nout);
+    if ((residual && !res) || !xin || !yo) return sc.oom();
+    if (res) launch_nchw_to_nhwc<S>(residual, res, B, Cout, Ho, Wo, Cout, sc.st);
+    if (k7) {
+      cudaMemsetAsync(xin, 0, nin * sizeof(S), sc.st);
+      launch_prep_input<S>(x, nullptr, xin, B, Cin, H, W, H, W, 8, 0, sc.st, 3, 3, W + 8, H + 6);
+    } else {
+      launch_nchw_to_nhwc<S>(x, xin, B, Cin, H, W, Cin, sc.st);
+    }
     Epilogue ep;
     memset(&ep, 0, sizeof ep);
     ep.bias = bias;
     ep.silu = silu;
-    launch_conv_simt<float>(g, xin, Cin, wp, ep, yo, Cout, nullptr, 0, 0, st);
-    launch_nhwc_to_nchw<float>(yo, Cout, y, B, Cout, g.Hout, g.Wout, st);
-    ctx->launches += 4;
-    if (cudaStreamSynchronize(st) != cudaSuccess || cudaGetLastError() != cudaSuccess) rc = fail(ctx, IRSDE_ERR_CUDA, "conv2d failed");
-  }
-  for (void* q : tmp) { cudaFree(q); }
-  return rc;
+    if (res) { ep.res = res; ep.res_pitch = Cout; }
+    const int rc = run_conv<S>(sc, engine, g, xin, k7 ? 8 : Cin, wl, w, ep, nchw ? nullptr : yo, Cout, nchw ? y : nullptr, Ho, Wo,
+                               tc_flags, nullptr);
+    if (!rc && !nchw) launch_nhwc_to_nchw<S>(yo, Cout, y, B, Cout, Ho, Wo, sc.st);
+    return rc;
+  };
+  const int rc = engine == 1 ? run((bf16*)nullptr) : run((float*)nullptr);
+  if (!rc) ctx->launches += engine == 2 ? 5 : 4;
+  return sc.finish(rc, engine == 1 ? "tensor-core conv2d failed" : engine == 2 ? "fp32x3 conv2d failed" : "conv2d failed");
 }
 
 int irsde_conv2d_fused(irsde_ctx* ctx, int32_t engine, const float* x, const float* w, const irsde_conv_epilogue* epi, float* y,
@@ -2348,30 +2372,27 @@ int irsde_conv2d_fused(irsde_ctx* ctx, int32_t engine, const float* x, const flo
   if (engine < 0 || engine > 2) return fail(ctx, IRSDE_ERR_INVALID, "unknown engine");
   if (B < 1 || Cin < 1 || H < 1 || W < 1 || Cout < 1) return fail(ctx, IRSDE_ERR_INVALID, "bad shape");
   const int up = upsample ? 2 : 1;
-  const bool k3 = KH == 3 && KW == 3 && stride == 1 && pad == 1, k1 = KH == 1 && KW == 1 && stride == 1 && pad == 0 && up == 1,
-             k4 = KH == 4 && KW == 4 && stride == 2 && pad == 1 && up == 1 && H % 2 == 0 && W % 2 == 0;
-  if (!(k3 || k1 || k4)) return fail(ctx, IRSDE_ERR_UNSUPPORTED, "fused conv: 3x3/1 (optionally after nearest x2), 1x1 or 4x4/2");
-  const int Ho = (H * up + 2 * pad - KH) / stride + 1, Wo = (W * up + 2 * pad - KW) / stride + 1;
+  const ConvShape s = conv_shape(KH, KW, stride, pad, up, H, W);
+  if (!(s.k3 || s.k1 || s.k4)) return fail(ctx, IRSDE_ERR_UNSUPPORTED, "fused conv: 3x3/1 (optionally after nearest x2), 1x1 or 4x4/2");
+  const ConvGeom g = conv_geom(B, Cin, H, W, Cout, KH, KW, stride, pad, up);
+  const int Ho = g.Hout, Wo = g.Wout;
   const bool nchw = e.crop_h != 0 || e.crop_w != 0;
   const bool qsm = (e.flags & IRSDE_CONV_QSOFTMAX) != 0;
   if (e.flags & ~IRSDE_CONV_QSOFTMAX) return fail(ctx, IRSDE_ERR_UNSUPPORTED, "fused conv: flags other than IRSDE_CONV_QSOFTMAX");
-  if (qsm && (engine != 1 || !k1 || Cout < 128 || nchw))
+  if (qsm && (engine != 1 || !s.k1 || Cout < 128 || nchw))
     return fail(ctx, IRSDE_ERR_INVALID, "q-softmax is the bf16 epilogue of a 1x1 conv with Cout >= 128");
   const int al = engine == 1 ? 8 : 4;  // elements per 16 bytes of the engine's storage type
-  auto view_ok = [&](int pitch, int off, int C) {
-    return off >= 0 && (long long)off + C <= pitch && off % al == 0 && pitch % al == 0;
-  };
   if (engine != 0 && (Cin % al || (!nchw && Cout % al)))
     return fail(ctx, IRSDE_ERR_INVALID, "tensor-core engines: Cin and Cout must be multiples of 16 bytes");
-  if (!view_ok(e.in_pitch, e.in_off, Cin)) return fail(ctx, IRSDE_ERR_INVALID, "input view outside its pitch or not 16-byte aligned");
+  if (!view_ok(e.in_pitch, e.in_off, Cin, al)) return fail(ctx, IRSDE_ERR_INVALID, "input view outside its pitch or not 16-byte aligned");
   if (nchw) {
-    if (!k3 || up != 1) return fail(ctx, IRSDE_ERR_UNSUPPORTED, "the cropped fp32 NCHW output is the 3x3 head's epilogue");
+    if (!s.k3 || up != 1) return fail(ctx, IRSDE_ERR_UNSUPPORTED, "the cropped fp32 NCHW output is the 3x3 head's epilogue");
     if (e.crop_h < 1 || e.crop_w < 1 || e.crop_h > Ho || e.crop_w > Wo) return fail(ctx, IRSDE_ERR_INVALID, "crop larger than the output");
     if (e.res) return fail(ctx, IRSDE_ERR_UNSUPPORTED, "no residual with the NCHW output");
-  } else if (!view_ok(e.out_pitch, e.out_off, Cout)) {
+  } else if (!view_ok(e.out_pitch, e.out_off, Cout, al)) {
     return fail(ctx, IRSDE_ERR_INVALID, "output view outside its pitch or not 16-byte aligned");
   }
-  if (e.res && !view_ok(e.res_pitch, e.res_off, Cout))
+  if (e.res && !view_ok(e.res_pitch, e.res_off, Cout, al))
     return fail(ctx, IRSDE_ERR_INVALID, "residual view outside its pitch or not 16-byte aligned");
   if (e.ss) {
     if (e.mult_vec) return fail(ctx, IRSDE_ERR_INVALID, "the time-modulation table and mult_vec cannot be combined");
@@ -2384,19 +2405,14 @@ int irsde_conv2d_fused(irsde_ctx* ctx, int32_t engine, const float* x, const flo
   for (const float* q : ptrs)
     if ((uintptr_t)q & 15) return fail(ctx, IRSDE_ERR_INVALID, "device buffers must be 16-byte aligned");
   int32_t info_local[4];
-  if (!info) info = info_local;
-  info[0] = info[1] = info[2] = info[3] = 0;
+  info = zeroed_info(info, info_local);
 
   cudaSetDevice(ctx->cfg.device);
-  cudaStream_t st = (cudaStream_t)stream;
   std::string terr;
   if (engine != 0 && !tc_init(&terr)) return fail(ctx, IRSDE_ERR_CUDA, "tc_init: " + terr);
-  const long long npix_out = (long long)B * Ho * Wo;
-  std::vector<void*> tmp;
-  int rc = IRSDE_OK;
-  int* t_dev = (int*)dev_alloc(ctx, sizeof(int), &tmp);
-  if (!t_dev) rc = fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
-  if (!rc) cudaMemcpyAsync(t_dev, &e.t_row, sizeof(int), cudaMemcpyHostToDevice, st);
+  Scratch sc(ctx, (cudaStream_t)stream);
+  const int* t_dev = sc.upload(e.t_row);
+  if (!t_dev) return sc.oom();
   Epilogue ep;
   memset(&ep, 0, sizeof ep);
   ep.bias = e.bias;
@@ -2406,71 +2422,28 @@ int irsde_conv2d_fused(irsde_ctx* ctx, int32_t engine, const float* x, const flo
   ep.ss_off = e.ss_off;
   if (e.ss) { ep.ss = e.ss; ep.t_ptr = t_dev; ep.ss_img_stride = e.ss_img_stride; }
   ep.res_pitch = e.res_pitch;
-  const WLayout wl = engine == 0 ? WL_SIMT : (k3 && up == 2) ? WL_UP : WL_TAPS;
-  auto blocks = [](long long n) { return (unsigned)std::min<long long>((n + 255) / 256, 65536); };
-  if (!rc && engine == 0) {
-    ConvGeom g;
-    g.B = B; g.Hin = H; g.Win = W; g.Cin = Cin; g.up = up; g.KH = KH; g.KW = KW; g.stride = stride; g.pad = pad;
-    g.Hout = Ho; g.Wout = Wo; g.Cout = Cout;
-    float* wp = (float*)dev_alloc(ctx, packed_weight_elems<float>(wl, Cout, Cin, KH, KW) * 4, &tmp);
-    if (!wp) rc = fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
-    if (!rc) {
-      pack_weight<float>(wl, w, wp, Cout, Cin, KH, KW, 1, st);
-      if (e.res) ep.res = e.res + e.res_off;
-      launch_conv_simt<float>(g, x + e.in_off, e.in_pitch, wp, ep, nchw ? nullptr : y + e.out_off, e.out_pitch, nchw ? y : nullptr,
-                              e.crop_h, e.crop_w, st);
-    }
-  } else if (!rc && engine == 1) {
-    const long long nin = (long long)B * H * W * e.in_pitch;
-    bf16* xb = (bf16*)dev_alloc(ctx, nin * 2, &tmp);
-    bf16* wp = (bf16*)dev_alloc(ctx, packed_weight_elems<bf16>(wl, Cout, Cin, KH, KW) * 2, &tmp);
-    bf16* rb = e.res ? (bf16*)dev_alloc(ctx, npix_out * e.res_pitch * 2, &tmp) : nullptr;
-    bf16* yb = nchw ? nullptr : (bf16*)dev_alloc(ctx, npix_out * e.out_pitch * 2, &tmp);
-    if (!xb || !wp || (e.res && !rb) || (!nchw && !yb)) rc = fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
-    if (!rc) {
-      cast_f32_bf16_kernel<<<blocks(nin), 256, 0, st>>>(x, xb, nin);
-      if (rb) cast_f32_bf16_kernel<<<blocks(npix_out * e.res_pitch), 256, 0, st>>>(e.res, rb, npix_out * e.res_pitch);
-      if (yb) cast_f32_bf16_kernel<<<blocks(npix_out * e.out_pitch), 256, 0, st>>>(y, yb, npix_out * e.out_pitch);
-      pack_weight<bf16>(wl, w, wp, Cout, Cin, KH, KW, 1, st);
-      if (rb) ep.res = rb + e.res_off;
-      rc = run_tc_conv<bf16>(ctx, "fused conv2d failed: ", xb + e.in_off, e.in_pitch, B, H, W, Cin, KH, up, wp, Cout, Ho, Wo, ep,
-                             nchw ? nullptr : yb + e.out_off, e.out_pitch, y, e.crop_h, e.crop_w, qsm ? TC_FLAG_QSOFTMAX : 0, info, st);
-      if (!rc && yb) cast_bf16_f32_kernel<<<blocks(npix_out * e.out_pitch), 256, 0, st>>>(yb, y, npix_out * e.out_pitch);
-    }
-  } else if (!rc) {
-    float* wp = (float*)dev_alloc(ctx, packed_weight_elems<float>(wl, Cout, Cin, KH, KW) * 4, &tmp);
-    if (!wp) rc = fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
-    if (!rc) {
-      pack_weight<float>(wl, w, wp, Cout, Cin, KH, KW, 1, st);
-      if (e.res) ep.res = e.res + e.res_off;
-      rc = run_tc_conv<float>(ctx, "fused conv2d failed: ", x + e.in_off, e.in_pitch, B, H, W, Cin, KH, up, wp, Cout, Ho, Wo, ep,
-                              nchw ? nullptr : y + e.out_off, e.out_pitch, y, e.crop_h, e.crop_w, 0, info, st);
-    }
-  }
-  if (!rc) {
-    ctx->launches += 4;
-    cudaError_t ce = cudaStreamSynchronize(st);
-    if (ce == cudaSuccess) ce = cudaGetLastError();
-    if (ce != cudaSuccess) rc = fail(ctx, IRSDE_ERR_CUDA, std::string("fused conv2d failed: ") + cudaGetErrorString(ce));
+  const WLayout wl = engine == 0 ? WL_SIMT : (s.k3 && up == 2) ? WL_UP : WL_TAPS;
+  float* out_nchw = nchw ? y : nullptr;
+  int rc;
+  if (engine == 1) {  // bf16 copies of the whole of x, res and y
+    const long long npix_out = (long long)B * Ho * Wo;
+    const bf16* xb = sc.in(x, (long long)B * H * W * e.in_pitch);
+    const bf16* rb = e.res ? sc.in(e.res, npix_out * e.res_pitch) : nullptr;
+    bf16* yb = nchw ? nullptr : sc.inout(y, npix_out * e.out_pitch);
+    if (!xb || (e.res && !rb) || (!nchw && !yb)) return sc.oom();
+    if (rb) ep.res = rb + e.res_off;
+    rc = run_conv<bf16>(sc, engine, g, xb + e.in_off, e.in_pitch, wl, w, ep, yb ? yb + e.out_off : nullptr, e.out_pitch, out_nchw,
+                        e.crop_h, e.crop_w, qsm ? TC_FLAG_QSOFTMAX : 0, info);
   } else {
-    cudaStreamSynchronize(st);  // conversions already queued read buffers freed below
+    if (e.res) ep.res = e.res + e.res_off;
+    rc = run_conv<float>(sc, engine, g, x + e.in_off, e.in_pitch, wl, w, ep, nchw ? nullptr : y + e.out_off, e.out_pitch, out_nchw,
+                         e.crop_h, e.crop_w, 0, info);
   }
-  for (void* q : tmp) cudaFree(q);
-  return rc;
+  if (!rc) ctx->launches += 4;
+  return sc.finish(rc, "fused conv2d failed");
 }
 
 // ---- one LayerNorm / attention op outside a plan ------------------------------------------------------------------
-static unsigned cast_blocks(long long n) { return (unsigned)std::min<long long>((n + 255) / 256, 65536); }
-
-// Waits for the stream, turns a launch error into the context's error and frees the scratch.
-static int finish_op(irsde_ctx* ctx, int rc, const char* what, cudaStream_t st, std::vector<void*>& tmp) {
-  cudaError_t ce = cudaStreamSynchronize(st);
-  if (ce == cudaSuccess) ce = cudaGetLastError();
-  if (!rc && ce != cudaSuccess) rc = fail(ctx, IRSDE_ERR_CUDA, std::string(what) + cudaGetErrorString(ce));
-  for (void* q : tmp) cudaFree(q);
-  return rc;
-}
-
 int irsde_layernorm(irsde_ctx* ctx, int32_t precision, const float* x, const irsde_ln_args* args, float* y, int32_t B, int32_t N,
                     int32_t C, int32_t* info, void* stream) {
   // ---- everything is validated here, before the first allocation or launch
@@ -2478,10 +2451,9 @@ int irsde_layernorm(irsde_ctx* ctx, int32_t precision, const float* x, const irs
   const irsde_ln_args& a = *args;
   if (precision < IRSDE_PREC_FP32 || precision > IRSDE_PREC_FP32X3) return fail(ctx, IRSDE_ERR_INVALID, "bad precision");
   if (B < 1 || N < 1 || C < 1) return fail(ctx, IRSDE_ERR_INVALID, "bad shape");
-  auto view_ok = [&](int pitch, int off) { return off >= 0 && (long long)off + C <= pitch; };
-  if (!view_ok(a.in_pitch, a.in_off)) return fail(ctx, IRSDE_ERR_INVALID, "input view outside its pitch");
-  if (!view_ok(a.out_pitch, a.out_off)) return fail(ctx, IRSDE_ERR_INVALID, "output view outside its pitch");
-  if (a.res && !view_ok(a.res_pitch, a.res_off)) return fail(ctx, IRSDE_ERR_INVALID, "residual view outside its pitch");
+  if (!view_ok(a.in_pitch, a.in_off, C)) return fail(ctx, IRSDE_ERR_INVALID, "input view outside its pitch");
+  if (!view_ok(a.out_pitch, a.out_off, C)) return fail(ctx, IRSDE_ERR_INVALID, "output view outside its pitch");
+  if (a.res && !view_ok(a.res_pitch, a.res_off, C)) return fail(ctx, IRSDE_ERR_INVALID, "residual view outside its pitch");
   if (a.ss) {
     if (a.t_row < 0 || a.ss_img_stride < 0 || (long long)a.t_row + (long long)(B - 1) * a.ss_img_stride >= a.ss_rows)
       return fail(ctx, IRSDE_ERR_INVALID, "time-modulation row outside the table");
@@ -2489,17 +2461,13 @@ int irsde_layernorm(irsde_ctx* ctx, int32_t precision, const float* x, const irs
       return fail(ctx, IRSDE_ERR_INVALID, "scale / shift columns outside the table row");
   }
   int32_t info_local[4];
-  if (!info) info = info_local;
-  info[0] = info[1] = info[2] = info[3] = 0;
+  info = zeroed_info(info, info_local);
 
   cudaSetDevice(ctx->cfg.device);
-  cudaStream_t st = (cudaStream_t)stream;
   const long long npix = (long long)B * N;
-  std::vector<void*> tmp;
-  int rc = IRSDE_OK;
-  int* t_dev = (int*)dev_alloc(ctx, sizeof(int), &tmp);
-  if (!t_dev) rc = fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
-  if (!rc) cudaMemcpyAsync(t_dev, &a.t_row, sizeof(int), cudaMemcpyHostToDevice, st);
+  Scratch sc(ctx, (cudaStream_t)stream);
+  const int* t_dev = sc.upload(a.t_row);
+  if (!t_dev) return sc.oom();
   LnMod m;
   memset(&m, 0, sizeof m);
   if (a.ss) {
@@ -2508,33 +2476,25 @@ int irsde_layernorm(irsde_ctx* ctx, int32_t precision, const float* x, const irs
   }
   m.pix_per_img = N;
   LnPick k{};
-  if (!rc && precision == IRSDE_PREC_BF16) {
-    const long long nx = npix * a.in_pitch, ny = npix * a.out_pitch, nr = a.res ? npix * a.res_pitch : 0;
-    bf16* xb = (bf16*)dev_alloc(ctx, nx * 2, &tmp);
-    bf16* yb = (bf16*)dev_alloc(ctx, ny * 2, &tmp);
-    bf16* rb = a.res ? (bf16*)dev_alloc(ctx, nr * 2, &tmp) : nullptr;
-    if (!xb || !yb || (a.res && !rb)) rc = fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
-    if (!rc) {
-      cast_f32_bf16_kernel<<<cast_blocks(nx), 256, 0, st>>>(x, xb, nx);
-      cast_f32_bf16_kernel<<<cast_blocks(ny), 256, 0, st>>>(y, yb, ny);
-      if (rb) cast_f32_bf16_kernel<<<cast_blocks(nr), 256, 0, st>>>(a.res, rb, nr);
-      const bf16 *xv = xb + a.in_off, *rv = rb ? rb + a.res_off : nullptr;
-      bf16* yv = yb + a.out_off;
-      k = ln_pick<bf16>(C, npix, a.in_pitch, a.res_pitch, a.out_pitch, xv, a.g, rv, yv);
-      launch_layernorm<bf16>(xv, a.in_pitch, a.g, rv, a.res_pitch, yv, a.out_pitch, npix, C, st, &m);
-      cast_bf16_f32_kernel<<<cast_blocks(ny), 256, 0, st>>>(yb, y, ny);
-    }
-  } else if (!rc) {
-    const float *xv = x + a.in_off, *rv = a.res ? a.res + a.res_off : nullptr;
-    float* yv = y + a.out_off;
-    k = ln_pick<float>(C, npix, a.in_pitch, a.res_pitch, a.out_pitch, xv, a.g, rv, yv);
-    launch_layernorm<float>(xv, a.in_pitch, a.g, rv, a.res_pitch, yv, a.out_pitch, npix, C, st, &m);
+  auto run = [&](auto* xs, auto* rs, auto* ys) {
+    using S = std::remove_pointer_t<decltype(ys)>;
+    const S *xv = xs + a.in_off, *rv = rs ? rs + a.res_off : nullptr;
+    S* yv = ys + a.out_off;
+    k = ln_pick<S>(C, npix, a.in_pitch, a.res_pitch, a.out_pitch, xv, a.g, rv, yv);
+    launch_layernorm<S>(xv, a.in_pitch, a.g, rv, a.res_pitch, yv, a.out_pitch, npix, C, sc.st, &m);
+  };
+  if (precision == IRSDE_PREC_BF16) {
+    const bf16* xb = sc.in(x, npix * a.in_pitch);
+    bf16* yb = sc.inout(y, npix * a.out_pitch);
+    const bf16* rb = a.res ? sc.in(a.res, npix * a.res_pitch) : nullptr;
+    if (!xb || !yb || (a.res && !rb)) return sc.oom();
+    run(xb, rb, yb);
+  } else {
+    run(x, a.res, y);
   }
-  if (!rc) {
-    info[0] = k.kind; info[1] = k.maxv; info[2] = k.lpp; info[3] = k.pp;
-    ctx->launches++;
-  }
-  return finish_op(ctx, rc, "layernorm failed: ", st, tmp);
+  info[0] = k.kind; info[1] = k.maxv; info[2] = k.lpp; info[3] = k.pp;
+  ctx->launches++;
+  return sc.finish(IRSDE_OK, "layernorm failed");
 }
 
 int irsde_attention(irsde_ctx* ctx, int32_t precision, int32_t kind, const float* qkv, int32_t qkv_pitch, int32_t qkv_off,
@@ -2551,73 +2511,60 @@ int irsde_attention(irsde_ctx* ctx, int32_t precision, int32_t kind, const float
   if (lin && !ctx_out) return fail(ctx, IRSDE_ERR_INVALID, "linear attention needs ctx_out");
   if (fold && (!wout || Cout < 1 || ((uintptr_t)wout & 15)))
     return fail(ctx, IRSDE_ERR_INVALID, "the fold needs 16-byte aligned to_out weights [Cout][128], Cout >= 1");
-  if (qkv_off < 0 || (long long)qkv_off + 384 > qkv_pitch) return fail(ctx, IRSDE_ERR_INVALID, "qkv view outside its pitch");
-  if (!fold && (out_off < 0 || (long long)out_off + 128 > out_pitch))
-    return fail(ctx, IRSDE_ERR_INVALID, "hidden view outside its pitch");
+  if (!view_ok(qkv_pitch, qkv_off, 384)) return fail(ctx, IRSDE_ERR_INVALID, "qkv view outside its pitch");
+  if (!fold && !view_ok(out_pitch, out_off, 128)) return fail(ctx, IRSDE_ERR_INVALID, "hidden view outside its pitch");
   // the views the launchers get: the caller's buffers (fp32), or bf16 copies that start on 256 bytes
   const size_t elem = bf ? 2 : 4;
   auto at = [&](const float* base, int off) { return (const void*)((bf ? 0 : (uintptr_t)base) + (uintptr_t)off * elem); };
   if (lin && !linattn_views_ok(at(qkv, qkv_off), qkv_pitch, fold ? nullptr : at(out, out_off), out_pitch, elem))
     return fail(ctx, IRSDE_ERR_INVALID, "linear attention: views must start on 16 bytes and pitches be multiples of 16 bytes");
   int32_t info_local[4];
-  if (!info) info = info_local;
-  info[0] = info[1] = info[2] = info[3] = 0;
+  info = zeroed_info(info, info_local);
 
   cudaSetDevice(ctx->cfg.device);
-  cudaStream_t st = (cudaStream_t)stream;
   const long long npix = (long long)B * N;
-  std::vector<void*> tmp;
-  int rc = IRSDE_OK;
-  float* part = lin ? (float*)dev_alloc(ctx, linattn_partial_floats(B, N) * sizeof(float), &tmp) : nullptr;
-  float* cx = lin ? (float*)dev_alloc(ctx, (size_t)B * 4096 * sizeof(float), &tmp) : nullptr;
-  if (lin && (!part || !cx)) rc = fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
-  bool launched = false;
+  Scratch sc(ctx, (cudaStream_t)stream);
+  float* part = lin ? sc.alloc<float>(linattn_partial_floats(B, N)) : nullptr;
+  float* cx = lin ? sc.alloc<float>((long long)B * 4096) : nullptr;
+  if (lin && (!part || !cx)) return sc.oom();
   int kern = 0;
-  if (!rc && bf) {
-    const long long nq = npix * qkv_pitch, no = fold ? (long long)B * Cout * 128 : npix * out_pitch;
-    bf16* qb = (bf16*)dev_alloc(ctx, nq * 2, &tmp);
-    bf16* ob = (bf16*)dev_alloc(ctx, no * 2, &tmp);
-    if (!qb || !ob) rc = fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
-    if (!rc) {
-      cast_f32_bf16_kernel<<<cast_blocks(nq), 256, 0, st>>>(qkv, qb, nq);
-      if (!fold) cast_f32_bf16_kernel<<<cast_blocks(no), 256, 0, st>>>(out, ob, no);
-      const bf16* qv = qb + qkv_off;
-      if (kind == IRSDE_ATTN_LINEAR) {
-        kern = 2;
-        launched = launch_linattn<bf16>(qv, qkv_pitch, part, cx, ob + out_off, out_pitch, B, N, st);
-      } else if (fold) {
-        kern = 2;
-        launched = launch_linattn_ctx<bf16>(qv, qkv_pitch, part, cx, B, N, st);
-        if (launched) launch_la_fold(cx, wout, ob, B, Cout, st);
-      } else {
-        kern = fullattn_pick<bf16>(qv, qkv_pitch, ob + out_off, out_pitch) == FA_MMA ? 4 : 3;
-        launch_fullattn<bf16>(qv, qkv_pitch, ob + out_off, out_pitch, B, N, st);
-        launched = true;
+  // kern: 1 / 2 the fp32 / bf16 linear attention, 3 the scalar and 4 the MMA full attention
+  auto run = [&](auto* qs, auto* os) -> bool {
+    using S = std::remove_pointer_t<decltype(os)>;
+    const S* qv = qs + qkv_off;
+    if (lin) kern = bf ? 2 : 1;
+    if constexpr (std::is_same<S, bf16>::value) {
+      if (fold) {
+        if (!launch_linattn_ctx<bf16>(qv, qkv_pitch, part, cx, B, N, sc.st)) return false;
+        launch_la_fold(cx, wout, os, B, Cout, sc.st);
+        return true;
       }
-      if (launched) cast_bf16_f32_kernel<<<cast_blocks(no), 256, 0, st>>>(ob, out, no);
     }
-  } else if (!rc) {
-    if (lin) {
-      kern = 1;
-      launched = launch_linattn<float>(qkv + qkv_off, qkv_pitch, part, cx, out + out_off, out_pitch, B, N, st);
-    } else {
-      kern = 3;
-      launch_fullattn<float>(qkv + qkv_off, qkv_pitch, out + out_off, out_pitch, B, N, st);
-      launched = true;
-    }
+    if (lin) return launch_linattn<S>(qv, qkv_pitch, part, cx, os + out_off, out_pitch, B, N, sc.st);
+    kern = fullattn_pick<S>(qv, qkv_pitch, os + out_off, out_pitch) == FA_MMA ? 4 : 3;
+    launch_fullattn<S>(qv, qkv_pitch, os + out_off, out_pitch, B, N, sc.st);
+    return true;
+  };
+  bool launched;
+  if (bf) {
+    const long long no = fold ? (long long)B * Cout * 128 : npix * out_pitch;
+    const bf16* qb = sc.in(qkv, npix * qkv_pitch);
+    bf16* ob = fold ? sc.out(out, no) : sc.inout(out, no);
+    if (!qb || !ob) return sc.oom();
+    launched = run(qb, ob);
+  } else {
+    launched = run(qkv, out);
   }
-  if (!rc && !launched) rc = fail(ctx, IRSDE_ERR_INVALID, "the linear-attention launcher refused the views");
-  if (!rc) {
-    if (lin) {
-      int nblk, nchunks;
-      linattn_partition(B, N, &nblk, &nchunks);
-      info[1] = nblk; info[2] = nchunks;
-      cudaMemcpyAsync(ctx_out, cx, (size_t)B * 4096 * sizeof(float), cudaMemcpyDeviceToDevice, st);
-    }
-    info[0] = kern;
-    ctx->launches += lin ? 3 : 1;
+  if (!launched) return fail(ctx, IRSDE_ERR_INVALID, "the linear-attention launcher refused the views");
+  if (lin) {
+    int nblk, nchunks;
+    linattn_partition(B, N, &nblk, &nchunks);
+    info[1] = nblk; info[2] = nchunks;
+    cudaMemcpyAsync(ctx_out, cx, (size_t)B * 4096 * sizeof(float), cudaMemcpyDeviceToDevice, sc.st);
   }
-  return finish_op(ctx, rc, "attention failed: ", st, tmp);
+  info[0] = kern;
+  ctx->launches += lin ? 3 : 1;
+  return sc.finish(IRSDE_OK, "attention failed");
 }
 
 int irsde_linattn_block(irsde_ctx* ctx, const float* x, int32_t x_pitch, int32_t x_off, float* out, int32_t out_pitch,
@@ -2628,40 +2575,32 @@ int irsde_linattn_block(irsde_ctx* ctx, const float* x, int32_t x_pitch, int32_t
   if (B < 1 || N < 1) return fail(ctx, IRSDE_ERR_INVALID, "bad shape");
   if (int rc = check_shape_limits(ctx, B, "B", N, 1)) return rc;
   if (C != 64 && C != 128) return fail(ctx, IRSDE_ERR_UNSUPPORTED, "the fused linear-attention block takes C = 64 or 128");
-  if (x_off < 0 || (long long)x_off + C > x_pitch) return fail(ctx, IRSDE_ERR_INVALID, "input view outside its pitch");
-  if (out_off < 0 || (long long)out_off + C > out_pitch) return fail(ctx, IRSDE_ERR_INVALID, "output view outside its pitch");
+  if (!view_ok(x_pitch, x_off, C)) return fail(ctx, IRSDE_ERR_INVALID, "input view outside its pitch");
+  if (!view_ok(out_pitch, out_off, C)) return fail(ctx, IRSDE_ERR_INVALID, "output view outside its pitch");
   if (x_pitch % 8 || x_off % 8 || out_pitch % 2 || out_off % 2)
     return fail(ctx, IRSDE_ERR_INVALID, "input view: pitch and offset multiples of 8; output view: multiples of 2");
   if (((uintptr_t)g1 | (uintptr_t)g2 | (uintptr_t)bout | (uintptr_t)wout) & 15)
     return fail(ctx, IRSDE_ERR_INVALID, "g1, g2, bout and wout must start on 16 bytes");
   cudaSetDevice(ctx->cfg.device);
-  cudaStream_t st = (cudaStream_t)stream;
-  const long long npix = (long long)B * N, nx = npix * x_pitch, no = npix * out_pitch;
-  std::vector<void*> tmp;
-  int rc = IRSDE_OK;
-  float* part = (float*)dev_alloc(ctx, linattn_partial_floats(B, N) * sizeof(float), &tmp);
-  float* cx = (float*)dev_alloc(ctx, (size_t)B * 4096 * sizeof(float), &tmp);
-  bf16* xb = (bf16*)dev_alloc(ctx, nx * 2, &tmp);
-  bf16* ob = (bf16*)dev_alloc(ctx, no * 2, &tmp);
-  bf16* wp = (bf16*)dev_alloc(ctx, (size_t)384 * C * 2, &tmp);
-  bf16* Mb = (bf16*)dev_alloc(ctx, (size_t)B * C * 128 * 2, &tmp);
-  bf16* xnb = xn_out ? (bf16*)dev_alloc(ctx, npix * C * 2, &tmp) : nullptr;
-  if (!part || !cx || !xb || !ob || !wp || !Mb || (xn_out && !xnb)) rc = fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
-  if (!rc && !linattn_fused_ok(C, xb + x_off, x_pitch, ob + out_off, out_pitch))
-    rc = fail(ctx, IRSDE_ERR_INVALID, "the fused linear-attention passes refused the views");
-  if (!rc) {
-    cast_f32_bf16_kernel<<<cast_blocks(nx), 256, 0, st>>>(x, xb, nx);
-    cast_f32_bf16_kernel<<<cast_blocks(no), 256, 0, st>>>(out, ob, no);
-    pack_weight<bf16>(WL_TAPS, wqkv, wp, 384, C, 1, 1, 1, st);  // the layout irsde_finalize_weights gives to_qkv
-    launch_la_kv_ln(xb + x_off, x_pitch, g1, wp + 128 * C, part, B, N, C, xnb, st);
-    launch_la_combine(part, cx, B, N, st);
-    launch_la_fold(cx, wout, Mb, B, C, st);
-    launch_la_out_ln(xb + x_off, x_pitch, g1, wp, Mb, bout, g2, ob + out_off, out_pitch, B, N, C, st);
-    cast_bf16_f32_kernel<<<cast_blocks(no), 256, 0, st>>>(ob, out, no);
-    if (xnb) cast_bf16_f32_kernel<<<cast_blocks(npix * C), 256, 0, st>>>(xnb, xn_out, npix * C);
-    ctx->launches += 4;
-  }
-  return finish_op(ctx, rc, "linear-attention block failed: ", st, tmp);
+  const long long npix = (long long)B * N;
+  Scratch sc(ctx, (cudaStream_t)stream);
+  float* part = sc.alloc<float>(linattn_partial_floats(B, N));
+  float* cx = sc.alloc<float>((long long)B * 4096);
+  const bf16* xb = sc.in(x, npix * x_pitch);
+  bf16* ob = sc.inout(out, npix * out_pitch);
+  bf16* wp = sc.alloc<bf16>(384LL * C);
+  bf16* Mb = sc.alloc<bf16>((long long)B * C * 128);
+  bf16* xnb = xn_out ? sc.out(xn_out, npix * C) : nullptr;
+  if (!part || !cx || !xb || !ob || !wp || !Mb || (xn_out && !xnb)) return sc.oom();
+  if (!linattn_fused_ok(C, xb + x_off, x_pitch, ob + out_off, out_pitch))
+    return fail(ctx, IRSDE_ERR_INVALID, "the fused linear-attention passes refused the views");
+  pack_weight<bf16>(WL_TAPS, wqkv, wp, 384, C, 1, 1, 1, sc.st);  // the layout irsde_finalize_weights gives to_qkv
+  launch_la_kv_ln(xb + x_off, x_pitch, g1, wp + 128 * C, part, B, N, C, xnb, sc.st);
+  launch_la_combine(part, cx, B, N, sc.st);
+  launch_la_fold(cx, wout, Mb, B, C, sc.st);
+  launch_la_out_ln(xb + x_off, x_pitch, g1, wp, Mb, bout, g2, ob + out_off, out_pitch, B, N, C, sc.st);
+  ctx->launches += 4;
+  return sc.finish(IRSDE_OK, "linear-attention block failed");
 }
 
 // ---- one NAFNet op, time embedding, sampler step or input packing outside a plan ----------------------------------
@@ -2678,68 +2617,55 @@ int irsde_nafnet_op(irsde_ctx* ctx, int32_t precision, int32_t kind, const irsde
   if (dw && c > kScaMaxC) return fail(ctx, IRSDE_ERR_UNSUPPORTED, "c > 12288: the SCA mat-vec needs more than 48 KB of shared memory");
   if (dw && (!a.w || !a.bias || !a.sca_w || !a.sca_b || !a.sca)) return fail(ctx, IRSDE_ERR_INVALID, "DWGATE_SCA needs w, bias, sca_w, sca_b and sca");
   if ((ps || kind == IRSDE_NAF_ADD) && !a.y) return fail(ctx, IRSDE_ERR_INVALID, "PIXEL_SHUFFLE_ADD and ADD need y");
-  auto view_ok = [](int pitch, int off, long long width) { return off >= 0 && (long long)off + width <= pitch; };
   const long long xw = ps ? 4LL * c : kind == IRSDE_NAF_ADD ? c : 2LL * c;
   if (!view_ok(a.x_pitch, a.x_off, xw)) return fail(ctx, IRSDE_ERR_INVALID, "x view outside its pitch");
   if (a.y && (ps || kind == IRSDE_NAF_ADD) && !view_ok(a.y_pitch, a.y_off, c)) return fail(ctx, IRSDE_ERR_INVALID, "y view outside its pitch");
   if (!view_ok(a.out_pitch, a.out_off, c)) return fail(ctx, IRSDE_ERR_INVALID, "out view outside its pitch");
   int32_t info_local[4];
-  if (!info) info = info_local;
-  info[0] = info[1] = info[2] = info[3] = 0;
+  info = zeroed_info(info, info_local);
 
   cudaSetDevice(ctx->cfg.device);
-  cudaStream_t st = (cudaStream_t)stream;
   const int N = H * W;
   const long long npix_in = (long long)B * N, npix_out = ps ? 4 * npix_in : npix_in;  // PIXEL_SHUFFLE_ADD: H x W is the input
   const int nchunks = dw ? dwgate_chunks(H, W) : 0;
-  std::vector<void*> tmp;
-  int rc = IRSDE_OK;
-  float* partial = dw ? (float*)dev_alloc(ctx, (size_t)B * nchunks * c * sizeof(float), &tmp) : nullptr;
-  if (dw && !partial) rc = fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
+  Scratch sc(ctx, (cudaStream_t)stream);
+  float* partial = dw ? sc.alloc<float>((long long)B * nchunks * c) : nullptr;
+  if (dw && !partial) return sc.oom();
   int sca_launches = 0;
   // one launch path for both storage types: S = float views of the caller's buffers, or bf16 copies of them
   auto run = [&](auto* xs, auto* ys, auto* os) {
-    using S = std::remove_const_t<std::remove_pointer_t<decltype(xs)>>;
+    using S = std::remove_pointer_t<decltype(os)>;
     const S* xv = xs + a.x_off;
     const S* yv = ys ? ys + a.y_off : nullptr;
     S* ov = os + a.out_off;
     if (dw) {
-      launch_dwgate<S>(xv, a.x_pitch, a.w, a.bias, ov, a.out_pitch, partial, B, H, W, c, st);
-      launch_sca_scale<S>(partial, a.sca_w, a.sca_b, a.sca, ov, a.out_pitch, B, c, nchunks, N, &sca_launches, st);
+      launch_dwgate<S>(xv, a.x_pitch, a.w, a.bias, ov, a.out_pitch, partial, B, H, W, c, sc.st);
+      launch_sca_scale<S>(partial, a.sca_w, a.sca_b, a.sca, ov, a.out_pitch, B, c, nchunks, N, &sca_launches, sc.st);
     } else if (kind == IRSDE_NAF_SIMPLE_GATE) {
-      launch_simple_gate<S>(xv, a.x_pitch, ov, a.out_pitch, npix_in, c, st);
+      launch_simple_gate<S>(xv, a.x_pitch, ov, a.out_pitch, npix_in, c, sc.st);
     } else if (ps) {
-      launch_pixel_shuffle_add<S>(xv, a.x_pitch, yv, a.y_pitch, ov, a.out_pitch, B, H, W, c, st);
+      launch_pixel_shuffle_add<S>(xv, a.x_pitch, yv, a.y_pitch, ov, a.out_pitch, B, H, W, c, sc.st);
     } else {
-      launch_add<S>(xv, a.x_pitch, yv, a.y_pitch, ov, a.out_pitch, npix_in, c, st);
+      launch_add<S>(xv, a.x_pitch, yv, a.y_pitch, ov, a.out_pitch, npix_in, c, sc.st);
     }
   };
   const bool has_y = ps || kind == IRSDE_NAF_ADD;
-  if (!rc && precision == IRSDE_PREC_BF16) {
-    const long long nx = npix_in * a.x_pitch, ny = has_y ? npix_out * a.y_pitch : 0, no = npix_out * a.out_pitch;
-    bf16* xb = (bf16*)dev_alloc(ctx, nx * 2, &tmp);
-    bf16* yb = has_y ? (bf16*)dev_alloc(ctx, ny * 2, &tmp) : nullptr;
-    bf16* ob = (bf16*)dev_alloc(ctx, no * 2, &tmp);
-    if (!xb || !ob || (has_y && !yb)) rc = fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
-    if (!rc) {
-      cast_f32_bf16_kernel<<<cast_blocks(nx), 256, 0, st>>>(a.x, xb, nx);
-      if (yb) cast_f32_bf16_kernel<<<cast_blocks(ny), 256, 0, st>>>(a.y, yb, ny);
-      cast_f32_bf16_kernel<<<cast_blocks(no), 256, 0, st>>>(a.out, ob, no);
-      run((const bf16*)xb, (const bf16*)yb, ob);
-      cast_bf16_f32_kernel<<<cast_blocks(no), 256, 0, st>>>(ob, a.out, no);
-    }
-  } else if (!rc) {
+  if (precision == IRSDE_PREC_BF16) {
+    const bf16* xb = sc.in(a.x, npix_in * a.x_pitch);
+    const bf16* yb = has_y ? sc.in(a.y, npix_out * a.y_pitch) : nullptr;
+    bf16* ob = sc.inout(a.out, npix_out * a.out_pitch);
+    if (!xb || !ob || (has_y && !yb)) return sc.oom();
+    run(xb, yb, ob);
+  } else {
     run(a.x, has_y ? a.y : (const float*)nullptr, a.out);
   }
-  if (!rc) {
-    if (dw) {
-      info[0] = dw_pix(N); info[1] = nchunks; info[2] = sca_launches;
-      ctx->launches += 1 + sca_launches;
-    } else {
-      ctx->launches++;
-    }
+  if (dw) {
+    info[0] = dw_pix(N); info[1] = nchunks; info[2] = sca_launches;
+    ctx->launches += 1 + sca_launches;
+  } else {
+    ctx->launches++;
   }
-  return finish_op(ctx, rc, "NAFNet op failed: ", st, tmp);
+  return sc.finish(IRSDE_OK, "NAFNet op failed");
 }
 
 int irsde_step_philox(irsde_ctx* ctx, int32_t mode, const float* x, const float* mu, const float* noise, int32_t t, float* out,
@@ -2770,17 +2696,14 @@ int irsde_time_embedding(int32_t family, const float* times, int32_t rows, int32
   if (int rc = check_shape_limits(nullptr, rows, "rows", 1, 1)) return rc;
   if ((family == 0 ? time_mlp_smem(width) : naf_time_mlp_smem(width)) > kTimeMlpSmemMax)
     return fail(nullptr, IRSDE_ERR_UNSUPPORTED, "the time MLP of this width needs more than 48 KB of shared memory");
-  cudaStream_t st = (cudaStream_t)stream;
+  Scratch sc(nullptr, (cudaStream_t)stream);
   if (family == 0) {
-    launch_time_table(times, rows, width, w1, b1, w2, b2, wall, ball, S, temb, table, st);
+    launch_time_table(times, rows, width, w1, b1, w2, b2, wall, ball, S, temb, table, sc.st);
   } else {
-    launch_naf_time_gate(times, rows, width, w1, b1, w2, b2, temb, st);
-    launch_time_rows(temb, rows, 2 * width, wall, ball, S, table, st);
+    launch_naf_time_gate(times, rows, width, w1, b1, w2, b2, temb, sc.st);
+    launch_time_rows(temb, rows, 2 * width, wall, ball, S, table, sc.st);
   }
-  cudaError_t ce = cudaStreamSynchronize(st);
-  if (ce == cudaSuccess) ce = cudaGetLastError();
-  if (ce != cudaSuccess) return fail(nullptr, IRSDE_ERR_CUDA, std::string("time embedding failed: ") + cudaGetErrorString(ce));
-  return IRSDE_OK;
+  return sc.finish(IRSDE_OK, "time embedding failed");
 }
 
 int irsde_prep_input(int32_t precision, const float* xt, const float* cond, float* out, int32_t B, int32_t C, int32_t H, int32_t W,
@@ -2796,23 +2719,19 @@ int irsde_prep_input(int32_t precision, const float* xt, const float* cond, floa
   if (row_pix != 0 && (pad_top < 0 || pad_left < 0 || (long long)pad_top + Hp > img_rows || (long long)pad_left + Wp > row_pix))
     return fail(nullptr, IRSDE_ERR_INVALID, "the padded image does not fit inside its border");
   const long long n = (long long)B * (row_pix ? (long long)img_rows * row_pix : (long long)Hp * Wp) * pitch;
-  cudaStream_t st = (cudaStream_t)stream;
-  bf16* ob = nullptr;
+  Scratch sc(nullptr, (cudaStream_t)stream);
+  auto run = [&](auto* o) {
+    launch_prep_input(xt, cond, o, B, C, H, W, Hp, Wp, pitch, conditional ? 1 : 0, sc.st, pad_top, pad_left, row_pix, img_rows,
+                      zero_pad ? 1 : 0);
+  };
   if (precision == IRSDE_PREC_BF16) {
-    if (cudaMalloc(&ob, n * 2) != cudaSuccess) return fail(nullptr, IRSDE_ERR_CUDA, "cudaMalloc failed");
-    cast_f32_bf16_kernel<<<cast_blocks(n), 256, 0, st>>>(out, ob, n);
-    launch_prep_input<bf16>(xt, cond, ob, B, C, H, W, Hp, Wp, pitch, conditional ? 1 : 0, st, pad_top, pad_left, row_pix, img_rows,
-                            zero_pad ? 1 : 0);
-    cast_bf16_f32_kernel<<<cast_blocks(n), 256, 0, st>>>(ob, out, n);
+    bf16* ob = sc.inout(out, n);
+    if (!ob) return sc.oom();
+    run(ob);
   } else {
-    launch_prep_input<float>(xt, cond, out, B, C, H, W, Hp, Wp, pitch, conditional ? 1 : 0, st, pad_top, pad_left, row_pix, img_rows,
-                             zero_pad ? 1 : 0);
+    run(out);
   }
-  cudaError_t ce = cudaStreamSynchronize(st);
-  if (ce == cudaSuccess) ce = cudaGetLastError();
-  if (ob) cudaFree(ob);
-  if (ce != cudaSuccess) return fail(nullptr, IRSDE_ERR_CUDA, std::string("prep_input failed: ") + cudaGetErrorString(ce));
-  return IRSDE_OK;
+  return sc.finish(IRSDE_OK, "prep_input failed");
 }
 
 // ---- image conversion / metrics (stateless) ----------------------------------------------------------------
