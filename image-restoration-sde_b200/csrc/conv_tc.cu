@@ -10,13 +10,15 @@
 // This one kernel serves: 3x3 (9 taps), 1x1 (1 tap), 4x4/s2 (16 taps over 4 space-to-depth planes),
 // nearest-x2-upsample + 3x3 (4 output phases x 4 taps with pre-summed weights).
 //
-// One persistent kernel (conv_tc_persist_kernel<BN, MODE, EKT>), 288 threads: warps 0..7 = two consumer warpgroups (each
-// issues wgmma.m64nBNk16 for 64 of the 128 pixel rows into its registers, then runs the epilogue: registers -> fp32 staging
-// in shared memory -> bias / (scale+1)*x+shift / SiLU / q-softmax / +residual -> bf16 -> swizzled staging -> TMA bulk store
-// at the channel offset of the destination concat buffer), warp 8 = TMA producer.  Pipeline: STAGES-deep smem ring with
-// full/empty mbarriers.  Each consumer warpgroup issues a stage's MMAs as one wgmma group and keeps it in flight while it
-// waits for the next stage's bytes and issues that stage's group; wgmma.wait_group 1 then shows the older group done and
-// the warpgroup releases its slot.  The producer runs ahead into the next tile while the consumers run the epilogue.
+// One persistent kernel (conv_tc_persist_kernel<BN, MODE, EKT>), 384 threads: warps 0..7 = two consumer warpgroups (each
+// issues wgmma.m64nBNk16 into its registers, then runs the epilogue: registers -> fp32 staging in shared memory -> bias /
+// (scale+1)*x+shift / SiLU / q-softmax / +residual -> bf16 -> swizzled staging -> TMA bulk store at the channel offset of
+// the destination concat buffer), warp 8 = TMA producer (warps 9..11 only give their registers to the consumers: setmaxnreg
+// 40 / 232).  Schedule: bf16 BN = 64 / 128 PING-PONG (a warpgroup computes all 128 rows of every other tile, so its
+// epilogue overlaps the other warpgroup's MMAs), otherwise COOPERATIVE (each warpgroup 64 rows of every tile).
+// Pipeline: STAGES-deep smem ring with full/empty mbarriers.  Each consumer warpgroup issues a stage's MMAs as one wgmma
+// group and keeps it in flight while it waits for the next stage's bytes and issues that stage's group; wgmma.wait_group 1
+// then shows the older group done and the warpgroup releases its slot.  The producer runs ahead into the next tile.
 // No function call may sit inside the wgmma window (see mbar_wait), or ptxas serializes every wgmma; the kernel makes no
 // external call at all.  (The fp32x3 epilogue keeps calls to the IEEE-division slow path, a subroutine of the kernel
 // itself that runs after the K loop's final wait.)
@@ -98,6 +100,8 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
 // compiles to a call of vprintf, and ptxas serializes every wgmma of a kernel whose wgmma window contains a function call
 // (warning C7510: each HGMMA is then followed by a wait for zero groups in flight).  The consumers wait here while their
 // previous stage's MMAs are still running, so the call must not exist; tests/test_conv_tc_sass.py checks that it does not.
+// The launch is failed by a store to address 0 rather than by `trap`: a reachable trap makes ptxas hold the consumer
+// warpgroups to the launch's 168 registers even after setmaxnreg has raised them to 232, and the ping-pong tiles spill.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   long long t0 = 0;
   uint32_t spins = 0;
@@ -105,7 +109,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     if ((++spins & 0xfffu) == 0) {
       long long now = clock64();
       if (t0 == 0) t0 = now;
-      else if (now - t0 > 4000000000LL) __trap();  // ~2 s
+      else if (now - t0 > 4000000000LL) asm volatile("st.global.u32 [%0], 0;" ::"l"(0ull) : "memory");  // ~2 s: fault
     }
   }
 }
@@ -241,10 +245,14 @@ struct TcCfgP {
   // Epilogue staging for the TMA stores: STG_BUFS = 1 is one 2 KB tile per consumer warp; 0: no TMA store (fp32x3) or the
   // tile is inside the fp32 staging rows (COMPACT).
   static constexpr int STG_BUFS = (TF3 || COMPACT) ? 0 : 1;
+  // PING-PONG schedule (bf16, BN = 64 / 128): a CTA's tiles alternate between the two consumer warpgroups, each computing
+  // all 128 rows of its tile, so one warpgroup's epilogue runs while the other issues its MMAs.  BN = 256 (128 accumulator
+  // registers per 64 rows), BN = 32 and fp32x3 keep the COOPERATIVE schedule: both warpgroups on one tile, 64 rows each.
+  static constexpr bool PP = !TF3 && (BN == 64 || BN == 128);
   static constexpr int BSUB = ROWS ? 3 : (TF3 ? 2 : 1);  // weight tiles per stage
   static constexpr int A_SLOT = TF3 ? 2 * A_STAGE_BYTES : (ROWS ? ROWS_A_SLOT : A_STAGE_BYTES);
   static constexpr int STAGE_BYTES = A_SLOT + BSUB * B_STAGE_BYTES;
-  static constexpr int EPI_FLOATS = 2 * BN;
+  static constexpr int EPI_FLOATS = 2 * 2 * BN;  // one (mult, add) table per consumer warpgroup
   static constexpr int STG_BYTES = STG_BUFS * 8 * 2048;  // per consumer warp: a 32 rows x 64 B staging tile
   static constexpr int ACC_WG_BYTES = 64 * ACC_PITCH * 4;  // fp32 staging of one warpgroup: 64 rows x ACC_COLS columns
   static constexpr int ACC_BYTES = 2 * ACC_WG_BYTES;
@@ -321,7 +329,7 @@ __device__ __forceinline__ TileCoord decode_tile(const TcParams& P, int tile, in
     if (P.dbg) {                                \
       long long _t0 = clock64();                \
       mbar_wait(bar, par);                      \
-      ctr += clock64() - _t0;                   \
+      ctr += (unsigned)(clock64() - _t0);       \
     } else {                                    \
       mbar_wait(bar, par);                      \
     }                                           \
@@ -331,8 +339,11 @@ __device__ __forceinline__ TileCoord decode_tile(const TcParams& P, int tile, in
 // EKT: EK_* features the epilogue is compiled for.  Only the per-tap and ROWS instantiations that serve the common layer kinds
 // (res_conv: 0, to_qkv: EK_QSM, to_out: EK_AFF, ResBlock convs: EK_AFF|EK_SILU, EK_SILU|EK_RES) are specialised - there the
 // kernel is issue-bound on epilogue instructions; everything else runs EK_GENERIC (every feature checked at run time).
+constexpr int TC_THREADS = 384;  // consumer warpgroups 0 and 1, producer warpgroup 2 (warp 8 issues the TMA loads)
+constexpr int TC_DBG_SLOTS = 16;  // IRSDE_TC_DEBUG counters per CTA
+
 template <int BN, int MODE, int EKT = 16 /* EK_GENERIC */>
-__global__ void __launch_bounds__(288, 1) conv_tc_persist_kernel(const __grid_constant__ CUtensorMap map_a,
+__global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_persist_kernel(const __grid_constant__ CUtensorMap map_a,
                                                                  const __grid_constant__ CUtensorMap map_b,
                                                                  const __grid_constant__ OutMaps map_o,
                                                                  const __grid_constant__ TcParams P, int tiles_m,
@@ -341,7 +352,9 @@ __global__ void __launch_bounds__(288, 1) conv_tc_persist_kernel(const __grid_co
   constexpr bool ROWS = Cfg::ROWS;
   constexpr bool TF3 = Cfg::TF3;
   constexpr int STAGES = Cfg::STAGES;
-  constexpr int NACC = BN / 2;  // accumulator registers per thread: m64 x BN per warpgroup
+  constexpr bool PP = Cfg::PP;
+  constexpr int NACC = BN / 2;  // accumulator registers per thread for one m64 x BN block
+  constexpr int MH = PP ? 2 : 1;  // 64-row halves of a tile held by one warpgroup
   pdl_trigger();  // the next kernel may be scheduled; this one's prologue below touches no global memory
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -360,7 +373,7 @@ __global__ void __launch_bounds__(288, 1) conv_tc_persist_kernel(const __grid_co
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 2);  // one arrive per consumer warpgroup
+      mbar_init(&empty_bar[s], PP ? 1 : 2);  // one arrive per warpgroup that reads the stage
     }
     fence_barrier_init();
   }
@@ -373,7 +386,11 @@ __global__ void __launch_bounds__(288, 1) conv_tc_persist_kernel(const __grid_co
   // (activations, the device step counter behind P.t_ptr) and buffers it may still be reading are overwritten
   pdl_wait();
 
-  if (warp == 8) {
+  // Register split (128 x 40 + 256 x 232 <= 64 K): the launch gives every thread 168, the producer warpgroup hands its
+  // surplus to the consumers, whose ping-pong tiles keep 2 x BN / 2 accumulators per thread.
+  if (warp >= 8) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+    if (warp != 8) return;
     // ================= TMA producer (whole warp loops; one elected lane issues) =================
     int it = 0;
     long long w_prod = 0, t_start = clock64();
@@ -429,34 +446,60 @@ __global__ void __launch_bounds__(288, 1) conv_tc_persist_kernel(const __grid_co
         }
       }
     }
-    if (P.dbg && lane == 0) { P.dbg[blockIdx.x * 8 + 0] = (unsigned long long)w_prod; P.dbg[blockIdx.x * 8 + 1] = (unsigned long long)(clock64() - t_start); }
+    if (P.dbg && lane == 0) {
+      P.dbg[blockIdx.x * TC_DBG_SLOTS + 0] = (unsigned long long)w_prod;
+      P.dbg[blockIdx.x * TC_DBG_SLOTS + 1] = (unsigned long long)(clock64() - t_start);
+    }
     return;
   }
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
 
-  // ================= consumers: warpgroup wg owns pixel rows 64*wg .. 64*wg+63 of every tile =================
+  // ================= consumers =================
+  // COOPERATIVE: warpgroup wg owns pixel rows 64*wg .. 64*wg+63 of every tile.  PING-PONG: warpgroup wg owns every row of
+  // the CTA's tiles lt with lt & 1 == wg; their turns at the tensor cores alternate through named barriers 4 + wg (below).
   const int wg = warp >> 2;
   const int wq = warp & 3;               // wgmma layout: this warp holds accumulator rows 16*wq + lane/4 (+8)
-  const int quad = wg * 2 + (wq & 1);    // epilogue layout: pixel m = quad*32 + lane, 32-channel chunks alternate by `half`
-  const int half = wq >> 1;
-  const int m = quad * 32 + lane;
-  const int et = threadIdx.x;  // 0..255
+  const int half = wq >> 1;              // epilogue layout: 32-channel chunks alternate by `half`
+  const int et = threadIdx.x & 127;
   const int trow = P.t_ptr ? *P.t_ptr : 0;
   const bool affine = (P.ss != nullptr) || (P.bias != nullptr) || (P.mult_vec != nullptr);
   constexpr int ACC_PITCH = Cfg::ACC_PITCH;
   float* const acc_stg = s_acc + wg * 64 * ACC_PITCH;
+  float* const epi = s_epi + wg * 2 * BN;  // this warpgroup's (mult, add) table
   uint8_t* const stg = Cfg::COMPACT ? reinterpret_cast<uint8_t*>(acc_stg) + wq * 2048 : smem_stg + warp * 2048;
-  const uint32_t a_off = (uint32_t)(wg * 64 * 128);  // this warpgroup's 64 pixel rows inside every A box
+  const uint32_t a_off = PP ? 0u : (uint32_t)(wg * 64 * 128);  // cooperative: this warpgroup's 64 pixel rows of every A box
+  const int NST = ROWS ? 3 * P.kchunks : KI;  // ring stages per tile
   const bool signaller = (threadIdx.x & 127) == 0;
-  long long w_full = 0, t_start = clock64();
+  unsigned w_full = 0, w_turn = 0, c_epi = 0;  // debug cycle counts: 32 bits span a launch many times over
+  const unsigned t_start = (unsigned)clock();
   int it = 0, lt = 0, epi_n0 = -1, epi_b = -1;
   for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++lt) {
+    if (PP && (lt & 1) != wg) continue;
+    it = lt * NST;  // the ring position of the tile's first stage (the other warpgroup consumed the stages in between)
     const TileCoord t = decode_tile(P, tile, tiles_m, BN);
-    float acc[NACC];
+    float acc[MH][NACC];
     float sum[TF3 ? NACC : 1];  // fp32x3: the tile's K segments summed with round-to-nearest adds
 #pragma unroll
-    for (int r = 0; r < NACC; ++r) acc[r] = 0.f;
+    for (int h = 0; h < MH; ++h)
+#pragma unroll
+      for (int r = 0; r < NACC; ++r) acc[h][r] = 0.f;
 #pragma unroll
     for (int r = 0; r < (TF3 ? NACC : 1); ++r) sum[r] = 0.f;
+    // Ping-pong turn: wait until the other warpgroup has waited on every full barrier of the previous tile.  Besides
+    // ordering the MMAs, this is what makes the parity waits exact: a warpgroup that ran ahead could otherwise wait on
+    // a slot whose previous fill (the other warpgroup's stage it - STAGES) has not landed yet, and the phase bit of that
+    // barrier would already read as "this fill complete".
+    if constexpr (PP) {
+      if (lt > 0) {
+        const unsigned t0 = (unsigned)clock();
+        asm volatile("bar.sync %0, 256;" ::"r"(4 + wg) : "memory");
+        w_turn += (unsigned)clock() - t0;
+      }
+    }
+    auto pass_turn = [&]() __attribute__((always_inline)) {  // after the tile's last full-barrier wait
+      if constexpr (PP)
+        if (tile + (int)gridDim.x < num_tiles) asm volatile("bar.arrive %0, 256;" ::"r"(4 + (wg ^ 1)) : "memory");
+    };
     // one stage: wait for its bytes, issue this warpgroup's MMAs on it, then release the PREVIOUS stage once its MMAs have
     // finished reading shared memory (one wgmma group stays in flight)
     int prev_s = -1;
@@ -473,7 +516,8 @@ __global__ void __launch_bounds__(288, 1) conv_tc_persist_kernel(const __grid_co
     };
     auto drain = [&]() __attribute__((always_inline)) {
       wgmma_wait<0>();
-      acc_fence<NACC>(acc);
+#pragma unroll
+      for (int h = 0; h < MH; ++h) acc_fence<NACC>(acc[h]);
       if (prev_s >= 0 && signaller) mbar_arrive(&empty_bar[prev_s]);
       prev_s = -1;
     };
@@ -493,58 +537,66 @@ __global__ void __launch_bounds__(288, 1) conv_tc_persist_kernel(const __grid_co
           const uint64_t b_lo = make_sw128_desc(smem_u32(smem_b + (s * 2 + 1) * Cfg::B_STAGE_BYTES));
           // the two small cross terms first, the dominant hi*hi product last
 #pragma unroll
-          for (int k = 0; k < 4; ++k) wgmma_tf32<BN>(acc, a_lo + (uint64_t)(k * 2), b_hi + (uint64_t)(k * 2));
+          for (int k = 0; k < 4; ++k) wgmma_tf32<BN>(acc[0], a_lo + (uint64_t)(k * 2), b_hi + (uint64_t)(k * 2));
 #pragma unroll
-          for (int k = 0; k < 4; ++k) wgmma_tf32<BN>(acc, a_hi + (uint64_t)(k * 2), b_lo + (uint64_t)(k * 2));
+          for (int k = 0; k < 4; ++k) wgmma_tf32<BN>(acc[0], a_hi + (uint64_t)(k * 2), b_lo + (uint64_t)(k * 2));
 #pragma unroll
-          for (int k = 0; k < 4; ++k) wgmma_tf32<BN>(acc, a_hi + (uint64_t)(k * 2), b_hi + (uint64_t)(k * 2));
+          for (int k = 0; k < 4; ++k) wgmma_tf32<BN>(acc[0], a_hi + (uint64_t)(k * 2), b_hi + (uint64_t)(k * 2));
           stage_end(s);
         }
         drain();
 #pragma unroll
         for (int r = 0; r < NACC; ++r) {
-          sum[(TF3 ? r : 0)] = __fadd_rn(sum[(TF3 ? r : 0)], acc[r]);
-          acc[r] = 0.f;
+          sum[(TF3 ? r : 0)] = __fadd_rn(sum[(TF3 ? r : 0)], acc[0][r]);
+          acc[0][r] = 0.f;
         }
       }
     } else if constexpr (ROWS) {
-      const int nst = 3 * P.kchunks;
-      for (int si = 0; si < nst; ++si) {
+      for (int si = 0; si < NST; ++si) {
         const int s = it % STAGES;
         stage_begin(s);
         const uint32_t a0 = smem_u32(smem_a + s * ROWS_A_SLOT) + a_off;
 #pragma unroll
         for (int j = 0; j < 3; ++j) {  // vertical tap dh = j-1: row window starting j*BW pixel rows into the box
-          const uint64_t adesc = make_sw128_desc(a0 + (uint32_t)(j * P.BW * 128));
           const uint64_t bdesc = make_sw128_desc(smem_u32(smem_b + (s * 3 + j) * Cfg::B_STAGE_BYTES));
 #pragma unroll
-          for (int k = 0; k < 4; ++k) wgmma_bf16<BN>(acc, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2));
+          for (int h = 0; h < MH; ++h) {
+            const uint64_t adesc = make_sw128_desc(a0 + (uint32_t)(j * P.BW * 128 + h * 64 * 128));
+#pragma unroll
+            for (int k = 0; k < 4; ++k) wgmma_bf16<BN>(acc[h], adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2));
+          }
         }
         stage_end(s);
       }
+      pass_turn();
       drain();
     } else {
       for (int ki = 0; ki < KI; ++ki) {
         const int s = it % STAGES;
         stage_begin(s);
-        const uint64_t adesc = make_sw128_desc(smem_u32(smem_a + s * A_STAGE_BYTES) + a_off);
         const uint64_t bdesc = make_sw128_desc(smem_u32(smem_b + s * Cfg::B_STAGE_BYTES));
 #pragma unroll
-        for (int k = 0; k < 4; ++k) wgmma_bf16<BN>(acc, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2));
+        for (int h = 0; h < MH; ++h) {
+          const uint64_t adesc = make_sw128_desc(smem_u32(smem_a + s * A_STAGE_BYTES) + a_off + (uint32_t)(h * 64 * 128));
+#pragma unroll
+          for (int k = 0; k < 4; ++k) wgmma_bf16<BN>(acc[h], adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2));
+        }
         stage_end(s);
       }
+      pass_turn();
       drain();
     }
 
     // ---- epilogue
+    const unsigned t_epi = (unsigned)clock();
     // The per-channel (mult, add) table depends on the N tile (and on the image only with per-image timesteps):
-    // rebuild it - two barriers and a dependent global load - only when that changes.
+    // rebuild it - two warpgroup barriers and a dependent global load - only when that changes.
     const int key_b = P.ss_img_stride ? t.b : 0;
     if (affine && (t.n0 != epi_n0 || key_b != epi_b)) {
       epi_n0 = t.n0; epi_b = key_b;
-      asm volatile("bar.sync 1, 256;" ::: "memory");  // previous tile's reads of s_epi are done
+      asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");  // previous tile's reads of the table are done
       const float* ssrow = P.ss ? P.ss + (long long)(trow + t.b * P.ss_img_stride) * P.ss_S + P.ss_off : nullptr;
-      for (int j = et; j < BN; j += 256) {
+      for (int j = et; j < BN; j += 128) {
         const int n = t.n0 + j;
         float mult = 1.f, add = 0.f, bias = 0.f;
         if (n < P.Cout) {
@@ -552,33 +604,95 @@ __global__ void __launch_bounds__(288, 1) conv_tc_persist_kernel(const __grid_co
           if (P.mult_vec) mult *= P.mult_vec[n];
           if (P.bias) bias = P.bias[n];
         }
-        s_epi[j] = mult; s_epi[BN + j] = bias * mult + add;  // (x + bias) * mult + add == x * mult + (bias * mult + add)
+        epi[j] = mult; epi[BN + j] = bias * mult + add;  // (x + bias) * mult + add == x * mult + (bias * mult + add)
       }
-      asm volatile("bar.sync 1, 256;" ::: "memory");
+      asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
     }
-    const int hh = t.h0 + (m >> P.logBW), ww = t.w0 + (m & (P.BW - 1));
-    const bool pvalid = hh < P.H && ww < P.W;
-    const long long opix = ((long long)t.b * P.Hout + (hh * P.os + t.py)) * P.Wout + (ww * P.os + t.px);
-    const bf16* rrow = P.res ? P.res + opix * P.res_pitch + t.n0 : nullptr;
-      // KC: std::integral_constant<int, KIND>.  KIND = the EK_* features this conv has, fixed per launch: feature blocks
-      // outside KIND do not exist in the instantiation (the compiler had turned several of them into predicated code that
-      // was issued for every chunk), EK_GENERIC keeps every run-time check and the fp32 NCHW output.
-      auto process = [&](auto KC, uint32_t* v, const int c0) __attribute__((always_inline)) {
-        constexpr int KIND = decltype(KC)::value;
-        constexpr bool GEN = KIND == EK_GENERIC;
-        if constexpr (TF3) {  // fp32 in, fp32 out: IEEE arithmetic, no fast-math approximations
-          if (affine) {
+    // one 64-row half of the tile per pass: its accumulators go through this warpgroup's staging rows
 #pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(fmaf(__uint_as_float(v[j]), s_epi[c0 + j], s_epi[BN + c0 + j]));
+    for (int h = 0; h < MH; ++h) {
+      const int quad = (PP ? h : wg) * 2 + (wq & 1);  // pixel m = quad*32 + lane of the tile
+      const int m = quad * 32 + lane;
+      const int hh = t.h0 + (m >> P.logBW), ww = t.w0 + (m & (P.BW - 1));
+      const bool pvalid = hh < P.H && ww < P.W;
+      const long long opix = ((long long)t.b * P.Hout + (hh * P.os + t.py)) * P.Wout + (ww * P.os + t.px);
+      const bf16* rrow = P.res ? P.res + opix * P.res_pitch + t.n0 : nullptr;
+        // KC: std::integral_constant<int, KIND>.  KIND = the EK_* features this conv has, fixed per launch: feature blocks
+        // outside KIND do not exist in the instantiation (the compiler had turned several of them into predicated code that
+        // was issued for every chunk), EK_GENERIC keeps every run-time check and the fp32 NCHW output.
+        auto process = [&](auto KC, uint32_t* v, const int c0) __attribute__((always_inline)) {
+          constexpr int KIND = decltype(KC)::value;
+          constexpr bool GEN = KIND == EK_GENERIC;
+          if constexpr (TF3) {  // fp32 in, fp32 out: IEEE arithmetic, no fast-math approximations
+            if (affine) {
+#pragma unroll
+              for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(fmaf(__uint_as_float(v[j]), epi[c0 + j], epi[BN + c0 + j]));
+            }
+            if (P.silu) {
+#pragma unroll
+              for (int j = 0; j < 32; ++j) {
+                const float x = __uint_as_float(v[j]);
+                v[j] = __float_as_uint(x / (1.0f + expf(-x)));
+              }
+            }
+            if (P.out_nchw) {
+              if (pvalid && hh < P.cropH && ww < P.cropW) {
+#pragma unroll
+                for (int j = 0; j < 32; ++j) {
+                  const int n = t.n0 + c0 + j;
+                  if (n < P.Cout) P.out_nchw[(((long long)t.b * P.Cout + n) * P.cropH + hh) * P.cropW + ww] = __uint_as_float(v[j]);
+                }
+              }
+              return;
+            }
+            if (!pvalid) return;
+            float* of = P.out_f32 + opix * P.out_pitch + t.n0 + c0;
+            const float* rf = P.res_f32 ? P.res_f32 + opix * P.res_pitch + t.n0 + c0 : nullptr;
+#pragma unroll
+            for (int g = 0; g < 8; ++g) {
+              if (t.n0 + c0 + g * 4 < P.Cout) {
+                float4 o = make_float4(__uint_as_float(v[g * 4]), __uint_as_float(v[g * 4 + 1]), __uint_as_float(v[g * 4 + 2]),
+                                       __uint_as_float(v[g * 4 + 3]));
+                if (rf) {
+                  const float4 r = *reinterpret_cast<const float4*>(rf + g * 4);
+                  o.x += r.x; o.y += r.y; o.z += r.z; o.w += r.w;
+                }
+                *reinterpret_cast<float4*>(of + g * 4) = o;
+              }
+            }
+            return;
           }
-          if (P.silu) {
+          if constexpr (GEN || (KIND & EK_QSM)) if ((!GEN || P.qsm) && t.n0 + c0 < 128) {  // one chunk == one attention head of this pixel's q (module_util.py:168,171)
+            float mx = __uint_as_float(v[0]);
+#pragma unroll
+            for (int j = 1; j < 32; ++j) mx = fmaxf(mx, __uint_as_float(v[j]));
+            float sm = 0.f;
 #pragma unroll
             for (int j = 0; j < 32; ++j) {
+              const float e = __expf(__uint_as_float(v[j]) - mx);
+              v[j] = __float_as_uint(e);
+              sm += e;
+            }
+            const float inv = __fdividef(0.17677669529663687f, sm);
+#pragma unroll
+            for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(__uint_as_float(v[j]) * inv);
+          }
+          if constexpr (GEN || (KIND & EK_AFF)) if (!GEN || affine) {
+#pragma unroll
+            for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(fmaf(__uint_as_float(v[j]), epi[c0 + j], epi[BN + c0 + j]));
+          }
+          if constexpr (GEN || (KIND & EK_SILU)) if (!GEN || P.silu) {
+#pragma unroll
+            for (int j = 0; j < 32; ++j) {
+              // SiLU(x) = x * (0.5 + 0.5 tanh(x/2)): one MUFU op (tanh.approx, rel. error 2^-11 << bf16 rounding) instead of
+              // ex2 + rcp; on the narrow layers the epilogue is MUFU-bound (128 x BN outputs per tile, 16 MUFU/clk/SM)
               const float x = __uint_as_float(v[j]);
-              v[j] = __float_as_uint(x / (1.0f + expf(-x)));
+              float th;
+              asm("tanh.approx.f32 %0, %1;" : "=f"(th) : "f"(0.5f * x));
+              v[j] = __float_as_uint(x * fmaf(th, 0.5f, 0.5f));
             }
           }
-          if (P.out_nchw) {
+          if constexpr (GEN) if (P.out_nchw) {
             if (pvalid && hh < P.cropH && ww < P.cropW) {
 #pragma unroll
               for (int j = 0; j < 32; ++j) {
@@ -588,175 +702,123 @@ __global__ void __launch_bounds__(288, 1) conv_tc_persist_kernel(const __grid_co
             }
             return;
           }
-          if (!pvalid) return;
-          float* of = P.out_f32 + opix * P.out_pitch + t.n0 + c0;
-          const float* rf = P.res_f32 ? P.res_f32 + opix * P.res_pitch + t.n0 + c0 : nullptr;
+          uint4 ov[4];
 #pragma unroll
-          for (int g = 0; g < 8; ++g) {
-            if (t.n0 + c0 + g * 4 < P.Cout) {
-              float4 o = make_float4(__uint_as_float(v[g * 4]), __uint_as_float(v[g * 4 + 1]), __uint_as_float(v[g * 4 + 2]),
-                                     __uint_as_float(v[g * 4 + 3]));
-              if (rf) {
-                const float4 r = *reinterpret_cast<const float4*>(rf + g * 4);
-                o.x += r.x; o.y += r.y; o.z += r.z; o.w += r.w;
+          for (int g = 0; g < 4; ++g) {
+            const int cg = c0 + g * 8;
+            float f[8];
+#pragma unroll
+            for (int j = 0; j < 8; ++j) f[j] = __uint_as_float(v[g * 8 + j]);
+            if constexpr (GEN || (KIND & EK_RES)) if (rrow && pvalid && t.n0 + cg < P.Cout) {
+              uint4 r = *reinterpret_cast<const uint4*>(rrow + cg);
+              const __nv_bfloat162* r2 = reinterpret_cast<const __nv_bfloat162*>(&r);
+#pragma unroll
+              for (int j = 0; j < 4; ++j) {
+                f[2 * j] += __low2float(r2[j]);
+                f[2 * j + 1] += __high2float(r2[j]);
               }
-              *reinterpret_cast<float4*>(of + g * 4) = o;
             }
+            __nv_bfloat162* o2 = reinterpret_cast<__nv_bfloat162*>(&ov[g]);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) o2[j] = __floats2bfloat162_rn(f[2 * j], f[2 * j + 1]);
           }
-          return;
-        }
-        if constexpr (GEN || (KIND & EK_QSM)) if ((!GEN || P.qsm) && t.n0 + c0 < 128) {  // one chunk == one attention head of this pixel's q (module_util.py:168,171)
-          float mx = __uint_as_float(v[0]);
+          // bf16 NHWC through shared memory + TMA store: each lane owns one pixel row of 32 channels (64 B); the
+          // staging tile uses the 64B swizzle so the 16-byte st.shared are conflict free and the bulk store writes
+          // full, coalesced lines (out-of-range pixels / channels are clipped by TMA).
+          if (lane == 0) bulk_wait_read0();  // the bulk store that last used the tile has finished reading it
+          __syncwarp();
 #pragma unroll
-          for (int j = 1; j < 32; ++j) mx = fmaxf(mx, __uint_as_float(v[j]));
-          float sm = 0.f;
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const float e = __expf(__uint_as_float(v[j]) - mx);
-            v[j] = __float_as_uint(e);
-            sm += e;
+          for (int g = 0; g < 4; ++g)
+            *reinterpret_cast<uint4*>(stg + lane * 64 + ((g ^ ((lane >> 1) & 3)) << 4)) = ov[g];
+          fence_proxy_async();
+          __syncwarp();
+          if (lane == 0) {
+            const int m0 = quad * 32;
+            tma_store_4d(&map_o.m[t.phase], stg, t.n0 + c0, t.w0 + (m0 & (P.BW - 1)), t.h0 + (m0 >> P.logBW), t.b);
+            bulk_commit();
           }
-          const float inv = __fdividef(0.17677669529663687f, sm);
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(__uint_as_float(v[j]) * inv);
-        }
-        if constexpr (GEN || (KIND & EK_AFF)) if (!GEN || affine) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(fmaf(__uint_as_float(v[j]), s_epi[c0 + j], s_epi[BN + c0 + j]));
-        }
-        if constexpr (GEN || (KIND & EK_SILU)) if (!GEN || P.silu) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            // SiLU(x) = x * (0.5 + 0.5 tanh(x/2)): one MUFU op (tanh.approx, rel. error 2^-11 << bf16 rounding) instead of
-            // ex2 + rcp; on the narrow layers the epilogue is MUFU-bound (128 x BN outputs per tile, 16 MUFU/clk/SM)
-            const float x = __uint_as_float(v[j]);
-            float th;
-            asm("tanh.approx.f32 %0, %1;" : "=f"(th) : "f"(0.5f * x));
-            v[j] = __float_as_uint(x * fmaf(th, 0.5f, 0.5f));
-          }
-        }
-        if constexpr (GEN) if (P.out_nchw) {
-          if (pvalid && hh < P.cropH && ww < P.cropW) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              const int n = t.n0 + c0 + j;
-              if (n < P.Cout) P.out_nchw[(((long long)t.b * P.Cout + n) * P.cropH + hh) * P.cropW + ww] = __uint_as_float(v[j]);
-            }
-          }
-          return;
-        }
-        uint4 ov[4];
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          const int cg = c0 + g * 8;
-          float f[8];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) f[j] = __uint_as_float(v[g * 8 + j]);
-          if constexpr (GEN || (KIND & EK_RES)) if (rrow && pvalid && t.n0 + cg < P.Cout) {
-            uint4 r = *reinterpret_cast<const uint4*>(rrow + cg);
-            const __nv_bfloat162* r2 = reinterpret_cast<const __nv_bfloat162*>(&r);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              f[2 * j] += __low2float(r2[j]);
-              f[2 * j + 1] += __high2float(r2[j]);
-            }
-          }
-          __nv_bfloat162* o2 = reinterpret_cast<__nv_bfloat162*>(&ov[g]);
-#pragma unroll
-          for (int j = 0; j < 4; ++j) o2[j] = __floats2bfloat162_rn(f[2 * j], f[2 * j + 1]);
-        }
-        // bf16 NHWC through shared memory + TMA store: each lane owns one pixel row of 32 channels (64 B); the
-        // staging tile uses the 64B swizzle so the 16-byte st.shared are conflict free and the bulk store writes
-        // full, coalesced lines (out-of-range pixels / channels are clipped by TMA).
-        if (lane == 0) bulk_wait_read0();  // the bulk store that last used the tile has finished reading it
-        __syncwarp();
-#pragma unroll
-        for (int g = 0; g < 4; ++g)
-          *reinterpret_cast<uint4*>(stg + lane * 64 + ((g ^ ((lane >> 1) & 3)) << 4)) = ov[g];
-        fence_proxy_async();
-        __syncwarp();
-        if (lane == 0) {
-          const int m0 = quad * 32;
-          tma_store_4d(&map_o.m[t.phase], stg, t.n0 + c0, t.w0 + (m0 & (P.BW - 1)), t.h0 + (m0 >> P.logBW), t.b);
-          bulk_commit();
-        }
-      };
+        };
 
-    // registers (wgmma layout) -> fp32 staging rows (one pixel per row) in 64-column rounds -> per-pixel 32-channel chunks
-    auto fin = [&](int r) __attribute__((always_inline)) -> float {
-      if constexpr (TF3) return sum[r];
-      else return acc[r];
-    };
-    constexpr int NR = (BN + 63) / 64;
-    if constexpr (!Cfg::COMPACT) {
+      // registers (wgmma layout) -> fp32 staging rows (one pixel per row) in 64-column rounds -> per-pixel 32-channel chunks
+      auto fin = [&](int r) __attribute__((always_inline)) -> float {
+        if constexpr (TF3) return sum[r];
+        else return acc[h][r];
+      };
+      constexpr int NR = (BN + 63) / 64;
+      if constexpr (!Cfg::COMPACT) {
 #pragma unroll
-      for (int i = 0; i < NR; ++i) {
-        asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");  // this warpgroup's previous reads of the staging rows are done
-#pragma unroll
-        for (int jj = 0; jj < 8; ++jj) {
-          const int j = i * 8 + jj;  // n8 block of the accumulator: registers 4j .. 4j+3
-          if (j * 8 < BN) {
-            const int row = wq * 16 + (lane >> 2), col = jj * 8 + 2 * (lane & 3);
-            *reinterpret_cast<float2*>(acc_stg + row * ACC_PITCH + col) = make_float2(fin(4 * j), fin(4 * j + 1));
-            *reinterpret_cast<float2*>(acc_stg + (row + 8) * ACC_PITCH + col) = make_float2(fin(4 * j + 2), fin(4 * j + 3));
-          }
-        }
-        asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
-        const int c0 = i * 64 + half * 32;
-        if (c0 < BN && t.n0 + c0 < P.Cout) {  // chunks entirely past Cout carry no output
-          uint32_t v[32];
-          const float* src = acc_stg + ((wq & 1) * 32 + lane) * ACC_PITCH + half * 32;
-#pragma unroll
-          for (int g = 0; g < 8; ++g) {
-            const float4 f = *reinterpret_cast<const float4*>(src + 4 * g);
-            v[4 * g] = __float_as_uint(f.x); v[4 * g + 1] = __float_as_uint(f.y);
-            v[4 * g + 2] = __float_as_uint(f.z); v[4 * g + 3] = __float_as_uint(f.w);
-          }
-          process(std::integral_constant<int, EKT>{}, v, c0);  // EKT: the instantiation's epilogue specialisation
-        }
-      }
-    } else {
-      // COMPACT: a 64-column round is staged in two 32-column passes; pass p carries columns 16p .. 16p+15 of both
-      // 32-channel chunks of the round, so every thread gathers its chunk's 32 values over the two passes.  The bf16
-      // store tiles live in the staging rows: before a round writes them, each warp waits until its previous bulk store
-      // has read its tile, and process() (which writes the tile) starts only after every read of the round.
-#pragma unroll
-      for (int i = 0; i < NR; ++i) {
-        const int c0 = i * 64 + half * 32;  // BN is a multiple of 64 here
-        uint32_t v[32];
-#pragma unroll
-        for (int p = 0; p < 2; ++p) {
-          if (p == 0 && lane == 0) bulk_wait_read0();
-          asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");  // the staging rows are free
+        for (int i = 0; i < NR; ++i) {
+          asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");  // this warpgroup's previous reads of the staging rows are done
 #pragma unroll
           for (int jj = 0; jj < 8; ++jj) {
             const int j = i * 8 + jj;  // n8 block of the accumulator: registers 4j .. 4j+3
-            if (((jj >> 1) & 1) == p) {
-              const int row = wq * 16 + (lane >> 2), col = (jj >> 2) * 16 + (jj & 1) * 8 + 2 * (lane & 3);
+            if (j * 8 < BN) {
+              const int row = wq * 16 + (lane >> 2), col = jj * 8 + 2 * (lane & 3);
               *reinterpret_cast<float2*>(acc_stg + row * ACC_PITCH + col) = make_float2(fin(4 * j), fin(4 * j + 1));
               *reinterpret_cast<float2*>(acc_stg + (row + 8) * ACC_PITCH + col) = make_float2(fin(4 * j + 2), fin(4 * j + 3));
             }
           }
           asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
-          // read even when the chunk is past Cout: v then stays defined on every path (fewer live registers)
-          const float* src = acc_stg + ((wq & 1) * 32 + lane) * ACC_PITCH + half * 16;
+          const int c0 = i * 64 + half * 32;
+          if (c0 < BN && t.n0 + c0 < P.Cout) {  // chunks entirely past Cout carry no output
+            uint32_t v[32];
+            const float* src = acc_stg + ((wq & 1) * 32 + lane) * ACC_PITCH + half * 32;
 #pragma unroll
-          for (int g = 0; g < 4; ++g) {
-            const float4 f = *reinterpret_cast<const float4*>(src + 4 * g);
-            v[p * 16 + 4 * g] = __float_as_uint(f.x); v[p * 16 + 4 * g + 1] = __float_as_uint(f.y);
-            v[p * 16 + 4 * g + 2] = __float_as_uint(f.z); v[p * 16 + 4 * g + 3] = __float_as_uint(f.w);
+            for (int g = 0; g < 8; ++g) {
+              const float4 f = *reinterpret_cast<const float4*>(src + 4 * g);
+              v[4 * g] = __float_as_uint(f.x); v[4 * g + 1] = __float_as_uint(f.y);
+              v[4 * g + 2] = __float_as_uint(f.z); v[4 * g + 3] = __float_as_uint(f.w);
+            }
+            process(std::integral_constant<int, EKT>{}, v, c0);  // EKT: the instantiation's epilogue specialisation
           }
         }
-        asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");  // every read of the round is done
-        if (t.n0 + c0 < P.Cout) process(std::integral_constant<int, EKT>{}, v, c0);
+      } else {
+        // COMPACT: a 64-column round is staged in two 32-column passes; pass p carries columns 16p .. 16p+15 of both
+        // 32-channel chunks of the round, so every thread gathers its chunk's 32 values over the two passes.  The bf16
+        // store tiles live in the staging rows: before a round writes them, each warp waits until its previous bulk store
+        // has read its tile, and process() (which writes the tile) starts only after every read of the round.
+#pragma unroll
+        for (int i = 0; i < NR; ++i) {
+          const int c0 = i * 64 + half * 32;  // BN is a multiple of 64 here
+          uint32_t v[32];
+#pragma unroll
+          for (int p = 0; p < 2; ++p) {
+            if (p == 0 && lane == 0) bulk_wait_read0();
+            asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");  // the staging rows are free
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+              const int j = i * 8 + jj;  // n8 block of the accumulator: registers 4j .. 4j+3
+              if (((jj >> 1) & 1) == p) {
+                const int row = wq * 16 + (lane >> 2), col = (jj >> 2) * 16 + (jj & 1) * 8 + 2 * (lane & 3);
+                *reinterpret_cast<float2*>(acc_stg + row * ACC_PITCH + col) = make_float2(fin(4 * j), fin(4 * j + 1));
+                *reinterpret_cast<float2*>(acc_stg + (row + 8) * ACC_PITCH + col) = make_float2(fin(4 * j + 2), fin(4 * j + 3));
+              }
+            }
+            asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
+            // read even when the chunk is past Cout: v then stays defined on every path (fewer live registers)
+            const float* src = acc_stg + ((wq & 1) * 32 + lane) * ACC_PITCH + half * 16;
+#pragma unroll
+            for (int g = 0; g < 4; ++g) {
+              const float4 f = *reinterpret_cast<const float4*>(src + 4 * g);
+              v[p * 16 + 4 * g] = __float_as_uint(f.x); v[p * 16 + 4 * g + 1] = __float_as_uint(f.y);
+              v[p * 16 + 4 * g + 2] = __float_as_uint(f.z); v[p * 16 + 4 * g + 3] = __float_as_uint(f.w);
+            }
+          }
+          asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");  // every read of the round is done
+          if (t.n0 + c0 < P.Cout) process(std::integral_constant<int, EKT>{}, v, c0);
+        }
       }
     }
+    if (P.dbg) c_epi += (unsigned)clock() - t_epi;
   }
   if (lane == 0) bulk_wait_all();  // staging smem must stay valid until the last bulk store has read it
-  if (P.dbg && threadIdx.x == 0) {
-    P.dbg[blockIdx.x * 8 + 2] = (unsigned long long)w_full;
-    P.dbg[blockIdx.x * 8 + 4] = (unsigned long long)(clock64() - t_start);
-    P.dbg[blockIdx.x * 8 + 7] = (unsigned long long)lt;
+  if (P.dbg && signaller) {
+    unsigned long long* dbg = P.dbg + blockIdx.x * TC_DBG_SLOTS;
+    dbg[2 + wg] = (unsigned long long)w_full;
+    dbg[4 + wg] = (unsigned long long)c_epi;
+    dbg[6 + wg] = (unsigned long long)w_turn;
+    dbg[8 + wg] = (unsigned long long)((unsigned)clock() - t_start);
+    dbg[10 + wg] = (unsigned long long)(PP ? (lt + 1 - wg) / 2 : lt);  // this warpgroup's tiles
   }
 }
 
@@ -1126,12 +1188,12 @@ int tc_conv_launch(TcConvDesc* d, cudaStream_t st) {
     const char* dbg_env = getenv("IRSDE_TC_DEBUG");
     const bool dbg = dbg_env && dbg_env[0] == '1';
     if (dbg) {
-      if (!dbg_dev) cudaMalloc(&dbg_dev, 256 * 8 * sizeof(unsigned long long));
-      cudaMemsetAsync(dbg_dev, 0, 256 * 8 * sizeof(unsigned long long), st);
+      if (!dbg_dev) cudaMalloc(&dbg_dev, 256 * TC_DBG_SLOTS * sizeof(unsigned long long));
+      cudaMemsetAsync(dbg_dev, 0, 256 * TC_DBG_SLOTS * sizeof(unsigned long long), st);
     }
     d->P.dbg = dbg ? dbg_dev : nullptr;
 #define TC_LAUNCH(BNV, PV, EKV)                                                                                            \
-  pdl_launch(conv_tc_persist_kernel<BNV, PV, EKV>, g, 288, TcCfgP<BNV, PV>::SMEM_BYTES, st, d->map_a, d->map_b, d->map_o, d->P, \
+  pdl_launch(conv_tc_persist_kernel<BNV, PV, EKV>, g, TC_THREADS, TcCfgP<BNV, PV>::SMEM_BYTES, st, d->map_a, d->map_b, d->map_o, d->P, \
              d->tiles_m, d->num_tiles)
     const int ekt = tc_launch_ekt(d);
     if (d->mode == 3) {
@@ -1177,13 +1239,18 @@ int tc_conv_launch(TcConvDesc* d, cudaStream_t st) {
     }
 #undef TC_LAUNCH
     if (dbg) {
-      unsigned long long h[256 * 8];
+      // per CTA: [0] producer cycles waiting on empty barriers, [1] producer cycles; per consumer warpgroup w: [2+w] cycles
+      // waiting on full barriers, [4+w] in the epilogue, [6+w] waiting for its ping-pong turn, [8+w] in all, [10+w] tiles
+      unsigned long long h[256 * TC_DBG_SLOTS];
       cudaStreamSynchronize(st);
       cudaMemcpy(h, dbg_dev, sizeof h, cudaMemcpyDeviceToHost);
-      double a[8] = {0};
-      for (unsigned i = 0; i < g; ++i) for (int k = 0; k < 8; ++k) a[k] += (double)h[i * 8 + k] / g;
-      fprintf(stderr, "TCDBG BN=%d mode=%d grid=%u tiles=%d ntaps=%d kch=%d | prod wait %.0f / %.0f | consumer wait full %.0f / %.0f (tiles/cta %.1f)\n",
-              d->BN, d->mode, g, d->num_tiles, d->P.ntaps, d->P.kchunks, a[0], a[1], a[2], a[4], a[7]);
+      double a[TC_DBG_SLOTS] = {0};
+      for (unsigned i = 0; i < g; ++i) for (int k = 0; k < TC_DBG_SLOTS; ++k) a[k] += (double)h[i * TC_DBG_SLOTS + k] / g;
+      fprintf(stderr,
+              "TCDBG BN=%d mode=%d ekt=%d grid=%u tiles=%d ntaps=%d kch=%d | prod wait %.0f / %.0f | wg0 full %.0f epi %.0f turn %.0f"
+              " / %.0f (tiles/cta %.1f) | wg1 full %.0f epi %.0f turn %.0f / %.0f (tiles/cta %.1f)\n",
+              d->BN, d->mode, tc_launch_ekt(d), g, d->num_tiles, d->P.ntaps, d->P.kchunks, a[0], a[1], a[2], a[4], a[6], a[8], a[10],
+              a[3], a[5], a[7], a[9], a[11]);
     }
     return 1;
   }
