@@ -11,9 +11,9 @@
 // nearest-x2-upsample + 3x3 (4 output phases x 4 taps with pre-summed weights).
 //
 // One persistent kernel (conv_tc_persist_kernel<BN, MODE, EKT>), 384 threads: warps 0..7 = two consumer warpgroups (each
-// issues wgmma.m64nBNk16 into its registers, then runs the epilogue: registers -> fp32 staging in shared memory -> bias /
-// (scale+1)*x+shift / SiLU / q-softmax / +residual -> bf16 -> swizzled staging -> TMA bulk store at the channel offset of
-// the destination concat buffer), warp 8 = TMA producer (warps 9..11 only give their registers to the consumers: setmaxnreg
+// issues wgmma.m64nBNk16 into its registers, then runs the epilogue on them: q-softmax / bias / (scale+1)*x+shift / SiLU /
+// +residual (TMA-loaded into the warp's store tile) -> bf16 -> stmatrix into that tile -> TMA bulk store at the channel
+// offset of the destination concat buffer), warp 8 = TMA producer (warps 9..11 only give their registers to the consumers: setmaxnreg
 // 40 / 232).  Schedule: bf16 BN = 64 / 128 PING-PONG (a warpgroup computes all 128 rows of every other tile, so its
 // epilogue overlaps the other warpgroup's MMAs), otherwise COOPERATIVE (each warpgroup 64 rows of every tile).
 // Pipeline: STAGES-deep smem ring with full/empty mbarriers.  Each consumer warpgroup issues a stage's MMAs as one wgmma
@@ -234,17 +234,6 @@ struct TcCfgP {
   static constexpr bool ROWS = MODE == 2;
   static constexpr bool TF3 = MODE == 3;
   static constexpr int B_STAGE_BYTES = BN * 128;
-  // COMPACT epilogue (the two classes whose consumers wait longest on full barriers): the fp32 staging is filled in two
-  // 32-column passes per 64-column round, and each warp's bf16 TMA-store tile lives inside its warpgroup's fp32 staging
-  // rows.  That cuts the shared memory outside the ring from 54 528 B to 21 760 B (BN=256) / 53 504 B to 20 736 B
-  // (ROWS BN=128), which buys each of them one more ring stage.  Cost: per 64-column round three more warpgroup
-  // barriers, and the next round waits for the bulk stores to have read their tiles.
-  static constexpr bool COMPACT = (BN == 256 && MODE == 0) || (BN == 128 && MODE == 2);
-  static constexpr int ACC_COLS = COMPACT ? 32 : 64;      // fp32 columns staged per pass
-  static constexpr int ACC_PITCH = ACC_COLS + 4;          // + 4: conflict-free 16-byte row reads
-  // Epilogue staging for the TMA stores: STG_BUFS = 1 is one 2 KB tile per consumer warp; 0: no TMA store (fp32x3) or the
-  // tile is inside the fp32 staging rows (COMPACT).
-  static constexpr int STG_BUFS = (TF3 || COMPACT) ? 0 : 1;
   // PING-PONG schedule (bf16, BN = 64 / 128): a CTA's tiles alternate between the two consumer warpgroups, each computing
   // all 128 rows of its tile, so one warpgroup's epilogue runs while the other issues its MMAs.  BN = 256 (128 accumulator
   // registers per 64 rows), BN = 32 and fp32x3 keep the COOPERATIVE schedule: both warpgroups on one tile, 64 rows each.
@@ -253,20 +242,31 @@ struct TcCfgP {
   static constexpr int A_SLOT = TF3 ? 2 * A_STAGE_BYTES : (ROWS ? ROWS_A_SLOT : A_STAGE_BYTES);
   static constexpr int STAGE_BYTES = A_SLOT + BSUB * B_STAGE_BYTES;
   static constexpr int EPI_FLOATS = 2 * 2 * BN;  // one (mult, add) table per consumer warpgroup
-  static constexpr int STG_BYTES = STG_BUFS * 8 * 2048;  // per consumer warp: a 32 rows x 64 B staging tile
-  static constexpr int ACC_WG_BYTES = 64 * ACC_PITCH * 4;  // fp32 staging of one warpgroup: 64 rows x ACC_COLS columns
-  static constexpr int ACC_BYTES = 2 * ACC_WG_BYTES;
-  static constexpr int FIXED_BYTES = 1024 + STG_BYTES + ACC_BYTES + EPI_FLOATS * 4 + 256;
-  static constexpr int STAGES_FIT = (SMEM_LIMIT - FIXED_BYTES) / STAGE_BYTES;
+  // fp32x3 only: the accumulators pass through fp32 staging rows, 64 rows x 64 (+4: conflict-free 16-byte row reads)
+  // columns per warpgroup.  The bf16 epilogue works on the accumulator registers.
+  static constexpr int ACC_PITCH = 68;
+  static constexpr int ACC_BYTES = TF3 ? 2 * 64 * ACC_PITCH * 4 : 0;
+  // bf16: STG_BUFS store tiles per consumer warp, each 16 pixel rows x 32 channels (1 KB, 64B swizzle).  The ring takes
+  // as many stages as fit next to two tiles, the tiles then take what the ring leaves (at most four).  Stages / tiles:
+  // per-tap BN=256 / 128 / 64 / 32: 4/3, 6/3, 8/4, 8/4; ROWS BN=128 / 64 / 32: 3/2, 4/4, 6/4; fp32x3 BN=128 / 64 / 32: 2, 3, 4.
+  static constexpr int STG_TILE = 1024;
+  static constexpr int BAR_BYTES = 512;  // full and empty barriers of the ring, one residual barrier per store tile
+  static constexpr int OTHER_BYTES = 1024 + ACC_BYTES + EPI_FLOATS * 4 + BAR_BYTES;
+  static constexpr int STG_MIN = TF3 ? 0 : 2;
+  static constexpr int STAGES_FIT = (SMEM_LIMIT - OTHER_BYTES - STG_MIN * 8 * STG_TILE) / STAGE_BYTES;
   static constexpr int STAGES = STAGES_FIT > 8 ? 8 : STAGES_FIT;
+  static constexpr int STG_FIT = (SMEM_LIMIT - OTHER_BYTES - STAGES * STAGE_BYTES) / (8 * STG_TILE);
+  static constexpr int STG_BUFS = TF3 ? 0 : (STG_FIT > 4 ? 4 : STG_FIT);
+  static constexpr int STG_BYTES = STG_BUFS * 8 * STG_TILE;
+  static constexpr int FIXED_BYTES = OTHER_BYTES + STG_BYTES;
   static constexpr int A_BYTES = STAGES * A_SLOT;
   static constexpr int SMEM_BYTES = FIXED_BYTES + STAGES * STAGE_BYTES;
   static_assert(STAGES >= 2, "shared memory holds fewer than two pipeline stages");
+  static_assert(TF3 || STG_BUFS >= 2, "the bf16 epilogue needs two store tiles per warp");
+  static_assert(2 * 8 + 8 * 4 <= BAR_BYTES / 8, "barrier area too small");
   static_assert(SMEM_BYTES <= SMEM_LIMIT, "over the 227 KB per-CTA shared memory limit");
   static_assert(!(BN == 256 && MODE == 0) || STAGES == 4, "per-tap BN=256 is meant to run a 4-stage ring");
   static_assert(!(BN == 128 && MODE == 2) || STAGES == 3, "ROWS BN=128 is meant to run a 3-stage ring");
-  // COMPACT: four 2 KB store tiles per warpgroup inside its staging rows, 512-byte aligned for the 64B swizzle
-  static_assert(!COMPACT || (4 * 2048 <= ACC_WG_BYTES && ACC_WG_BYTES % 1024 == 0), "store tiles do not fit the staging rows");
 };
 
 // One elected lane of a converged warp (the compiler recognises elect.sync and emits straight-line uniform
@@ -293,9 +293,35 @@ __device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, const void*
                "r"(smem_u32(smem)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
                : "memory");
 }
+__device__ __forceinline__ void tma_load_4d(void* smem, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
+      ::"r"(smem_u32(smem)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+      : "memory");
+}
+__device__ __forceinline__ void tma_prefetch_4d(const CUtensorMap* map, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.prefetch.tensor.4d.L2.global.tile [%0, {%1, %2, %3, %4}];" ::"l"(map), "r"(c0), "r"(c1), "r"(c2),
+               "r"(c3)
+               : "memory");
+}
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// the bulk stores this thread committed, except the N most recent, have finished reading shared memory
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
 __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// four 8 x 8 bf16 matrices in the mma fragment layout (lane l: row l / 4, columns 2 (l % 4), +1); lane l addresses row
+// l % 8 of matrix l / 8
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, const uint32_t* r) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r[0]), "r"(r[1]), "r"(r[2]),
+               "r"(r[3])
+               : "memory");
+}
+__device__ __forceinline__ void ldmatrix_x4(uint32_t addr, uint32_t* r) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(addr)
+               : "memory");
+}
 
 struct TileCoord {
   int b, phase, py, px, h0, w0, n0;
@@ -346,6 +372,7 @@ template <int BN, int MODE, int EKT = 16 /* EK_GENERIC */>
 __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_persist_kernel(const __grid_constant__ CUtensorMap map_a,
                                                                  const __grid_constant__ CUtensorMap map_b,
                                                                  const __grid_constant__ OutMaps map_o,
+                                                                 const __grid_constant__ OutMaps map_r,
                                                                  const __grid_constant__ TcParams P, int tiles_m,
                                                                  int num_tiles) {
   using Cfg = TcCfgP<BN, MODE>;
@@ -360,8 +387,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_persist_kernel(const __
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* smem_a = smem;                       // A ring
   uint8_t* smem_b = smem + Cfg::A_BYTES;
-  uint8_t* smem_stg = smem_b + STAGES * Cfg::BSUB * Cfg::B_STAGE_BYTES;  // 1024-aligned
-  float* s_acc = reinterpret_cast<float*>(smem_stg + Cfg::STG_BYTES);
+  uint8_t* smem_stg = smem_b + STAGES * Cfg::BSUB * Cfg::B_STAGE_BYTES;  // 1024-aligned: bf16 store tiles
+  float* s_acc = reinterpret_cast<float*>(smem_stg + Cfg::STG_BYTES);       // fp32x3 staging rows
   float* s_epi = s_acc + Cfg::ACC_BYTES / 4;
   uint64_t* bars = reinterpret_cast<uint64_t*>(s_epi + Cfg::EPI_FLOATS);
   uint64_t* full_bar = bars;
@@ -375,6 +402,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_persist_kernel(const __
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], PP ? 1 : 2);  // one arrive per warpgroup that reads the stage
     }
+    for (int i = 0; i < 8 * Cfg::STG_BUFS; ++i) mbar_init(&bars[2 * STAGES + i], 1);  // residual loads into store tiles
     fence_barrier_init();
   }
   if (warp == 8 && lane == 0) {
@@ -459,24 +487,64 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_persist_kernel(const __
   // the CTA's tiles lt with lt & 1 == wg; their turns at the tensor cores alternate through named barriers 4 + wg (below).
   const int wg = warp >> 2;
   const int wq = warp & 3;               // wgmma layout: this warp holds accumulator rows 16*wq + lane/4 (+8)
-  const int half = wq >> 1;              // epilogue layout: 32-channel chunks alternate by `half`
   const int et = threadIdx.x & 127;
   const int trow = P.t_ptr ? *P.t_ptr : 0;
   const bool affine = (P.ss != nullptr) || (P.bias != nullptr) || (P.mult_vec != nullptr);
-  constexpr int ACC_PITCH = Cfg::ACC_PITCH;
-  float* const acc_stg = s_acc + wg * 64 * ACC_PITCH;
   float* const epi = s_epi + wg * 2 * BN;  // this warpgroup's (mult, add) table
-  uint8_t* const stg = Cfg::COMPACT ? reinterpret_cast<uint8_t*>(acc_stg) + wq * 2048 : smem_stg + warp * 2048;
   const uint32_t a_off = PP ? 0u : (uint32_t)(wg * 64 * 128);  // cooperative: this warpgroup's 64 pixel rows of every A box
   const int NST = ROWS ? 3 * P.kchunks : KI;  // ring stages per tile
   const bool signaller = (threadIdx.x & 127) == 0;
   unsigned w_full = 0, w_turn = 0, c_epi = 0;  // debug cycle counts: 32 bits span a launch many times over
   const unsigned t_start = (unsigned)clock();
+  // bf16 epilogue: the warp's output goes out in blocks of its 16 accumulator rows x 32 channels, block q of the launch
+  // through store tile q % NBUF, whose barrier res_bar[q % NBUF] signals the block's residual (TMA-loaded into that tile)
+  constexpr int NBUF = TF3 ? 1 : Cfg::STG_BUFS;  // (fp32x3 has no store tiles)
+  constexpr bool GEN = EKT == EK_GENERIC;
+  uint8_t* const stg = smem_stg + warp * NBUF * Cfg::STG_TILE;
+  uint64_t* const res_bar = bars + 2 * STAGES + warp * NBUF;
+  const bool has_res = !TF3 && (GEN ? (P.res != nullptr && P.out_nchw == nullptr) : (EKT & EK_RES) != 0);
+  // stmatrix / ldmatrix address of this lane in a store tile: row lane % 8 of 16-byte chunk lane / 8, 64B swizzle
+  const uint32_t frag_off = (uint32_t)((lane & 7) * 64 + (((lane >> 3) ^ ((lane >> 1) & 3)) << 4));
+  unsigned blk = 0;
   int it = 0, lt = 0, epi_n0 = -1, epi_b = -1;
   for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++lt) {
     if (PP && (lt & 1) != wg) continue;
     it = lt * NST;  // the ring position of the tile's first stage (the other warpgroup consumed the stages in between)
     const TileCoord t = decode_tile(P, tile, tiles_m, BN);
+    // this warp's output blocks of the tile: nblk 32-channel blocks (those below Cout) per 64-row half, halves in order
+    const int nblk = (P.Cout - t.n0 + 31) / 32 < BN / 32 ? (P.Cout - t.n0 + 31) / 32 : BN / 32;
+    const int NB = MH * nblk;
+    // TMA coordinates of block i (c: channel, x, y: image column and row of its first pixel)
+    auto blk_coord = [&](int i, int& c, int& x, int& y) __attribute__((always_inline)) {
+      const int h = (MH == 2 && i >= nblk) ? 1 : 0;
+      const int m0 = (PP ? h : wg) * 64 + wq * 16;
+      c = t.n0 + (i - h * nblk) * 32;
+      x = t.w0 + (m0 & (P.BW - 1));
+      y = t.h0 + (m0 >> P.logBW);
+    };
+    auto res_load = [&](int i) __attribute__((always_inline)) {  // lane 0: block i's residual into its store tile
+      int c, x, y;
+      blk_coord(i, c, x, y);
+      const unsigned q = blk + (unsigned)i;
+      mbar_expect_tx(&res_bar[q % NBUF], Cfg::STG_TILE);
+      tma_load_4d(stg + (q % NBUF) * Cfg::STG_TILE, &map_r.m[t.phase], &res_bar[q % NBUF], c, x, y, t.b);
+    };
+    // Residual fetched ahead, before the main loop: the first NBUF - 1 blocks into the (idle) store tiles, the rest of
+    // the tile's residual into L2.  Block i + NBUF - 1 is loaded once block i is stored.
+    if constexpr (!TF3) {
+      if (has_res && lane == 0) {
+        bulk_wait_read<0>();
+        for (int i = 0; i < NB; ++i) {
+          if (i < NBUF - 1) {
+            res_load(i);
+          } else {
+            int c, x, y;
+            blk_coord(i, c, x, y);
+            tma_prefetch_4d(&map_r.m[t.phase], c, x, y, t.b);
+          }
+        }
+      }
+    }
     float acc[MH][NACC];
     float sum[TF3 ? NACC : 1];  // fp32x3: the tile's K segments summed with round-to-nearest adds
 #pragma unroll
@@ -608,206 +676,209 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_persist_kernel(const __
       }
       asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
     }
-    // one 64-row half of the tile per pass: its accumulators go through this warpgroup's staging rows
-#pragma unroll
-    for (int h = 0; h < MH; ++h) {
-      const int quad = (PP ? h : wg) * 2 + (wq & 1);  // pixel m = quad*32 + lane of the tile
-      const int m = quad * 32 + lane;
+    if constexpr (TF3) {
+      // fp32 in, fp32 out, IEEE arithmetic: one 64-row half of the tile per pass through this warpgroup's staging rows,
+      // then per lane one pixel x 32 channels
+      constexpr int ACC_PITCH = Cfg::ACC_PITCH;
+      float* const acc_stg = s_acc + wg * 64 * ACC_PITCH;
+      const int half = wq >> 1;  // 32-channel chunks alternate by `half`
+      const int m = (wg * 2 + (wq & 1)) * 32 + lane;  // pixel of the tile
       const int hh = t.h0 + (m >> P.logBW), ww = t.w0 + (m & (P.BW - 1));
       const bool pvalid = hh < P.H && ww < P.W;
       const long long opix = ((long long)t.b * P.Hout + (hh * P.os + t.py)) * P.Wout + (ww * P.os + t.px);
-      const bf16* rrow = P.res ? P.res + opix * P.res_pitch + t.n0 : nullptr;
-        // KC: std::integral_constant<int, KIND>.  KIND = the EK_* features this conv has, fixed per launch: feature blocks
-        // outside KIND do not exist in the instantiation (the compiler had turned several of them into predicated code that
-        // was issued for every chunk), EK_GENERIC keeps every run-time check and the fp32 NCHW output.
-        auto process = [&](auto KC, uint32_t* v, const int c0) __attribute__((always_inline)) {
-          constexpr int KIND = decltype(KC)::value;
-          constexpr bool GEN = KIND == EK_GENERIC;
-          if constexpr (TF3) {  // fp32 in, fp32 out: IEEE arithmetic, no fast-math approximations
-            if (affine) {
+      auto process = [&](uint32_t* v, const int c0) __attribute__((always_inline)) {
+        if (affine) {
 #pragma unroll
-              for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(fmaf(__uint_as_float(v[j]), epi[c0 + j], epi[BN + c0 + j]));
-            }
-            if (P.silu) {
+          for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(fmaf(__uint_as_float(v[j]), epi[c0 + j], epi[BN + c0 + j]));
+        }
+        if (P.silu) {
 #pragma unroll
-              for (int j = 0; j < 32; ++j) {
-                const float x = __uint_as_float(v[j]);
-                v[j] = __float_as_uint(x / (1.0f + expf(-x)));
-              }
-            }
-            if (P.out_nchw) {
-              if (pvalid && hh < P.cropH && ww < P.cropW) {
-#pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                  const int n = t.n0 + c0 + j;
-                  if (n < P.Cout) P.out_nchw[(((long long)t.b * P.Cout + n) * P.cropH + hh) * P.cropW + ww] = __uint_as_float(v[j]);
-                }
-              }
-              return;
-            }
-            if (!pvalid) return;
-            float* of = P.out_f32 + opix * P.out_pitch + t.n0 + c0;
-            const float* rf = P.res_f32 ? P.res_f32 + opix * P.res_pitch + t.n0 + c0 : nullptr;
-#pragma unroll
-            for (int g = 0; g < 8; ++g) {
-              if (t.n0 + c0 + g * 4 < P.Cout) {
-                float4 o = make_float4(__uint_as_float(v[g * 4]), __uint_as_float(v[g * 4 + 1]), __uint_as_float(v[g * 4 + 2]),
-                                       __uint_as_float(v[g * 4 + 3]));
-                if (rf) {
-                  const float4 r = *reinterpret_cast<const float4*>(rf + g * 4);
-                  o.x += r.x; o.y += r.y; o.z += r.z; o.w += r.w;
-                }
-                *reinterpret_cast<float4*>(of + g * 4) = o;
-              }
-            }
-            return;
+          for (int j = 0; j < 32; ++j) {
+            const float x = __uint_as_float(v[j]);
+            v[j] = __float_as_uint(x / (1.0f + expf(-x)));
           }
-          if constexpr (GEN || (KIND & EK_QSM)) if ((!GEN || P.qsm) && t.n0 + c0 < 128) {  // one chunk == one attention head of this pixel's q (module_util.py:168,171)
-            float mx = __uint_as_float(v[0]);
-#pragma unroll
-            for (int j = 1; j < 32; ++j) mx = fmaxf(mx, __uint_as_float(v[j]));
-            float sm = 0.f;
+        }
+        if (P.out_nchw) {
+          if (pvalid && hh < P.cropH && ww < P.cropW) {
 #pragma unroll
             for (int j = 0; j < 32; ++j) {
-              const float e = __expf(__uint_as_float(v[j]) - mx);
-              v[j] = __float_as_uint(e);
-              sm += e;
+              const int n = t.n0 + c0 + j;
+              if (n < P.Cout) P.out_nchw[(((long long)t.b * P.Cout + n) * P.cropH + hh) * P.cropW + ww] = __uint_as_float(v[j]);
             }
-            const float inv = __fdividef(0.17677669529663687f, sm);
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(__uint_as_float(v[j]) * inv);
           }
-          if constexpr (GEN || (KIND & EK_AFF)) if (!GEN || affine) {
+          return;
+        }
+        if (!pvalid) return;
+        float* of = P.out_f32 + opix * P.out_pitch + t.n0 + c0;
+        const float* rf = P.res_f32 ? P.res_f32 + opix * P.res_pitch + t.n0 + c0 : nullptr;
 #pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(fmaf(__uint_as_float(v[j]), epi[c0 + j], epi[BN + c0 + j]));
+        for (int g = 0; g < 8; ++g) {
+          if (t.n0 + c0 + g * 4 < P.Cout) {
+            float4 o = make_float4(__uint_as_float(v[g * 4]), __uint_as_float(v[g * 4 + 1]), __uint_as_float(v[g * 4 + 2]),
+                                   __uint_as_float(v[g * 4 + 3]));
+            if (rf) {
+              const float4 r = *reinterpret_cast<const float4*>(rf + g * 4);
+              o.x += r.x; o.y += r.y; o.z += r.z; o.w += r.w;
+            }
+            *reinterpret_cast<float4*>(of + g * 4) = o;
           }
-          if constexpr (GEN || (KIND & EK_SILU)) if (!GEN || P.silu) {
+        }
+      };
+      constexpr int NR = (BN + 63) / 64;
 #pragma unroll
-            for (int j = 0; j < 32; ++j) {
+      for (int i = 0; i < NR; ++i) {
+        asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");  // this warpgroup's previous reads of the staging rows are done
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+          const int j = i * 8 + jj;  // n8 block of the accumulator: registers 4j .. 4j+3
+          if (j * 8 < BN) {
+            const int row = wq * 16 + (lane >> 2), col = jj * 8 + 2 * (lane & 3);
+            *reinterpret_cast<float2*>(acc_stg + row * ACC_PITCH + col) = make_float2(sum[4 * j], sum[4 * j + 1]);
+            *reinterpret_cast<float2*>(acc_stg + (row + 8) * ACC_PITCH + col) = make_float2(sum[4 * j + 2], sum[4 * j + 3]);
+          }
+        }
+        asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
+        const int c0 = i * 64 + half * 32;
+        if (c0 < BN && t.n0 + c0 < P.Cout) {  // chunks entirely past Cout carry no output
+          uint32_t v[32];
+          const float* src = acc_stg + ((wq & 1) * 32 + lane) * ACC_PITCH + half * 32;
+#pragma unroll
+          for (int g = 0; g < 8; ++g) {
+            const float4 f = *reinterpret_cast<const float4*>(src + 4 * g);
+            v[4 * g] = __float_as_uint(f.x); v[4 * g + 1] = __float_as_uint(f.y);
+            v[4 * g + 2] = __float_as_uint(f.z); v[4 * g + 3] = __float_as_uint(f.w);
+          }
+          process(v, c0);
+        }
+      }
+    } else {
+      // bf16: on the accumulator registers.  Thread (wq, lane) holds rows 16 wq + lane / 4 + 8 i (i = 0, 1) of each 64-row
+      // half and, per n8 block j, the channel pair 8 j + 2 (lane % 4) + e: register 4 j + 2 i + e.  Block (h, cb) is the
+      // 16 rows x channels 32 cb .. 32 cb + 31 of half h.  EKT: the EK_* features compiled in (feature blocks outside it
+      // do not exist in the instantiation); EK_GENERIC keeps every run-time check and the fp32 NCHW output.
+      const int cq = 2 * (lane & 3);
+#pragma unroll
+      for (int h = 0; h < MH; ++h) {
+#pragma unroll
+        for (int cb = 0; cb < BN / 32; ++cb) {
+          if (cb >= nblk) continue;  // blocks entirely past Cout carry no output
+          float* const v = &acc[h][cb * 16];
+          const int c0 = cb * 32;
+          const int i = h * nblk + cb;
+          const unsigned q = blk + (unsigned)i;
+          if constexpr (GEN || (EKT & EK_QSM)) if ((!GEN || P.qsm) && t.n0 + c0 < 128) {
+            // one block row == one attention head of a pixel's q (module_util.py:168,171), spread over four lanes; its
+            // sum is taken in channel order 0 .. 31 by each of them
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+              float mx = v[2 * r];
+#pragma unroll
+              for (int jj = 0; jj < 4; ++jj) mx = fmaxf(fmaxf(mx, v[4 * jj + 2 * r]), v[4 * jj + 2 * r + 1]);
+              mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+              mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+#pragma unroll
+              for (int jj = 0; jj < 4; ++jj)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) v[4 * jj + 2 * r + e] = __expf(v[4 * jj + 2 * r + e] - mx);
+              float sm = 0.f;
+#pragma unroll
+              for (int jj = 0; jj < 4; ++jj)
+#pragma unroll
+                for (int l4 = 0; l4 < 4; ++l4)
+#pragma unroll
+                  for (int e = 0; e < 2; ++e) sm += __shfl_sync(0xffffffffu, v[4 * jj + 2 * r + e], (lane & ~3) | l4);
+              const float inv = __fdividef(0.17677669529663687f, sm);
+#pragma unroll
+              for (int jj = 0; jj < 4; ++jj)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) v[4 * jj + 2 * r + e] = v[4 * jj + 2 * r + e] * inv;
+            }
+          }
+          if constexpr (GEN || (EKT & EK_AFF)) if (!GEN || affine) {
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj) {
+              const float2 mu = *reinterpret_cast<const float2*>(epi + c0 + 8 * jj + cq);
+              const float2 ad = *reinterpret_cast<const float2*>(epi + BN + c0 + 8 * jj + cq);
+#pragma unroll
+              for (int r = 0; r < 2; ++r) {
+                v[4 * jj + 2 * r] = fmaf(v[4 * jj + 2 * r], mu.x, ad.x);
+                v[4 * jj + 2 * r + 1] = fmaf(v[4 * jj + 2 * r + 1], mu.y, ad.y);
+              }
+            }
+          }
+          if constexpr (GEN || (EKT & EK_SILU)) if (!GEN || P.silu) {
+#pragma unroll
+            for (int k = 0; k < 16; ++k) {
               // SiLU(x) = x * (0.5 + 0.5 tanh(x/2)): one MUFU op (tanh.approx, rel. error 2^-11 << bf16 rounding) instead of
               // ex2 + rcp; on the narrow layers the epilogue is MUFU-bound (128 x BN outputs per tile, 16 MUFU/clk/SM)
-              const float x = __uint_as_float(v[j]);
+              const float x = v[k];
               float th;
               asm("tanh.approx.f32 %0, %1;" : "=f"(th) : "f"(0.5f * x));
-              v[j] = __float_as_uint(x * fmaf(th, 0.5f, 0.5f));
+              v[k] = x * fmaf(th, 0.5f, 0.5f);
             }
           }
-          if constexpr (GEN) if (P.out_nchw) {
-            if (pvalid && hh < P.cropH && ww < P.cropW) {
+          if constexpr (GEN) if (P.out_nchw) {  // fp32 NCHW, cropped
 #pragma unroll
-              for (int j = 0; j < 32; ++j) {
-                const int n = t.n0 + c0 + j;
-                if (n < P.Cout) P.out_nchw[(((long long)t.b * P.Cout + n) * P.cropH + hh) * P.cropW + ww] = __uint_as_float(v[j]);
+            for (int r = 0; r < 2; ++r) {
+              const int m = (PP ? h : wg) * 64 + wq * 16 + (lane >> 2) + 8 * r;
+              const int hh = t.h0 + (m >> P.logBW), ww = t.w0 + (m & (P.BW - 1));
+              if (hh < P.H && ww < P.W && hh < P.cropH && ww < P.cropW) {
+#pragma unroll
+                for (int jj = 0; jj < 4; ++jj)
+#pragma unroll
+                  for (int e = 0; e < 2; ++e) {
+                    const int n = t.n0 + c0 + 8 * jj + cq + e;
+                    if (n < P.Cout) P.out_nchw[(((long long)t.b * P.Cout + n) * P.cropH + hh) * P.cropW + ww] = v[4 * jj + 2 * r + e];
+                  }
               }
             }
-            return;
+            continue;
           }
-          uint4 ov[4];
+          uint8_t* const tile_s = stg + (q % NBUF) * Cfg::STG_TILE;
+          const uint32_t fa = smem_u32(tile_s) + frag_off;
+          uint32_t rv[8];  // residual, bf16 pairs: [4 r + jj]
+          if constexpr (GEN || (EKT & EK_RES)) if (has_res) {
+            mbar_wait(&res_bar[q % NBUF], (q / NBUF) & 1);
+            ldmatrix_x4(fa, rv);
+            ldmatrix_x4(fa + 512, rv + 4);
 #pragma unroll
-          for (int g = 0; g < 4; ++g) {
-            const int cg = c0 + g * 8;
-            float f[8];
+            for (int jj = 0; jj < 4; ++jj)
 #pragma unroll
-            for (int j = 0; j < 8; ++j) f[j] = __uint_as_float(v[g * 8 + j]);
-            if constexpr (GEN || (KIND & EK_RES)) if (rrow && pvalid && t.n0 + cg < P.Cout) {
-              uint4 r = *reinterpret_cast<const uint4*>(rrow + cg);
-              const __nv_bfloat162* r2 = reinterpret_cast<const __nv_bfloat162*>(&r);
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                f[2 * j] += __low2float(r2[j]);
-                f[2 * j + 1] += __high2float(r2[j]);
+              for (int r = 0; r < 2; ++r) {
+                const __nv_bfloat162 r2 = *reinterpret_cast<const __nv_bfloat162*>(&rv[4 * r + jj]);
+                v[4 * jj + 2 * r] += __low2float(r2);
+                v[4 * jj + 2 * r + 1] += __high2float(r2);
               }
-            }
-            __nv_bfloat162* o2 = reinterpret_cast<__nv_bfloat162*>(&ov[g]);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) o2[j] = __floats2bfloat162_rn(f[2 * j], f[2 * j + 1]);
           }
-          // bf16 NHWC through shared memory + TMA store: each lane owns one pixel row of 32 channels (64 B); the
-          // staging tile uses the 64B swizzle so the 16-byte st.shared are conflict free and the bulk store writes
-          // full, coalesced lines (out-of-range pixels / channels are clipped by TMA).
-          if (lane == 0) bulk_wait_read0();  // the bulk store that last used the tile has finished reading it
-          __syncwarp();
+          uint32_t ov[8];  // [4 r + jj]: matrix jj of rows 8 r .. 8 r + 7
 #pragma unroll
-          for (int g = 0; g < 4; ++g)
-            *reinterpret_cast<uint4*>(stg + lane * 64 + ((g ^ ((lane >> 1) & 3)) << 4)) = ov[g];
+          for (int jj = 0; jj < 4; ++jj)
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+              const __nv_bfloat162 o2 = __floats2bfloat162_rn(v[4 * jj + 2 * r], v[4 * jj + 2 * r + 1]);
+              ov[4 * r + jj] = *reinterpret_cast<const uint32_t*>(&o2);
+            }
+          if (!has_res) {  // with a residual, its load into the tile already waited for the tile's previous store
+            if (lane == 0) bulk_wait_read<NBUF - 1>();  // the store of block q - NBUF has read the tile
+            __syncwarp();
+          }
+          stmatrix_x4(fa, ov);
+          stmatrix_x4(fa + 512, ov + 4);
           fence_proxy_async();
           __syncwarp();
           if (lane == 0) {
-            const int m0 = quad * 32;
-            tma_store_4d(&map_o.m[t.phase], stg, t.n0 + c0, t.w0 + (m0 & (P.BW - 1)), t.h0 + (m0 >> P.logBW), t.b);
+            int c, x, y;
+            blk_coord(i, c, x, y);
+            tma_store_4d(&map_o.m[t.phase], tile_s, c, x, y, t.b);
             bulk_commit();
-          }
-        };
-
-      // registers (wgmma layout) -> fp32 staging rows (one pixel per row) in 64-column rounds -> per-pixel 32-channel chunks
-      auto fin = [&](int r) __attribute__((always_inline)) -> float {
-        if constexpr (TF3) return sum[r];
-        else return acc[h][r];
-      };
-      constexpr int NR = (BN + 63) / 64;
-      if constexpr (!Cfg::COMPACT) {
-#pragma unroll
-        for (int i = 0; i < NR; ++i) {
-          asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");  // this warpgroup's previous reads of the staging rows are done
-#pragma unroll
-          for (int jj = 0; jj < 8; ++jj) {
-            const int j = i * 8 + jj;  // n8 block of the accumulator: registers 4j .. 4j+3
-            if (j * 8 < BN) {
-              const int row = wq * 16 + (lane >> 2), col = jj * 8 + 2 * (lane & 3);
-              *reinterpret_cast<float2*>(acc_stg + row * ACC_PITCH + col) = make_float2(fin(4 * j), fin(4 * j + 1));
-              *reinterpret_cast<float2*>(acc_stg + (row + 8) * ACC_PITCH + col) = make_float2(fin(4 * j + 2), fin(4 * j + 3));
+            if (has_res && i + NBUF - 1 < NB) {
+              bulk_wait_read<1>();  // the store of block q - 1 has read tile (q + NBUF - 1) % NBUF
+              res_load(i + NBUF - 1);
             }
           }
-          asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
-          const int c0 = i * 64 + half * 32;
-          if (c0 < BN && t.n0 + c0 < P.Cout) {  // chunks entirely past Cout carry no output
-            uint32_t v[32];
-            const float* src = acc_stg + ((wq & 1) * 32 + lane) * ACC_PITCH + half * 32;
-#pragma unroll
-            for (int g = 0; g < 8; ++g) {
-              const float4 f = *reinterpret_cast<const float4*>(src + 4 * g);
-              v[4 * g] = __float_as_uint(f.x); v[4 * g + 1] = __float_as_uint(f.y);
-              v[4 * g + 2] = __float_as_uint(f.z); v[4 * g + 3] = __float_as_uint(f.w);
-            }
-            process(std::integral_constant<int, EKT>{}, v, c0);  // EKT: the instantiation's epilogue specialisation
-          }
-        }
-      } else {
-        // COMPACT: a 64-column round is staged in two 32-column passes; pass p carries columns 16p .. 16p+15 of both
-        // 32-channel chunks of the round, so every thread gathers its chunk's 32 values over the two passes.  The bf16
-        // store tiles live in the staging rows: before a round writes them, each warp waits until its previous bulk store
-        // has read its tile, and process() (which writes the tile) starts only after every read of the round.
-#pragma unroll
-        for (int i = 0; i < NR; ++i) {
-          const int c0 = i * 64 + half * 32;  // BN is a multiple of 64 here
-          uint32_t v[32];
-#pragma unroll
-          for (int p = 0; p < 2; ++p) {
-            if (p == 0 && lane == 0) bulk_wait_read0();
-            asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");  // the staging rows are free
-#pragma unroll
-            for (int jj = 0; jj < 8; ++jj) {
-              const int j = i * 8 + jj;  // n8 block of the accumulator: registers 4j .. 4j+3
-              if (((jj >> 1) & 1) == p) {
-                const int row = wq * 16 + (lane >> 2), col = (jj >> 2) * 16 + (jj & 1) * 8 + 2 * (lane & 3);
-                *reinterpret_cast<float2*>(acc_stg + row * ACC_PITCH + col) = make_float2(fin(4 * j), fin(4 * j + 1));
-                *reinterpret_cast<float2*>(acc_stg + (row + 8) * ACC_PITCH + col) = make_float2(fin(4 * j + 2), fin(4 * j + 3));
-              }
-            }
-            asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
-            // read even when the chunk is past Cout: v then stays defined on every path (fewer live registers)
-            const float* src = acc_stg + ((wq & 1) * 32 + lane) * ACC_PITCH + half * 16;
-#pragma unroll
-            for (int g = 0; g < 4; ++g) {
-              const float4 f = *reinterpret_cast<const float4*>(src + 4 * g);
-              v[p * 16 + 4 * g] = __float_as_uint(f.x); v[p * 16 + 4 * g + 1] = __float_as_uint(f.y);
-              v[p * 16 + 4 * g + 2] = __float_as_uint(f.z); v[p * 16 + 4 * g + 3] = __float_as_uint(f.w);
-            }
-          }
-          asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");  // every read of the round is done
-          if (t.n0 + c0 < P.Cout) process(std::integral_constant<int, EKT>{}, v, c0);
         }
       }
+      blk += (unsigned)NB;
     }
     if (P.dbg) c_epi += (unsigned)clock() - t_epi;
   }
@@ -828,7 +899,7 @@ int g_num_sms = 132;
 
 struct TcConvDesc {
   CUtensorMap map_a, map_b;
-  OutMaps map_o;
+  OutMaps map_o, map_r;  // bf16 output and residual views, one map per upsample phase
   TcParams P;
   int BN;
   dim3 grid;
@@ -1026,28 +1097,34 @@ TcConvDesc* tc_conv_create(const bf16* in, int in_pitch, int B, int Hin, int Win
       return nullptr;
     }
   }
-  // output maps for the TMA-store epilogue: [B][H][W][C] view of the destination (channel offset already in
-  // `out`), pixel stride os*pitch; one map per upsample phase (base shifted by (py,px))
+  // maps of the epilogue's store tiles (16 pixel rows of the tile = one box of 32 channels, 64B swizzle): the TMA stores
+  // into the destination and the TMA loads of the residual.  [B][H][W][C] view of the tensor (channel offset already in
+  // the pointer), pixel stride os*pitch; one map per upsample phase (base shifted by (py,px)).
   memset(&d->map_o, 0, sizeof d->map_o);
-  if (!nchw_out) {
-    const int bw = P.BW < 32 ? P.BW : 32, bh = 32 / bw;
+  memset(&d->map_r, 0, sizeof d->map_r);
+  auto tile_maps = [&](OutMaps& maps, const bf16* t, int pitch, CUtensorMapL2promotion l2, const char* what) -> bool {
+    const int bw = P.BW < 16 ? P.BW : 16, bh = 16 / bw;
     for (int ph = 0; ph < nphases; ++ph) {
       const int py = ph >> 1, px = ph & 1;
-      bf16* base = out + ((long long)py * Wout + px) * out_pitch;
+      const bf16* base = t + ((long long)py * Wout + px) * pitch;
       cuuint64_t dims[4] = {(cuuint64_t)Cout, (cuuint64_t)Win, (cuuint64_t)Hin, (cuuint64_t)B};
-      cuuint64_t strides[3] = {(cuuint64_t)P.os * out_pitch * 2, (cuuint64_t)P.os * Wout * out_pitch * 2,
-                               (cuuint64_t)Hout * Wout * out_pitch * 2};
+      cuuint64_t strides[3] = {(cuuint64_t)P.os * pitch * 2, (cuuint64_t)P.os * Wout * pitch * 2, (cuuint64_t)Hout * Wout * pitch * 2};
       cuuint32_t box[4] = {32, (cuuint32_t)bw, (cuuint32_t)bh, 1};
       cuuint32_t es[4] = {1, 1, 1, 1};
-      CUresult r = g_encode(&d->map_o.m[ph], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, (void*)base, dims, strides, box, es,
-                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+      CUresult r = g_encode(&maps.m[ph], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, (void*)base, dims, strides, box, es,
+                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, l2, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
       if (r != CUDA_SUCCESS) {
         delete d;
-        if (err) { char b[96]; snprintf(b, sizeof b, "cuTensorMapEncodeTiled(out) failed: %d", (int)r); *err = b; }
-        return nullptr;
+        if (err) { char b[96]; snprintf(b, sizeof b, "cuTensorMapEncodeTiled(%s) failed: %d", what, (int)r); *err = b; }
+        return false;
       }
     }
+    return true;
+  };
+  if (!nchw_out) {
+    if (!tile_maps(d->map_o, out, out_pitch, CU_TENSOR_MAP_L2_PROMOTION_NONE, "out")) return nullptr;
+    if (ep.res && !tile_maps(d->map_r, (const bf16*)ep.res, ep.res_pitch, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "residual"))
+      return nullptr;
   }
   tc_fill_magic(d);
   return d;
@@ -1137,6 +1214,7 @@ TcConvDesc* tc_conv_create_f32x3(const float* in_split, int B, int Hin, int Win,
     }
   }
   memset(&d->map_o, 0, sizeof d->map_o);
+  memset(&d->map_r, 0, sizeof d->map_r);
   tc_fill_magic(d);
   return d;
 }
@@ -1193,8 +1271,8 @@ int tc_conv_launch(TcConvDesc* d, cudaStream_t st) {
     }
     d->P.dbg = dbg ? dbg_dev : nullptr;
 #define TC_LAUNCH(BNV, PV, EKV)                                                                                            \
-  pdl_launch(conv_tc_persist_kernel<BNV, PV, EKV>, g, TC_THREADS, TcCfgP<BNV, PV>::SMEM_BYTES, st, d->map_a, d->map_b, d->map_o, d->P, \
-             d->tiles_m, d->num_tiles)
+  pdl_launch(conv_tc_persist_kernel<BNV, PV, EKV>, g, TC_THREADS, TcCfgP<BNV, PV>::SMEM_BYTES, st, d->map_a, d->map_b, d->map_o, \
+             d->map_r, d->P, d->tiles_m, d->num_tiles)
     const int ekt = tc_launch_ekt(d);
     if (d->mode == 3) {
       switch (d->BN) {
