@@ -72,7 +72,7 @@ struct Epilogue {
   int ss_off;             // offset of this block's (scale[Cout], shift[Cout]) inside a row
   int ss_img_stride;      // rows per image (0 = shared time, 1 = per-image time)
   // per-output-channel multiplier (NAFBlock beta / gamma) or null: out = (acc + bias) * mult_vec.  Never combined with the
-  // time table (tc_conv_create* and the plan builder refuse it), so the engines need no common order for the two.
+  // time table (tc_conv_create and the plan builder refuse it), so the engines need no common order for the two.
   const float* mult_vec;
   int silu;               // apply SiLU after modulation
   const void* res;        // residual view (same dtype as output) or null
@@ -219,15 +219,16 @@ struct TcTap {
   int plane;    // 5th coordinate of the A tensor map (space-to-depth plane), 0 otherwise
 };
 struct TcConvDesc;  // opaque: tensor maps + tap table + tile config
-TcConvDesc* tc_conv_create(const bf16* in, int in_pitch, int B, int Hin, int Win, int Cin, int planes,
-                           const bf16* wpacked /*[phase][tap][Cout][Cin]*/, int Cout, int ntaps, const TcTap* taps,
-                           int nphases /*1 or 4 (upsample phases)*/, const Epilogue& ep, bf16* out, int out_pitch,
-                           int Hout, int Wout, std::string* err, int flags = 0);
-enum { TC_FLAG_QSOFTMAX = 1, TC_FLAG_W_PER_IMAGE = 2 };
-// fp32x3 mode (3 x tf32 wgmma on hi/lo split fp32 operands, fp32 output); see conv_tc.cu MODE 3
-TcConvDesc* tc_conv_create_f32x3(const float* in_split /*[2][planes][B][H][W][Cin]*/, int B, int Hin, int Win, int Cin, int planes,
-                                 const float* wsplit /*[phase*tap][2][Cout_w][Cin]*/, int Cout, int ntaps, const TcTap* taps,
-                                 int nphases, const Epilogue& ep, float* out, int out_pitch, int Hout, int Wout, std::string* err);
+// S = bf16, or float for fp32x3 (3 x tf32 wgmma on hi/lo split fp32 operands, fp32 output; see conv_tc.cu MODE 3).
+// in: [planes][B][Hin][Win] pixels of in_pitch elements; fp32x3: the launch_split_tf32 output [2][planes][B][H][W][Cin]
+// (in_pitch = Cin); the 7x7 stem (bf16, planes < 0): its padded [B][Hin+6][Win+8][8] layout (in_pitch = 8; the creator
+// takes Cin = 64, whatever is passed).  w: [phase][tap][Cout_w][Cin] (bf16 per-image weights: [B][Cout_w][Cin]); fp32x3: [phase*tap][2][Cout_w][Cin].
+// nphases: 1 or 4 (upsample phases).  out == nullptr: fp32 NCHW output, set at launch (tc_conv_set_out_nchw).
+template <typename S>
+TcConvDesc* tc_conv_create(const S* in, int in_pitch, int B, int Hin, int Win, int Cin, int planes, const S* w, int Cout, int ntaps,
+                           const TcTap* taps, int nphases, const Epilogue& ep, S* out, int out_pitch, int Hout, int Wout,
+                           std::string* err, int flags = 0);
+enum { TC_FLAG_QSOFTMAX = 1, TC_FLAG_W_PER_IMAGE = 2 };  // bf16 only
 // hi = rn_tf32(x), lo = rn_tf32(x - hi) of a pitched NHWC fp32 view -> dense out[0][npix][C] (hi), out[1][npix][C] (lo)
 void launch_split_tf32(const float* in, int in_pitch, float* out, long long npix, int C, cudaStream_t st);
 void tc_conv_destroy(TcConvDesc*);

@@ -28,6 +28,7 @@
 #include <stdio.h>
 #include <stdlib.h>
 
+#include <memory>
 #include <type_traits>
 
 #include "common.cuh"
@@ -61,7 +62,7 @@ struct TcParams {
   // tile decode without integer divisions (they cost ~25 instructions + a MUFU.RCP each, five per tile and warp: on layers
   // with one k-iteration per tile the kernel is ISSUE-bound on them): q = umulhi(x, mg) with mg = ceil(2^32 / d)
   unsigned mg_tiles_m, mg_tiles_n, mg_tilesW, mg_tilesH, mg_B;  // 0: divisor is 1 (or fast path not provable): see fdiv
-  int epi_kind;         // EK_* combination the epilogue is specialised for (EK_GENERIC: every feature checked at run time)
+  int epi_kind;         // host-only (no kernel reads it): the EKT of the instantiation tc_conv_launch runs, set there
   int n_fast;           // tile order: N tiles of one M tile are consecutive (1x1 convs with several N tiles, see tc_conv_create)
   int tiles_n;
   int rows_a_bytes;     // ROWS mode: bytes of one A box ((BH+2) x BW x 128)
@@ -907,9 +908,44 @@ struct TcConvDesc {
   int mode;  // 0 per-tap boxes, 2 ROWS (row-window reuse), 3 fp32x3
 };
 
+// One row per compiled conv_tc_persist_kernel instantiation: tc_init sets each row's shared memory, tc_pick chooses the row
+// a descriptor runs.  An instantiation is added or removed here and nowhere else; tests/test_conv_tc_sass.py checks that
+// tests/test_gpu_conv_epilogues.py has a case for each.
+struct TcKernel {
+  int BN, mode, ekt;
+  void (*fn)(CUtensorMap, CUtensorMap, OutMaps, OutMaps, TcParams, int, int);
+  int smem;
+};
 template <int BN, int MODE, int EKT = EK_GENERIC>
-static void tc_set_smem() {
-  cudaFuncSetAttribute(conv_tc_persist_kernel<BN, MODE, EKT>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfgP<BN, MODE>::SMEM_BYTES);
+static TcKernel tc_kernel() {
+  return TcKernel{BN, MODE, EKT, conv_tc_persist_kernel<BN, MODE, EKT>, TcCfgP<BN, MODE>::SMEM_BYTES};
+}
+static const TcKernel TC_KERNELS[] = {
+    tc_kernel<32, 0>(),
+    tc_kernel<64, 0>(),  tc_kernel<64, 0, 0>(),  tc_kernel<64, 0, EK_AFF>(),
+    tc_kernel<128, 0>(), tc_kernel<128, 0, 0>(), tc_kernel<128, 0, EK_AFF>(), tc_kernel<128, 0, EK_QSM>(),
+    tc_kernel<256, 0>(), tc_kernel<256, 0, 0>(), tc_kernel<256, 0, EK_AFF>(),  // deep res_conv; downsample / to_out (bias)
+    tc_kernel<32, 2>(),
+    tc_kernel<64, 2>(),  tc_kernel<64, 2, EK_AFF | EK_SILU>(),  tc_kernel<64, 2, EK_SILU | EK_RES>(),
+    tc_kernel<128, 2>(), tc_kernel<128, 2, EK_AFF | EK_SILU>(), tc_kernel<128, 2, EK_SILU | EK_RES>(),
+    tc_kernel<32, 3>(),  tc_kernel<64, 3>(),  tc_kernel<128, 3>(),
+};
+
+// The row that runs d now: the one compiled for exactly the epilogue features d uses, else the EK_GENERIC row of its
+// (BN, mode).  fp32x3 and the fp32 NCHW output always run EK_GENERIC.  The time-modulation table (EK_AFF) usually arrives
+// after create, through tc_conv_set_runtime, so this is decided at launch; tc_conv_query asks the same function.
+static const TcKernel* tc_pick(const TcConvDesc* d) {
+  const TcParams& P = d->P;
+  int ek = EK_GENERIC;
+  if (d->mode != 3 && P.out)
+    ek = (P.qsm ? EK_QSM : 0) | (P.ss || P.bias || P.mult_vec ? EK_AFF : 0) | (P.silu ? EK_SILU : 0) | (P.res ? EK_RES : 0);
+  const TcKernel* generic = nullptr;
+  for (const TcKernel& k : TC_KERNELS) {
+    if (k.BN != d->BN || k.mode != d->mode) continue;
+    if (k.ekt == ek) return &k;
+    if (k.ekt == EK_GENERIC) generic = &k;
+  }
+  return generic;
 }
 
 bool tc_init(std::string* err) {
@@ -922,27 +958,7 @@ bool tc_init(std::string* err) {
     return false;
   }
   g_encode = (EncodeTiledFn)fn;
-  tc_set_smem<32, 0>();
-  tc_set_smem<32, 2>();
-  tc_set_smem<64, 0>();
-  tc_set_smem<64, 2>();
-  tc_set_smem<128, 0>();
-  tc_set_smem<128, 2>();
-  tc_set_smem<256, 0>();
-  tc_set_smem<64, 2, EK_AFF | EK_SILU>();
-  tc_set_smem<64, 2, EK_SILU | EK_RES>();
-  tc_set_smem<128, 2, EK_AFF | EK_SILU>();
-  tc_set_smem<128, 2, EK_SILU | EK_RES>();
-  tc_set_smem<64, 0, 0>();
-  tc_set_smem<64, 0, EK_AFF>();
-  tc_set_smem<128, 0, 0>();
-  tc_set_smem<128, 0, EK_AFF>();
-  tc_set_smem<128, 0, EK_QSM>();
-  tc_set_smem<256, 0, EK_AFF>();
-  tc_set_smem<256, 0, 0>();
-  tc_set_smem<32, 3>();
-  tc_set_smem<64, 3>();
-  tc_set_smem<128, 3>();
+  for (const TcKernel& k : TC_KERNELS) cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, k.smem);
   {
     int dev = 0, n = 0;
     cudaGetDevice(&dev);
@@ -959,7 +975,7 @@ bool tc_init(std::string* err) {
   return true;
 }
 
-// tile-decode multipliers and the epilogue specialisation of a finished descriptor (called at the end of both creators)
+// tile-decode multipliers of a finished descriptor
 static void tc_fill_magic(TcConvDesc* d) {
   TcParams& P = d->P;
   const unsigned long long max_x = (unsigned long long)d->num_tiles + 2;
@@ -973,55 +989,76 @@ static void tc_fill_magic(TcConvDesc* d) {
   P.mg_tilesW = mg(P.tilesW);
   P.mg_tilesH = mg(P.tilesH);
   P.mg_B = mg(P.B);
-  int k = 0;
-  if (P.qsm) k |= EK_QSM;
-  if (P.ss || P.bias || P.mult_vec) k |= EK_AFF;
-  if (P.silu) k |= EK_SILU;
-  if (P.res) k |= EK_RES;
-  const bool known = k == 0 || k == EK_QSM || k == EK_AFF || k == EK_SILU || k == (EK_AFF | EK_SILU) || k == (EK_AFF | EK_RES) ||
-                     k == (EK_SILU | EK_RES);
-  P.epi_kind = (d->mode != 3 && P.out && known) ? k : EK_GENERIC;
 }
 
-TcConvDesc* tc_conv_create(const bf16* in, int in_pitch, int B, int Hin, int Win, int Cin, int planes,
-                           const bf16* wpacked, int Cout, int ntaps, const TcTap* taps, int nphases, const Epilogue& ep,
-                           bf16* out, int out_pitch, int Hout, int Wout, std::string* err, int flags) {
+// cuTensorMapEncodeTiled with unit element strides, no interleave and zero out-of-bounds fill; on failure *err names `what`
+static bool tc_encode(CUtensorMap* map, CUtensorMapDataType type, cuuint32_t rank, const void* base, const cuuint64_t* dims,
+                      const cuuint64_t* strides, const cuuint32_t* box, CUtensorMapSwizzle swizzle, CUtensorMapL2promotion l2,
+                      const char* what, std::string* err) {
+  const cuuint32_t es[5] = {1, 1, 1, 1, 1};
+  const CUresult r = g_encode(map, type, rank, (void*)base, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, l2,
+                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r == CUDA_SUCCESS) return true;
+  if (err) { char b[96]; snprintf(b, sizeof b, "cuTensorMapEncodeTiled(%s) failed: %d", what, (int)r); *err = b; }
+  return false;
+}
+
+// Both storage types share every step; what depends on the element size follows from S (a K chunk is one 128-byte swizzled
+// row: 64 bf16 or 32 fp32 channels; 16 bytes are 8 or 4 elements), and what only bf16 has is marked so.
+template <typename S>
+TcConvDesc* tc_conv_create(const S* in, int in_pitch, int B, int Hin, int Win, int Cin, int planes, const S* w, int Cout, int ntaps,
+                           const TcTap* taps, int nphases, const Epilogue& ep, S* out, int out_pitch, int Hout, int Wout,
+                           std::string* err, int flags) {
+  constexpr bool f32 = std::is_same<S, float>::value;
+  constexpr int es = sizeof(S), al = 16 / es, kc = 128 / es;  // element bytes, elements per 16 bytes, channels per K chunk
+  constexpr CUtensorMapDataType dtype = f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
   auto bad = [&](const char* m) -> TcConvDesc* {
     if (err) *err = m;
     return nullptr;
   };
   if (!g_encode) return bad("tc_init not called");
   if (ntaps < 1 || ntaps > 16) return bad("ntaps out of range");
+  if (f32 && planes < 1) return bad("planes must be >= 1");  // the 7x7 stem is bf16 only
+  if (f32 && flags) return bad("the q-softmax and per-image weights are bf16 only");
+  if ((flags & TC_FLAG_W_PER_IMAGE) && (ntaps != 1 || nphases != 1)) return bad("per-image weights need a 1x1 conv");
+  // 7x7 stem "row trick" (planes < 0): the input is a zero-bordered [B][H+6][W+8][8ch] buffer; one GEMM K-chunk of 64
+  // elements = 8 consecutive pixels x 8 channels of one input row (overlapping pixel stride of 16 B), so kernel row r is a
+  // single tap (dh=r) and K = 7 x 64.
+  if (planes < 0) Cin = 64;
   const bool nchw_out = (out == nullptr);  // caller sets the fp32 NCHW pointer at launch (tc_conv_set_out_nchw)
   const int Cout_w = (Cout + 7) / 8 * 8;   // rows of the packed weight tensor (zero padded)
-  if (Cin % 8 || in_pitch % 8) return bad("input channel count / pitch must be multiples of 8");
-  if (!nchw_out && (Cout % 8 || out_pitch % 8)) return bad("output channel count / pitch must be multiples of 8");
-  if (((uintptr_t)in & 15) || ((uintptr_t)wpacked & 15) || ((uintptr_t)out & 15)) return bad("operands must be 16-byte aligned");
-  if (ep.res && (((uintptr_t)ep.res & 15) || ep.res_pitch % 8)) return bad("residual must be 16-byte aligned");
+  if (Cin % al || in_pitch % al) return bad("input channel count / pitch must be multiples of 16 bytes");
+  if (!nchw_out && (Cout % al || out_pitch % al)) return bad("output channel count / pitch must be multiples of 16 bytes");
+  if (((uintptr_t)in & 15) || ((uintptr_t)w & 15) || ((uintptr_t)out & 15)) return bad("operands must be 16-byte aligned");
+  if (ep.res && (((uintptr_t)ep.res & 15) || ep.res_pitch % al)) return bad("residual must be 16-byte aligned");
   if (ep.ss && ep.mult_vec) return bad("the time-modulation table and mult_vec cannot be combined");
-  TcConvDesc* d = new TcConvDesc();
+  std::unique_ptr<TcConvDesc> d(new TcConvDesc());  // value-initialised: every parameter and map starts zero
   TcParams& P = d->P;
-  memset(&P, 0, sizeof P);
   P.B = B; P.H = Hin; P.W = Win; P.Cin = Cin; P.Cout = Cout;
-  P.ntaps = ntaps; P.kchunks = (Cin + 63) / 64;
+  P.ntaps = ntaps; P.kchunks = (Cin + kc - 1) / kc;
   P.nphases = nphases;
   P.Hout = Hout; P.Wout = Wout; P.os = nphases == 4 ? 2 : 1;
-  P.out = out; P.out_pitch = out_pitch;
-  P.res = (const bf16*)ep.res; P.res_pitch = ep.res_pitch;
+  P.out_pitch = out_pitch; P.res_pitch = ep.res_pitch;
+  if constexpr (f32) {
+    P.out_f32 = out; P.res_f32 = (const float*)ep.res;
+    P.lo_plane_off = planes;
+  } else {
+    P.out = out; P.res = (const bf16*)ep.res;
+  }
   P.bias = ep.bias; P.mult_vec = ep.mult_vec; P.ss = ep.ss; P.t_ptr = ep.t_ptr; P.ss_S = ep.ss_S; P.ss_off = ep.ss_off;
   P.ss_img_stride = ep.ss_img_stride; P.silu = ep.silu;
   for (int i = 0; i < ntaps; ++i) P.taps[i] = taps[i];
   P.qsm = (flags & TC_FLAG_QSOFTMAX) ? 1 : 0;
   P.w_per_image = (flags & TC_FLAG_W_PER_IMAGE) ? 1 : 0;
-  if (P.w_per_image && (ntaps != 1 || nphases != 1)) return bad("per-image weights need a 1x1 conv");
-  int BN = Cout >= 256 ? 256 : (Cout > 64 ? 128 : (Cout > 32 ? 64 : 32));
-  if (BN == 256 && Cout % 256 != 0 && Cout % 128 == 0) BN = 128;  // e.g. to_qkv (384): no half-empty N tile
-  bool rows = false;
-  if (nphases == 1 && planes == 1 && ntaps == 9 && BN <= 128) {
+  int BN = Cout > 64 ? 128 : (Cout > 32 ? 64 : 32);
+  // bf16 only: BN = 256, except where Cout is a multiple of 128 but not of 256 (to_qkv, 384: no half-empty N tile)
+  if (!f32 && Cout >= 256 && !(Cout % 256 != 0 && Cout % 128 == 0)) BN = 256;
+  bool rows = false;  // bf16 only
+  if (!f32 && nphases == 1 && planes == 1 && ntaps == 9 && BN <= 128) {
     rows = true;
     for (int i = 0; rows && i < 9; ++i) rows = taps[i].dh == i / 3 - 1 && taps[i].dw == i % 3 - 1 && taps[i].plane == 0;
   }
-  d->mode = rows ? 2 : 0;
+  d->mode = f32 ? 3 : rows ? 2 : 0;
   // tile shape: BW x BH = 128 pixels, minimise padded work
   long long best = -1;
   for (int bw = 128; bw >= 8; bw >>= 1) {
@@ -1039,10 +1076,11 @@ TcConvDesc* tc_conv_create(const bf16* in, int in_pitch, int B, int Hin, int Win
   P.tilesH = (Hin + P.BH - 1) / P.BH;
   // Small problems (NAFNet's 16x16 levels, sharded deep UNet levels): fewer tiles than half the SMs means a handful
   // of CTAs stream all the weights; narrower N tiles spread that over more SMs.  Tap mode 0 accumulates in the same
-  // K order for every BN, so results do not depend on this choice (and hence not on the batch size).
-  if (!rows && !P.qsm && !nchw_out) {
-    const int tm = P.tilesW * P.tilesH * B * nphases;
-    while (BN > 64 && Cout % (BN / 2) == 0 && (long long)tm * ((Cout + BN - 1) / BN) < g_num_sms / 2) BN >>= 1;
+  // K order for every BN, so results do not depend on this choice (and hence not on the batch size).  bf16 keeps BN for
+  // ROWS, the q-softmax and the NCHW output, and goes no lower than 64; fp32x3 always halves, down to 32.
+  if (f32 || (!rows && !P.qsm && !nchw_out)) {
+    const int tm = P.tilesW * P.tilesH * B * nphases, bn_min = f32 ? 32 : 64;
+    while (BN > bn_min && Cout % (BN / 2) == 0 && (long long)tm * ((Cout + BN - 1) / BN) < g_num_sms / 2) BN >>= 1;
   }
   d->BN = BN;
   d->grid = dim3((unsigned)(P.tilesW * P.tilesH * B * nphases), (unsigned)((Cout + BN - 1) / BN));
@@ -1054,170 +1092,65 @@ TcConvDesc* tc_conv_create(const bf16* in, int in_pitch, int B, int Hin, int Win
   // than L2, and M-fastest re-read it from DRAM once per N tile (about 3x the input's bytes for to_qkv).  N fastest
   // makes the N tiles of one pixel tile run back to back in the same wave, so the second and third read hit L2.
   P.tiles_n = (Cout + BN - 1) / BN;
-  // (only where the input is too large to stay in L2 anyway; small inputs keep M-fastest and its once-per-N-tile epilogue table)
-  const long long a_bytes = (long long)B * Hin * Win * in_pitch * 2;
-  P.n_fast = (ntaps == 1 && P.tiles_n > 1 && !P.w_per_image && a_bytes > (24ll << 20)) ? 1 : 0;
-  // A: [planes][B][H][W][C] (C contiguous, pixel pitch in_pitch)
+  // (bf16 only, and only where the input is too large to stay in L2 anyway; small inputs keep M-fastest and its
+  // once-per-N-tile epilogue table)
+  const long long a_bytes = (long long)B * Hin * Win * in_pitch * es;
+  P.n_fast = (!f32 && ntaps == 1 && P.tiles_n > 1 && !P.w_per_image && a_bytes > (24ll << 20)) ? 1 : 0;
+  // A: [planes][B][H][W][C] (C contiguous, pixel pitch in_pitch); fp32x3: 2 x planes dense planes, hi then lo
   {
-    cuuint64_t dims[5] = {(cuuint64_t)Cin, (cuuint64_t)Win, (cuuint64_t)Hin, (cuuint64_t)B, (cuuint64_t)planes};
-    cuuint64_t strides[4] = {(cuuint64_t)in_pitch * 2, (cuuint64_t)Win * in_pitch * 2, (cuuint64_t)Hin * Win * in_pitch * 2,
-                             (cuuint64_t)B * Hin * Win * in_pitch * 2};
-    if (planes < 0) {
-      // 7x7 stem "row trick": the input is a zero-bordered [B][H+6][W+8][8ch] buffer; one GEMM K-chunk of
-      // 64 elements = 8 consecutive pixels x 8 channels of one input row (overlapping pixel stride of 16 B),
-      // so kernel row r is a single tap (dh=r) and K = 7 x 64.
-      dims[0] = 64; dims[1] = (cuuint64_t)Win; dims[2] = (cuuint64_t)(Hin + 6); dims[3] = (cuuint64_t)B; dims[4] = 1;
+    cuuint64_t dims[5] = {(cuuint64_t)Cin, (cuuint64_t)Win, (cuuint64_t)Hin, (cuuint64_t)B, (cuuint64_t)(f32 ? 2 * planes : planes)};
+    cuuint64_t strides[4] = {(cuuint64_t)in_pitch * es, (cuuint64_t)Win * in_pitch * es, (cuuint64_t)Hin * Win * in_pitch * es,
+                             (cuuint64_t)B * Hin * Win * in_pitch * es};
+    if (planes < 0) {  // the stem's overlapping 8-pixel rows (see above)
+      dims[2] = (cuuint64_t)(Hin + 6); dims[4] = 1;
       strides[0] = 16; strides[1] = (cuuint64_t)(Win + 8) * 16; strides[2] = (cuuint64_t)(Hin + 6) * (Win + 8) * 16;
       strides[3] = strides[2] * B;
     }
-    cuuint32_t box[5] = {64, (cuuint32_t)P.BW, (cuuint32_t)P.BH, 1, 1};
-    if (rows) { box[2] = (cuuint32_t)(P.BH + 2); }
-    cuuint32_t es[5] = {1, 1, 1, 1, 1};
-    CUresult r = g_encode(&d->map_a, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, (void*)in, dims, strides, box, es,
-                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-      delete d;
-      if (err) { char b[96]; snprintf(b, sizeof b, "cuTensorMapEncodeTiled(A) failed: %d", (int)r); *err = b; }
+    const cuuint32_t box[5] = {(cuuint32_t)kc, (cuuint32_t)P.BW, (cuuint32_t)(rows ? P.BH + 2 : P.BH), 1, 1};
+    if (!tc_encode(&d->map_a, dtype, 5, in, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   "A", err))
       return nullptr;
-    }
   }
-  // B: [phase*ntaps][Cout][Cin]
+  // B: [phase*ntaps][Cout_w][Cin]; bf16 per-image weights: [B][Cout_w][Cin]; fp32x3: [phase*ntaps][2 (hi, lo)][Cout_w][Cin]
   {
-    cuuint64_t dims[3] = {(cuuint64_t)Cin, (cuuint64_t)Cout_w, (cuuint64_t)(P.w_per_image ? B : nphases * ntaps)};
-    cuuint64_t strides[2] = {(cuuint64_t)Cin * 2, (cuuint64_t)Cout_w * Cin * 2};
-    cuuint32_t box[3] = {64, (cuuint32_t)BN, 1};
-    cuuint32_t es[3] = {1, 1, 1};
-    CUresult r = g_encode(&d->map_b, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, (void*)wpacked, dims, strides, box, es,
-                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-      delete d;
-      if (err) { char b[96]; snprintf(b, sizeof b, "cuTensorMapEncodeTiled(B) failed: %d", (int)r); *err = b; }
+    const cuuint64_t dims[3] = {(cuuint64_t)Cin, (cuuint64_t)Cout_w,
+                                (cuuint64_t)(P.w_per_image ? B : nphases * ntaps * (f32 ? 2 : 1))};
+    const cuuint64_t strides[2] = {(cuuint64_t)Cin * es, (cuuint64_t)Cout_w * Cin * es};
+    const cuuint32_t box[3] = {(cuuint32_t)kc, (cuuint32_t)BN, 1};
+    if (!tc_encode(&d->map_b, dtype, 3, w, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   "B", err))
       return nullptr;
-    }
   }
-  // maps of the epilogue's store tiles (16 pixel rows of the tile = one box of 32 channels, 64B swizzle): the TMA stores
-  // into the destination and the TMA loads of the residual.  [B][H][W][C] view of the tensor (channel offset already in
-  // the pointer), pixel stride os*pitch; one map per upsample phase (base shifted by (py,px)).
-  memset(&d->map_o, 0, sizeof d->map_o);
-  memset(&d->map_r, 0, sizeof d->map_r);
-  auto tile_maps = [&](OutMaps& maps, const bf16* t, int pitch, CUtensorMapL2promotion l2, const char* what) -> bool {
+  // bf16 only: maps of the epilogue's store tiles (16 pixel rows of the tile = one box of 32 channels, 64B swizzle): the
+  // TMA stores into the destination and the TMA loads of the residual.  [B][H][W][C] view of the tensor (channel offset
+  // already in the pointer), pixel stride os*pitch; one map per upsample phase (base shifted by (py,px)).
+  auto tile_maps = [&](OutMaps& maps, const S* t, int pitch, CUtensorMapL2promotion l2, const char* what) -> bool {
     const int bw = P.BW < 16 ? P.BW : 16, bh = 16 / bw;
     for (int ph = 0; ph < nphases; ++ph) {
       const int py = ph >> 1, px = ph & 1;
-      const bf16* base = t + ((long long)py * Wout + px) * pitch;
-      cuuint64_t dims[4] = {(cuuint64_t)Cout, (cuuint64_t)Win, (cuuint64_t)Hin, (cuuint64_t)B};
-      cuuint64_t strides[3] = {(cuuint64_t)P.os * pitch * 2, (cuuint64_t)P.os * Wout * pitch * 2, (cuuint64_t)Hout * Wout * pitch * 2};
-      cuuint32_t box[4] = {32, (cuuint32_t)bw, (cuuint32_t)bh, 1};
-      cuuint32_t es[4] = {1, 1, 1, 1};
-      CUresult r = g_encode(&maps.m[ph], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, (void*)base, dims, strides, box, es,
-                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, l2, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      if (r != CUDA_SUCCESS) {
-        delete d;
-        if (err) { char b[96]; snprintf(b, sizeof b, "cuTensorMapEncodeTiled(%s) failed: %d", what, (int)r); *err = b; }
+      const cuuint64_t dims[4] = {(cuuint64_t)Cout, (cuuint64_t)Win, (cuuint64_t)Hin, (cuuint64_t)B};
+      const cuuint64_t strides[3] = {(cuuint64_t)P.os * pitch * es, (cuuint64_t)P.os * Wout * pitch * es,
+                                     (cuuint64_t)Hout * Wout * pitch * es};
+      const cuuint32_t box[4] = {32, (cuuint32_t)bw, (cuuint32_t)bh, 1};
+      if (!tc_encode(&maps.m[ph], dtype, 4, t + ((long long)py * Wout + px) * pitch, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_64B,
+                     l2, what, err))
         return false;
-      }
     }
     return true;
   };
-  if (!nchw_out) {
+  if (!f32 && !nchw_out) {
     if (!tile_maps(d->map_o, out, out_pitch, CU_TENSOR_MAP_L2_PROMOTION_NONE, "out")) return nullptr;
-    if (ep.res && !tile_maps(d->map_r, (const bf16*)ep.res, ep.res_pitch, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "residual"))
+    if (ep.res && !tile_maps(d->map_r, (const S*)ep.res, ep.res_pitch, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "residual"))
       return nullptr;
   }
-  tc_fill_magic(d);
-  return d;
+  tc_fill_magic(d.get());
+  if (!tc_pick(d.get())) return bad("no conv_tc_persist_kernel instantiation for this BN and mode");
+  return d.release();
 }
-
-// fp32x3 mode: `in_split` is the conv input split by launch_split_tf32: [2 (hi, lo)][planes][B][Hin][Win][Cin] fp32 (dense,
-// pixel pitch Cin); `wsplit` is [phase*ntaps][2 (hi, lo)][Cout_w][Cin] fp32 (pack_tc_*_kernel<float>); fp32 NHWC output view.
-TcConvDesc* tc_conv_create_f32x3(const float* in_split, int B, int Hin, int Win, int Cin, int planes, const float* wsplit, int Cout,
-                                 int ntaps, const TcTap* taps, int nphases, const Epilogue& ep, float* out, int out_pitch, int Hout,
-                                 int Wout, std::string* err) {
-  auto bad = [&](const char* m) -> TcConvDesc* {
-    if (err) *err = m;
-    return nullptr;
-  };
-  if (!g_encode) return bad("tc_init not called");
-  if (ntaps < 1 || ntaps > 16) return bad("ntaps out of range");
-  if (planes < 1) return bad("fp32x3: planes must be >= 1");
-  const bool nchw_out = (out == nullptr);
-  const int Cout_w = (Cout + 7) / 8 * 8;
-  if (Cin % 4) return bad("fp32x3: input channels must be a multiple of 4");
-  if (!nchw_out && (Cout % 4 || out_pitch % 4)) return bad("fp32x3: output channels / pitch must be multiples of 4");
-  if (((uintptr_t)in_split & 15) || ((uintptr_t)wsplit & 15) || ((uintptr_t)out & 15)) return bad("operands must be 16-byte aligned");
-  if (ep.res && (((uintptr_t)ep.res & 15) || ep.res_pitch % 4)) return bad("residual must be 16-byte aligned");
-  if (ep.ss && ep.mult_vec) return bad("the time-modulation table and mult_vec cannot be combined");
-  TcConvDesc* d = new TcConvDesc();
-  TcParams& P = d->P;
-  memset(&P, 0, sizeof P);
-  P.B = B; P.H = Hin; P.W = Win; P.Cin = Cin; P.Cout = Cout;
-  P.ntaps = ntaps; P.kchunks = (Cin + 31) / 32;
-  P.nphases = nphases;
-  P.Hout = Hout; P.Wout = Wout; P.os = nphases == 4 ? 2 : 1;
-  P.out = nullptr; P.out_f32 = out; P.out_pitch = out_pitch;
-  P.res = nullptr; P.res_f32 = (const float*)ep.res; P.res_pitch = ep.res_pitch;
-  P.bias = ep.bias; P.mult_vec = ep.mult_vec; P.ss = ep.ss; P.t_ptr = ep.t_ptr; P.ss_S = ep.ss_S; P.ss_off = ep.ss_off;
-  P.ss_img_stride = ep.ss_img_stride; P.silu = ep.silu;
-  P.lo_plane_off = planes;
-  for (int i = 0; i < ntaps; ++i) P.taps[i] = taps[i];
-  int BN = Cout > 64 ? 128 : (Cout > 32 ? 64 : 32);
-  d->mode = 3;
-  long long best = -1;
-  for (int bw = 128; bw >= 8; bw >>= 1) {
-    int bh = 128 / bw;
-    long long cost = (long long)((Win + bw - 1) / bw) * bw * ((Hin + bh - 1) / bh) * bh;
-    if (best < 0 || cost < best) { best = cost; P.BW = bw; P.BH = bh; }
-  }
-  P.logBW = 0;
-  while ((1 << P.logBW) < P.BW) P.logBW++;
-  P.tilesW = (Win + P.BW - 1) / P.BW;
-  P.tilesH = (Hin + P.BH - 1) / P.BH;
-  {
-    const int tm = P.tilesW * P.tilesH * B * nphases;
-    while (BN > 32 && Cout % (BN / 2) == 0 && (long long)tm * ((Cout + BN - 1) / BN) < g_num_sms / 2) BN >>= 1;
-  }
-  d->BN = BN;
-  d->grid = dim3((unsigned)(P.tilesW * P.tilesH * B * nphases), (unsigned)((Cout + BN - 1) / BN));
-  d->tiles_m = P.tilesW * P.tilesH * B * nphases;
-  d->num_tiles = d->tiles_m * ((Cout + BN - 1) / BN);
-  P.tiles_n = (Cout + BN - 1) / BN;
-  P.n_fast = 0;
-  {
-    cuuint64_t dims[5] = {(cuuint64_t)Cin, (cuuint64_t)Win, (cuuint64_t)Hin, (cuuint64_t)B, (cuuint64_t)(2 * planes)};
-    cuuint64_t strides[4] = {(cuuint64_t)Cin * 4, (cuuint64_t)Win * Cin * 4, (cuuint64_t)Hin * Win * Cin * 4,
-                             (cuuint64_t)B * Hin * Win * Cin * 4};
-    cuuint32_t box[5] = {32, (cuuint32_t)P.BW, (cuuint32_t)P.BH, 1, 1};
-    cuuint32_t es[5] = {1, 1, 1, 1, 1};
-    CUresult r = g_encode(&d->map_a, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 5, (void*)in_split, dims, strides, box, es,
-                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-      delete d;
-      if (err) { char b[96]; snprintf(b, sizeof b, "cuTensorMapEncodeTiled(A fp32) failed: %d", (int)r); *err = b; }
-      return nullptr;
-    }
-  }
-  {
-    cuuint64_t dims[3] = {(cuuint64_t)Cin, (cuuint64_t)Cout_w, (cuuint64_t)(nphases * ntaps * 2)};
-    cuuint64_t strides[2] = {(cuuint64_t)Cin * 4, (cuuint64_t)Cout_w * Cin * 4};
-    cuuint32_t box[3] = {32, (cuuint32_t)BN, 1};
-    cuuint32_t es[3] = {1, 1, 1};
-    CUresult r = g_encode(&d->map_b, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, (void*)wsplit, dims, strides, box, es,
-                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-      delete d;
-      if (err) { char b[96]; snprintf(b, sizeof b, "cuTensorMapEncodeTiled(B fp32) failed: %d", (int)r); *err = b; }
-      return nullptr;
-    }
-  }
-  memset(&d->map_o, 0, sizeof d->map_o);
-  memset(&d->map_r, 0, sizeof d->map_r);
-  tc_fill_magic(d);
-  return d;
-}
+template TcConvDesc* tc_conv_create(const bf16*, int, int, int, int, int, int, const bf16*, int, int, const TcTap*, int,
+                                    const Epilogue&, bf16*, int, int, int, std::string*, int);
+template TcConvDesc* tc_conv_create(const float*, int, int, int, int, int, int, const float*, int, int, const TcTap*, int,
+                                    const Epilogue&, float*, int, int, int, std::string*, int);
 
 void tc_conv_destroy(TcConvDesc* d) { delete d; }
 
@@ -1231,107 +1164,44 @@ void tc_conv_set_runtime(TcConvDesc* d, const float* ss, const int* t_ptr, int s
   d->P.ss = ss;
   d->P.t_ptr = t_ptr;
   d->P.ss_img_stride = ss_img_stride;
-  if (ss && d->P.epi_kind != EK_GENERIC && !(d->P.epi_kind & EK_AFF)) {  // the time-modulation table arrives at launch time
-    const int k = d->P.epi_kind | EK_AFF;
-    d->P.epi_kind = (k == EK_AFF || k == (EK_AFF | EK_SILU) || k == (EK_AFF | EK_RES)) ? k : EK_GENERIC;
-  }
-}
-
-// EKT of the conv_tc_persist_kernel instantiation that runs this descriptor: its epilogue kind where an instantiation is
-// specialised for it, EK_GENERIC otherwise.  tc_conv_launch and tc_conv_query both read it, so what the query reports is
-// what runs.
-static int tc_launch_ekt(const TcConvDesc* d) {
-  if (d->mode == 3) return EK_GENERIC;
-  const int ek = d->P.epi_kind;
-  if (d->mode == 2) return d->BN != 32 && (ek == (EK_AFF | EK_SILU) || ek == (EK_SILU | EK_RES)) ? ek : EK_GENERIC;
-  switch (d->BN) {
-    case 64: return ek == 0 || ek == EK_AFF ? ek : EK_GENERIC;
-    case 128: return ek == 0 || ek == EK_AFF || ek == EK_QSM ? ek : EK_GENERIC;
-    case 256: return ek == 0 || ek == EK_AFF ? ek : EK_GENERIC;  // deep res_conv; downsample / to_out (bias)
-    default: return EK_GENERIC;
-  }
 }
 
 void tc_conv_query(const TcConvDesc* d, int info[4]) {
   info[0] = d->BN;
   info[1] = d->mode;
-  info[2] = tc_launch_ekt(d);
+  info[2] = tc_pick(d)->ekt;
   info[3] = d->num_tiles;
 }
 
 int tc_conv_launch(TcConvDesc* d, cudaStream_t st) {
-  {
-    const unsigned g = (unsigned)(d->num_tiles < g_num_sms ? d->num_tiles : g_num_sms);
-    static unsigned long long* dbg_dev = nullptr;
-    const char* dbg_env = getenv("IRSDE_TC_DEBUG");
-    const bool dbg = dbg_env && dbg_env[0] == '1';
-    if (dbg) {
-      if (!dbg_dev) cudaMalloc(&dbg_dev, 256 * TC_DBG_SLOTS * sizeof(unsigned long long));
-      cudaMemsetAsync(dbg_dev, 0, 256 * TC_DBG_SLOTS * sizeof(unsigned long long), st);
-    }
-    d->P.dbg = dbg ? dbg_dev : nullptr;
-#define TC_LAUNCH(BNV, PV, EKV)                                                                                            \
-  pdl_launch(conv_tc_persist_kernel<BNV, PV, EKV>, g, TC_THREADS, TcCfgP<BNV, PV>::SMEM_BYTES, st, d->map_a, d->map_b, d->map_o, \
-             d->map_r, d->P, d->tiles_m, d->num_tiles)
-    const int ekt = tc_launch_ekt(d);
-    if (d->mode == 3) {
-      switch (d->BN) {
-        case 32: TC_LAUNCH(32, 3, EK_GENERIC); break;
-        case 64: TC_LAUNCH(64, 3, EK_GENERIC); break;
-        default: TC_LAUNCH(128, 3, EK_GENERIC); break;
-      }
-    } else if (d->mode == 2) {
-      switch (d->BN) {
-        case 32: TC_LAUNCH(32, 2, EK_GENERIC); break;
-        case 64:
-          if (ekt == (EK_AFF | EK_SILU)) TC_LAUNCH(64, 2, EK_AFF | EK_SILU);
-          else if (ekt == (EK_SILU | EK_RES)) TC_LAUNCH(64, 2, EK_SILU | EK_RES);
-          else TC_LAUNCH(64, 2, EK_GENERIC);
-          break;
-        default:
-          if (ekt == (EK_AFF | EK_SILU)) TC_LAUNCH(128, 2, EK_AFF | EK_SILU);
-          else if (ekt == (EK_SILU | EK_RES)) TC_LAUNCH(128, 2, EK_SILU | EK_RES);
-          else TC_LAUNCH(128, 2, EK_GENERIC);
-          break;
-      }
-    } else {
-      switch (d->BN) {
-        case 32: TC_LAUNCH(32, 0, EK_GENERIC); break;
-        case 64:
-          if (ekt == 0) TC_LAUNCH(64, 0, 0);
-          else if (ekt == EK_AFF) TC_LAUNCH(64, 0, EK_AFF);
-          else TC_LAUNCH(64, 0, EK_GENERIC);
-          break;
-        case 128:
-          if (ekt == 0) TC_LAUNCH(128, 0, 0);
-          else if (ekt == EK_AFF) TC_LAUNCH(128, 0, EK_AFF);
-          else if (ekt == EK_QSM) TC_LAUNCH(128, 0, EK_QSM);
-          else TC_LAUNCH(128, 0, EK_GENERIC);
-          break;
-        default:
-          if (ekt == EK_AFF) TC_LAUNCH(256, 0, EK_AFF);
-          else if (ekt == 0) TC_LAUNCH(256, 0, 0);
-          else TC_LAUNCH(256, 0, EK_GENERIC);
-          break;
-      }
-    }
-#undef TC_LAUNCH
-    if (dbg) {
-      // per CTA: [0] producer cycles waiting on empty barriers, [1] producer cycles; per consumer warpgroup w: [2+w] cycles
-      // waiting on full barriers, [4+w] in the epilogue, [6+w] waiting for its ping-pong turn, [8+w] in all, [10+w] tiles
-      unsigned long long h[256 * TC_DBG_SLOTS];
-      cudaStreamSynchronize(st);
-      cudaMemcpy(h, dbg_dev, sizeof h, cudaMemcpyDeviceToHost);
-      double a[TC_DBG_SLOTS] = {0};
-      for (unsigned i = 0; i < g; ++i) for (int k = 0; k < TC_DBG_SLOTS; ++k) a[k] += (double)h[i * TC_DBG_SLOTS + k] / g;
-      fprintf(stderr,
-              "TCDBG BN=%d mode=%d ekt=%d grid=%u tiles=%d ntaps=%d kch=%d | prod wait %.0f / %.0f | wg0 full %.0f epi %.0f turn %.0f"
-              " / %.0f (tiles/cta %.1f) | wg1 full %.0f epi %.0f turn %.0f / %.0f (tiles/cta %.1f)\n",
-              d->BN, d->mode, tc_launch_ekt(d), g, d->num_tiles, d->P.ntaps, d->P.kchunks, a[0], a[1], a[2], a[4], a[6], a[8], a[10],
-              a[3], a[5], a[7], a[9], a[11]);
-    }
-    return 1;
+  const TcKernel& k = *tc_pick(d);
+  const unsigned g = (unsigned)(d->num_tiles < g_num_sms ? d->num_tiles : g_num_sms);
+  static unsigned long long* dbg_dev = nullptr;
+  const char* dbg_env = getenv("IRSDE_TC_DEBUG");
+  const bool dbg = dbg_env && dbg_env[0] == '1';
+  if (dbg) {
+    if (!dbg_dev) cudaMalloc(&dbg_dev, 256 * TC_DBG_SLOTS * sizeof(unsigned long long));
+    cudaMemsetAsync(dbg_dev, 0, 256 * TC_DBG_SLOTS * sizeof(unsigned long long), st);
   }
+  d->P.dbg = dbg ? dbg_dev : nullptr;
+  d->P.epi_kind = k.ekt;
+  const auto kernel = k.fn;
+  pdl_launch(kernel, g, TC_THREADS, k.smem, st, d->map_a, d->map_b, d->map_o, d->map_r, d->P, d->tiles_m, d->num_tiles);
+  if (dbg) {
+    // per CTA: [0] producer cycles waiting on empty barriers, [1] producer cycles; per consumer warpgroup w: [2+w] cycles
+    // waiting on full barriers, [4+w] in the epilogue, [6+w] waiting for its ping-pong turn, [8+w] in all, [10+w] tiles
+    unsigned long long h[256 * TC_DBG_SLOTS];
+    cudaStreamSynchronize(st);
+    cudaMemcpy(h, dbg_dev, sizeof h, cudaMemcpyDeviceToHost);
+    double a[TC_DBG_SLOTS] = {0};
+    for (unsigned i = 0; i < g; ++i) for (int j = 0; j < TC_DBG_SLOTS; ++j) a[j] += (double)h[i * TC_DBG_SLOTS + j] / g;
+    fprintf(stderr,
+            "TCDBG BN=%d mode=%d ekt=%d grid=%u tiles=%d ntaps=%d kch=%d | prod wait %.0f / %.0f | wg0 full %.0f epi %.0f turn %.0f"
+            " / %.0f (tiles/cta %.1f) | wg1 full %.0f epi %.0f turn %.0f / %.0f (tiles/cta %.1f)\n",
+            d->BN, d->mode, k.ekt, g, d->num_tiles, d->P.ntaps, d->P.kchunks, a[0], a[1], a[2], a[4], a[6], a[8], a[10], a[3], a[5],
+            a[7], a[9], a[11]);
+  }
+  return 1;
 }
 
 }  // namespace irsde

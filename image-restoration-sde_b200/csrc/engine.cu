@@ -691,8 +691,6 @@ struct Builder {
         a = s2d; a_pitch = in.C;
         release(s2d);  // safe: stream order; the next tmp user runs after this conv
       }
-      std::string terr;
-      TcConvDesc* d;
       if constexpr (f32) {
         // operand split (hi, lo) of the conv input: [2][planes][B][Ha][Wa][C]
         const long long npix_a = (long long)t.planes * plan->B * Ha * Wa;
@@ -704,14 +702,13 @@ struct Builder {
         }});
         plan->ops.back().label = wname + " tf32 hi/lo split of the input";
         plan->ops.back().bytes = 3.0 * npix_a * in.C * 4.0;
-        d = tc_conv_create_f32x3(split, plan->B, Ha, Wa, in.C, t.planes, wt, Cout, t.ntaps, t.taps, t.nph, ep, out.p, out.pitch,
-                                 g.Hout, g.Wout, &terr);
-        release(split);
-      } else {
-        d = tc_conv_create(a, a_pitch, plan->B, Ha, Wa, stem ? 64 : in.C, t.planes, wt, Cout, t.ntaps, t.taps, t.nph, ep, out.p,
-                           out.pitch, g.Hout, g.Wout, &terr, tc_flags);
+        a = split; a_pitch = in.C;
+        release(split);  // safe: stream order, as for s2d
       }
-      if (!d) { ok = false; err = (f32 ? "tc_conv_create_f32x3(" : "tc_conv_create(") + wname + "): " + terr; return; }
+      std::string terr;
+      TcConvDesc* d = tc_conv_create(a, a_pitch, plan->B, Ha, Wa, in.C, t.planes, wt, Cout, t.ntaps, t.taps, t.nph, ep, out.p,
+                                     out.pitch, g.Hout, g.Wout, &terr, tc_flags);
+      if (!d) { ok = false; err = "tc_conv_create(" + wname + "): " + terr; return; }
       plan->tc_descs.push_back(d);
       plan->ops.push_back(OpRec{CAT_TC, tc_flops, [=](Plan* p, cudaStream_t st) {
         if (use_ss) tc_conv_set_runtime(d, p->cur.ss, p->cur.t_ptr, p->cur.ss_img_stride);
@@ -1599,19 +1596,17 @@ int run_tc_conv(Scratch& sc, const ConvGeom& g, const S* in, int in_pitch, const
     in = s2d;
     in_pitch = g.Cin;
   }
+  if constexpr (f32) {
+    launch_split_tf32(in, in_pitch, split, npix, g.Cin, sc.st);
+    in = split;
+    in_pitch = g.Cin;
+  }
   Epilogue e0 = ep;
   e0.ss = nullptr; e0.t_ptr = nullptr; e0.ss_img_stride = 0;
   std::string terr;
-  TcConvDesc* d;
-  if constexpr (f32) {
-    launch_split_tf32(in, in_pitch, split, npix, g.Cin, sc.st);
-    d = tc_conv_create_f32x3(split, g.B, Ha, Wa, g.Cin, t.planes, w, g.Cout, t.ntaps, t.taps, t.nph, e0, out, out_pitch, g.Hout,
-                             g.Wout, &terr);
-  } else {
-    d = tc_conv_create(in, in_pitch, g.B, Ha, Wa, t.planes < 0 ? 64 : g.Cin, t.planes, w, g.Cout, t.ntaps, t.taps, t.nph, e0, out,
-                       out_pitch, g.Hout, g.Wout, &terr, flags);
-  }
-  if (!d) return fail(sc.ctx, IRSDE_ERR_INVALID, std::string(f32 ? "tc_conv_create_f32x3: " : "tc_conv_create: ") + terr);
+  TcConvDesc* d = tc_conv_create(in, in_pitch, g.B, Ha, Wa, g.Cin, t.planes, w, g.Cout, t.ntaps, t.taps, t.nph, e0, out, out_pitch,
+                                 g.Hout, g.Wout, &terr, flags);
+  if (!d) return fail(sc.ctx, IRSDE_ERR_INVALID, "tc_conv_create: " + terr);
   if (ep.ss) tc_conv_set_runtime(d, ep.ss, ep.t_ptr, ep.ss_img_stride);
   if (!out) tc_conv_set_out_nchw(d, out_nchw, crop_h, crop_w);
   if (info) tc_conv_query(d, info);
