@@ -8,8 +8,9 @@ Importing the package does not need a GPU; running anything does (no CPU fallbac
 """
 from . import _lib
 from .sde import IRSDE, DenoisingSDE
-from .unet import ConditionalUNet, DenoisingUNet, unet_param_shapes, adopt, infer_unet_config
-from .nafnet import ConditionalNAFNet, DenoisingNAFNet, nafnet_param_shapes
+from .unet import ConditionalUNet, DenoisingUNet, unet_param_shapes, infer_unet_config
+from .nafnet import ConditionalNAFNet, DenoisingNAFNet, nafnet_param_shapes, infer_nafnet_config
+from .shadow import adopt
 from .latent import UNet, latent_unet_param_shapes
 from . import imaging
 from .imaging import tensor2img, calculate_psnr, calculate_ssim
@@ -18,6 +19,6 @@ from .refusion import TiledRefusion, tile_boxes, plan_units
 from .dist import shard_range, sharded_reverse, broadcast_weights, NativeComm, comm_unique_id
 
 __all__ = ["IRSDE", "DenoisingSDE", "ConditionalUNet", "DenoisingUNet", "ConditionalNAFNet", "DenoisingNAFNet", "UNet", "unet_param_shapes", "adopt", "infer_unet_config", "latent_unet_param_shapes",
-           "nafnet_param_shapes", "shard_range",
+           "nafnet_param_shapes", "infer_nafnet_config", "shard_range",
            "sharded_reverse", "broadcast_weights", "NativeComm", "comm_unique_id", "TiledRefusion", "tile_boxes", "plan_units", "imaging", "Restorer", "plan_batches", "tensor2img", "calculate_psnr", "calculate_ssim", "_lib"]
 __version__ = "0.1"

@@ -63,6 +63,36 @@ def nafnet_param_shapes(img_channel, width, middle_blk_num, enc_blk_nums, dec_bl
     return S
 
 
+def infer_nafnet_config(state_dict):
+    """(img_channel, width, middle_blk_num, enc_blk_nums, dec_blk_nums, variant) of a ConditionalNAFNet state dict in the
+    reference's naming, or None.  Only an exact match with ``nafnet_param_shapes`` (same keys in the same order, same
+    shapes) is accepted, so networks with extra modules (stereo-sr's ``fusion.*``, latent-bokeh's ``cam_mlp.*``) decline.
+    The image-space and latent forms have identical state dicts; ``shadow.adopt`` tells them apart by a probe."""
+    try:
+        sd = state_dict
+        width, cin = sd["intro.weight"].shape[:2]
+        img_channel = sd["ending.weight"].shape[0]
+        variant = {img_channel: "denoising", 2 * img_channel: "conditional"}.get(cin)
+        if variant is None:
+            return None
+
+        def blocks(prefix):   # number of blocks j with keys "<prefix>j."
+            js = [int(k[len(prefix):].split(".")[0]) for k in sd if k.startswith(prefix)]
+            return max(js) + 1 if js else 0
+
+        enc = [blocks("encoders.%d." % i) for i in range(len([k for k in sd if k.startswith("downs.") and k.endswith(".weight")]))]
+        dec = [blocks("decoders.%d." % i) for i in range(len([k for k in sd if k.startswith("ups.")]))]
+        middle = blocks("middle_blks.")
+        if len(enc) != len(dec) or len(enc) > 8:
+            return None
+        shapes = nafnet_param_shapes(img_channel, width, middle, enc, dec, variant)
+        if list(shapes) != list(sd) or any(tuple(sd[k].shape) != tuple(v) for k, v in shapes.items()):
+            return None
+        return img_channel, width, middle, enc, dec, variant
+    except Exception:
+        return None
+
+
 class _NafConfig(ctypes.Structure):
     _fields_ = [("img_channel", ctypes.c_int32), ("width", ctypes.c_int32), ("middle_blk_num", ctypes.c_int32),
                 ("n_levels", ctypes.c_int32), ("enc_blk_nums", ctypes.c_int32 * 8), ("dec_blk_nums", ctypes.c_int32 * 8),

@@ -22,13 +22,14 @@ def _unwrap(model):
     m = getattr(model, "module", model)
     if m is None or isinstance(m, ConditionalUNet):
         return m
-    # A foreign nn.Module with the reference ConditionalUNet's state-dict layout (e.g. the reference's own PyTorch class
-    # being trained by autograd in train.py): sample through a native shadow that re-reads its parameters (unet.adopt).
-    # Opt out with IRSDE_B200_ADOPT=0; modules in training mode are left alone (autograd needs the PyTorch forward).
+    # A foreign nn.Module with the reference ConditionalUNet's or ConditionalNAFNet's state-dict layout (e.g. the reference's
+    # own PyTorch class being trained by autograd in train.py): sample through a native shadow that re-reads its parameters
+    # (shadow.adopt).  Opt out with IRSDE_B200_ADOPT=0; modules in training mode are left alone (autograd needs the PyTorch
+    # forward).
     if isinstance(m, torch.nn.Module) and os.environ.get("IRSDE_B200_ADOPT", "1") != "0" and not m.training:
         sh = getattr(m, "_irsde_b200_shadow", None)
         if sh is None:
-            from .unet import adopt
+            from .shadow import adopt
             sh = adopt(m) or False
             try:
                 object.__setattr__(m, "_irsde_b200_shadow", sh)

@@ -147,7 +147,7 @@ class ConditionalUNet(nn.Module):
         return self._ctx
 
     def sync_weights(self, device=None):
-        """Upload parameters to the native context if they changed since the last upload.  ``_source`` (set by ``adopt``)
+        """Upload parameters to the native context if they changed since the last upload.  ``_source`` (set by ``shadow.adopt``)
         names another module that owns the parameters: e.g. the reference's own PyTorch ConditionalUNet while it is being
         trained by autograd - the native network then shadows it (same state-dict names) for validation sampling."""
         import ctypes
@@ -167,6 +167,7 @@ class ConditionalUNet(nn.Module):
             _lib.check(L.irsde_load_tensor(ctx.h, name.encode(), ctypes.c_void_p(t.data_ptr()), t.dim(), shape), ctx.h)
         _lib.check(L.irsde_finalize_weights(ctx.h), ctx.h)
         self._sig = sig
+        self._uploads = getattr(self, "_uploads", 0) + 1
         return ctx
 
     # ---- forward ---------------------------------------------------------------------------------
@@ -242,6 +243,10 @@ class ConditionalUNet(nn.Module):
     def launch_count(self):
         return int(self._ctx.L.irsde_launch_count(self._ctx.h)) if self._ctx else 0
 
+    def upload_count(self):
+        """How many times ``sync_weights`` uploaded the parameters (once per change of their storage or version)."""
+        return getattr(self, "_uploads", 0)
+
 
 class DenoisingUNet(ConditionalUNet):
     """The denoising-sde variant: no condition input, full softmax ``Attention`` at ``mid_attn``
@@ -277,29 +282,3 @@ def infer_unet_config(state_dict):
     except Exception:
         return None
 
-
-def adopt(module, precision=None):
-    """Native shadow of a foreign ``nn.Module`` that has the reference ConditionalUNet's state-dict layout (the
-    reference's own PyTorch class, codes/config/*/models/modules/DenoisingUNet_arch.py): the shadow keeps no weights of its
-    own - every call re-reads the foreign module's parameters when their versions changed (optimizer steps bump them) -
-    so `train.py` can keep training the PyTorch module with autograd while validation sampling (train.py:261-281) runs on
-    the native kernels.  Returns None when the state dict is not a ConditionalUNet."""
-    sd = {k: v for k, v in module.state_dict().items()}
-    cfg = infer_unet_config(sd)
-    if cfg is None:
-        return None
-    in_nc, out_nc, nf, mult, variant = cfg
-    plain = mult == [2 ** (i + 1) for i in range(len(mult))]
-    if variant == "denoising":
-        if not plain:
-            return None
-        net = DenoisingUNet(in_nc, out_nc, nf, depth=len(mult), precision=precision)
-    else:
-        net = ConditionalUNet(in_nc, out_nc, nf, depth=len(mult), precision=precision, ch_mult=None if plain else mult)
-    if list(net._shapes.keys()) != list(sd.keys()) or any(tuple(sd[k].shape) != tuple(v) for k, v in net._shapes.items()):
-        return None
-    for p in net.parameters():       # the shadow's own tensors are never used: do not keep a second copy of the weights
-        p.data = torch.empty(0)
-    net._source = module
-    net.eval()
-    return net
