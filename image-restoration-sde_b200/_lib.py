@@ -17,6 +17,8 @@ NET_CONDITIONAL, NET_DENOISING = 0, 1
 MODE_SDE, MODE_ODE, MODE_POSTERIOR, MODE_DSDE_SDE, MODE_DSDE_ODE = range(5)
 NUM_COEF = 8
 FLAG_FORCE_SIMT = 1   # irsde_config.flags: bf16 storage through the SIMT conv engine (debug aid)
+# irsde_conv2d_fused engines: fp32 SIMT, bf16 wgmma, fp32x3 wgmma, SIMT over bf16 storage
+CONV_SIMT_FP32, CONV_TC_BF16, CONV_TC_FP32X3, CONV_SIMT_BF16 = range(4)
 
 # every symbol include/irsde_b200.h declares
 SYMBOLS = ["irsde_create", "irsde_create_ch_mult", "irsde_create_nafnet", "irsde_create_nafnet_variant", "irsde_create_latent_unet", "irsde_latent_shape", "irsde_latent_encode",

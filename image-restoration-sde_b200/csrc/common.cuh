@@ -96,6 +96,10 @@ struct ConvGeom {
 template <typename T>
 void launch_conv_simt(const ConvGeom& g, const T* in, int in_pitch, const float* w, const Epilogue& ep, T* out,
                       int out_pitch, float* out_nchw, int cropH, int cropW, cudaStream_t st);
+// The code path launch_conv_simt takes for these operands: {vecA (4-wide input gather), vecB (4-wide weight load), vecO
+// (4-wide NHWC store), blocks}.
+template <typename T>
+void conv_simt_path(const ConvGeom& g, const T* in, int in_pitch, const float* w, const T* out, int out_pitch, int32_t path[4]);
 
 // ---- elementwise / reduction kernels (elementwise.cu) -----------------------------------------
 template <typename T>

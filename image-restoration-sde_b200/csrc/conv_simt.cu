@@ -197,17 +197,27 @@ __global__ void __launch_bounds__(256) conv_simt_kernel(ConvGeom g, const T* __r
 }  // namespace
 
 template <typename T>
+void conv_simt_path(const ConvGeom& g, const T* in, int in_pitch, const float* w, const T* out, int out_pitch, int32_t path[4]) {
+  const long long M = (long long)g.B * g.Hout * g.Wout;
+  const int vw = 4 * sizeof(T);  // bytes of a 4-element vector
+  path[0] = (g.Cin % 4 == 0) && (in_pitch % 4 == 0) && (((uintptr_t)in) % vw == 0);
+  path[1] = (g.Cout % 4 == 0) && (((uintptr_t)w) % 16 == 0);
+  path[2] = out && (out_pitch % 4 == 0) && (((uintptr_t)out) % vw == 0);
+  path[3] = (int32_t)((M + BM - 1) / BM * ((g.Cout + BN - 1) / BN));
+}
+
+template <typename T>
 void launch_conv_simt(const ConvGeom& g, const T* in, int in_pitch, const float* w, const Epilogue& ep, T* out,
                       int out_pitch, float* out_nchw, int cropH, int cropW, cudaStream_t st) {
   long long M = (long long)g.B * g.Hout * g.Wout;
   dim3 grid((unsigned)((M + BM - 1) / BM), (unsigned)((g.Cout + BN - 1) / BN));
-  const int vw = 4 * sizeof(T);  // bytes of a 4-element vector
-  int vecA = (g.Cin % 4 == 0) && (in_pitch % 4 == 0) && (((uintptr_t)in) % vw == 0);
-  int vecB = (g.Cout % 4 == 0) && (((uintptr_t)w) % 16 == 0);
-  int vecO = out && (out_pitch % 4 == 0) && (((uintptr_t)out) % vw == 0);
-  pdl_launch(conv_simt_kernel<T>, grid, 256, 0, st, g, in, in_pitch, w, ep, out, out_pitch, out_nchw, cropH, cropW, vecA, vecB,
-                                            vecO);
+  int32_t path[4];
+  conv_simt_path<T>(g, in, in_pitch, w, out, out_pitch, path);
+  pdl_launch(conv_simt_kernel<T>, grid, 256, 0, st, g, in, in_pitch, w, ep, out, out_pitch, out_nchw, cropH, cropW, (int)path[0],
+             (int)path[1], (int)path[2]);
 }
+template void conv_simt_path<float>(const ConvGeom&, const float*, int, const float*, const float*, int, int32_t*);
+template void conv_simt_path<bf16>(const ConvGeom&, const bf16*, int, const float*, const bf16*, int, int32_t*);
 template void launch_conv_simt<float>(const ConvGeom&, const float*, int, const float*, const Epilogue&, float*, int,
                                       float*, int, int, cudaStream_t);
 template void launch_conv_simt<bf16>(const ConvGeom&, const bf16*, int, const float*, const Epilogue&, bf16*, int,

@@ -1564,13 +1564,14 @@ int32_t* zeroed_info(int32_t* info, int32_t* local) {
 }
 
 // Which of the tap-GEMM's conv shapes (tap_table) a standalone conv is: 3x3/1 pad 1 (also after nearest x2), 1x1, 4x4/2
-// pad 1 over an even H x W, or the 7x7/1 pad 3 stem.  Each entry applies its own engine rules on top.
+// pad 1 or 2x2/2 pad 0 over an even H x W, or the 7x7/1 pad 3 stem.  Each entry applies its own engine rules on top.
 struct ConvShape {
-  bool k3, k1, k4, k7;
+  bool k3, k1, k4, k2, k7;
 };
 ConvShape conv_shape(int KH, int KW, int stride, int pad, int up, int H, int W) {
+  const bool even = up == 1 && H % 2 == 0 && W % 2 == 0;
   return ConvShape{KH == 3 && KW == 3 && stride == 1 && pad == 1, KH == 1 && KW == 1 && stride == 1 && pad == 0 && up == 1,
-                   KH == 4 && KW == 4 && stride == 2 && pad == 1 && up == 1 && H % 2 == 0 && W % 2 == 0,
+                   KH == 4 && KW == 4 && stride == 2 && pad == 1 && even, KH == 2 && KW == 2 && stride == 2 && pad == 0 && even,
                    KH == 7 && KW == 7 && stride == 1 && pad == 3 && up == 1};
 }
 ConvGeom conv_geom(int B, int Cin, int H, int W, int Cout, int KH, int KW, int stride, int pad, int up) {
@@ -1615,22 +1616,25 @@ int run_tc_conv(Scratch& sc, const ConvGeom& g, const S* in, int in_pitch, const
   return IRSDE_OK;
 }
 
-// One conv outside a plan, on engine 0 (SIMT, fp32), 1 (bf16 tap-GEMM) or 2 (fp32x3 tap-GEMM): packs w into the scratch in
-// layout wl and runs it.  in and ep.res are NHWC views in the engine's storage type S (the stem's padded layout for K = 7).
-// The output is the NHWC view (out, out_pitch), or with out == nullptr fp32 NCHW at out_nchw cropped to crop_h x crop_w.
-// flags are the tap-GEMM's TC_FLAG_*; info (may be null) receives its tc_conv_query.
+// One conv outside a plan in storage type S: packs w into the scratch in layout wl and runs it, on the SIMT kernel for
+// WL_SIMT (fp32 weights, as in a plan) and on the tap-GEMM otherwise.  in and ep.res are NHWC views in S (the stem's
+// padded layout for K = 7).  The output is the NHWC view (out, out_pitch), or with out == nullptr fp32 NCHW at out_nchw
+// cropped to crop_h x crop_w.  flags are the tap-GEMM's TC_FLAG_*; info (may be null) receives the SIMT kernel's
+// conv_simt_path or the tap-GEMM's tc_conv_query.
 template <typename S>
-int run_conv(Scratch& sc, int engine, const ConvGeom& g, const S* in, int in_pitch, WLayout wl, const float* w, const Epilogue& ep,
-             S* out, int out_pitch, float* out_nchw, int crop_h, int crop_w, int flags, int32_t* info) {
+int run_conv(Scratch& sc, const ConvGeom& g, const S* in, int in_pitch, WLayout wl, const float* w, const Epilogue& ep, S* out,
+             int out_pitch, float* out_nchw, int crop_h, int crop_w, int flags, int32_t* info) {
+  if (wl == WL_SIMT) {
+    float* wp = sc.alloc<float>(packed_weight_elems<float>(wl, g.Cout, g.Cin, g.KH, g.KW));
+    if (!wp) return sc.oom();
+    pack_weight<float>(wl, w, wp, g.Cout, g.Cin, g.KH, g.KW, g.B, sc.st);
+    if (info) conv_simt_path<S>(g, in, in_pitch, wp, out, out_pitch, info);
+    launch_conv_simt<S>(g, in, in_pitch, wp, ep, out, out_pitch, out_nchw, crop_h, crop_w, sc.st);
+    return IRSDE_OK;
+  }
   S* wp = sc.alloc<S>(packed_weight_elems<S>(wl, g.Cout, g.Cin, g.KH, g.KW, g.B));
   if (!wp) return sc.oom();
   pack_weight<S>(wl, w, wp, g.Cout, g.Cin, g.KH, g.KW, g.B, sc.st);
-  if constexpr (std::is_same<S, float>::value) {
-    if (engine == 0) {
-      launch_conv_simt<float>(g, in, in_pitch, wp, ep, out, out_pitch, out_nchw, crop_h, crop_w, sc.st);
-      return IRSDE_OK;
-    }
-  }
   return run_tc_conv<S>(sc, g, in, in_pitch, wp, ep, out, out_pitch, out_nchw, crop_h, crop_w, flags, info);
 }
 
@@ -2348,8 +2352,8 @@ int irsde_conv2d_ex(irsde_ctx* ctx, int32_t engine, const float* x, const float*
     ep.bias = bias;
     ep.silu = silu;
     if (res) { ep.res = res; ep.res_pitch = Cout; }
-    const int rc = run_conv<S>(sc, engine, g, xin, k7 ? 8 : Cin, wl, w, ep, nchw ? nullptr : yo, Cout, nchw ? y : nullptr, Ho, Wo,
-                               tc_flags, nullptr);
+    const int rc = run_conv<S>(sc, g, xin, k7 ? 8 : Cin, wl, w, ep, nchw ? nullptr : yo, Cout, nchw ? y : nullptr, Ho, Wo, tc_flags,
+                               nullptr);
     if (!rc && !nchw) launch_nhwc_to_nchw<S>(yo, Cout, y, B, Cout, Ho, Wo, sc.st);
     return rc;
   };
@@ -2364,11 +2368,20 @@ int irsde_conv2d_fused(irsde_ctx* ctx, int32_t engine, const float* x, const flo
   // ---- everything is validated here, before the first launch: no argument may make a kernel index out of bounds
   if (!ctx || !x || !w || !y || !epi) return fail(ctx, IRSDE_ERR_INVALID, "null argument");
   const irsde_conv_epilogue& e = *epi;
-  if (engine < 0 || engine > 2) return fail(ctx, IRSDE_ERR_INVALID, "unknown engine");
+  if (engine < 0 || engine > 3) return fail(ctx, IRSDE_ERR_INVALID, "unknown engine");
   if (B < 1 || Cin < 1 || H < 1 || W < 1 || Cout < 1) return fail(ctx, IRSDE_ERR_INVALID, "bad shape");
+  const bool simt = engine == 0 || engine == 3, bf = engine == 1 || engine == 3;
   const int up = upsample ? 2 : 1;
   const ConvShape s = conv_shape(KH, KW, stride, pad, up, H, W);
-  if (!(s.k3 || s.k1 || s.k4)) return fail(ctx, IRSDE_ERR_UNSUPPORTED, "fused conv: 3x3/1 (optionally after nearest x2), 1x1 or 4x4/2");
+  const bool k7 = engine == 1 && s.k7;  // the bf16 tensor-core stem
+  if (simt) {  // the SIMT kernel takes any kernel size, stride and padding
+    if (KH < 1 || KW < 1 || KH > 16 || KW > 16 || stride < 1 || pad < 0 || pad >= KH || pad >= KW ||
+        H * up + 2 * pad < KH || W * up + 2 * pad < KW)
+      return fail(ctx, IRSDE_ERR_INVALID, "SIMT conv: bad kernel size, stride or padding");
+  } else if (!(s.k3 || s.k1 || s.k4 || s.k2 || k7)) {
+    return fail(ctx, IRSDE_ERR_UNSUPPORTED,
+                "tensor-core conv: 3x3/1 (optionally after nearest x2), 1x1, 4x4/2 or 2x2/2 over an even H x W, or the bf16 7x7 stem");
+  }
   const ConvGeom g = conv_geom(B, Cin, H, W, Cout, KH, KW, stride, pad, up);
   const int Ho = g.Hout, Wo = g.Wout;
   const bool nchw = e.crop_h != 0 || e.crop_w != 0;
@@ -2376,19 +2389,21 @@ int irsde_conv2d_fused(irsde_ctx* ctx, int32_t engine, const float* x, const flo
   if (e.flags & ~IRSDE_CONV_QSOFTMAX) return fail(ctx, IRSDE_ERR_UNSUPPORTED, "fused conv: flags other than IRSDE_CONV_QSOFTMAX");
   if (qsm && (engine != 1 || !s.k1 || Cout < 128 || nchw))
     return fail(ctx, IRSDE_ERR_INVALID, "q-softmax is the bf16 epilogue of a 1x1 conv with Cout >= 128");
-  const int al = engine == 1 ? 8 : 4;  // elements per 16 bytes of the engine's storage type
-  if (engine != 0 && (Cin % al || (!nchw && Cout % al)))
-    return fail(ctx, IRSDE_ERR_INVALID, "tensor-core engines: Cin and Cout must be multiples of 16 bytes");
-  if (!view_ok(e.in_pitch, e.in_off, Cin, al)) return fail(ctx, IRSDE_ERR_INVALID, "input view outside its pitch or not 16-byte aligned");
+  // views: offsets and pitches in 16 bytes of the tap-GEMM's storage type, or in the SIMT kernel's 4-element vectors
+  const int al = engine == 1 ? 8 : 4;
+  if (!simt && ((k7 ? Cin > 8 : Cin % al) || (!nchw && Cout % al)))
+    return fail(ctx, IRSDE_ERR_INVALID, "tensor-core engines: Cin and Cout must be multiples of 16 bytes (the stem: Cin <= 8)");
+  if (!view_ok(e.in_pitch, e.in_off, Cin, al)) return fail(ctx, IRSDE_ERR_INVALID, "input view outside its pitch or not aligned");
   if (nchw) {
-    if (!s.k3 || up != 1) return fail(ctx, IRSDE_ERR_UNSUPPORTED, "the cropped fp32 NCHW output is the 3x3 head's epilogue");
+    if (!simt && (!s.k3 || up != 1))
+      return fail(ctx, IRSDE_ERR_UNSUPPORTED, "the tensor-core engines' cropped fp32 NCHW output is the 3x3 head's epilogue");
     if (e.crop_h < 1 || e.crop_w < 1 || e.crop_h > Ho || e.crop_w > Wo) return fail(ctx, IRSDE_ERR_INVALID, "crop larger than the output");
     if (e.res) return fail(ctx, IRSDE_ERR_UNSUPPORTED, "no residual with the NCHW output");
   } else if (!view_ok(e.out_pitch, e.out_off, Cout, al)) {
-    return fail(ctx, IRSDE_ERR_INVALID, "output view outside its pitch or not 16-byte aligned");
+    return fail(ctx, IRSDE_ERR_INVALID, "output view outside its pitch or not aligned");
   }
   if (e.res && !view_ok(e.res_pitch, e.res_off, Cout, al))
-    return fail(ctx, IRSDE_ERR_INVALID, "residual view outside its pitch or not 16-byte aligned");
+    return fail(ctx, IRSDE_ERR_INVALID, "residual view outside its pitch or not aligned");
   if (e.ss) {
     if (e.mult_vec) return fail(ctx, IRSDE_ERR_INVALID, "the time-modulation table and mult_vec cannot be combined");
     if (e.t_row < 0 || e.ss_img_stride < 0 || (long long)e.t_row + (long long)(B - 1) * e.ss_img_stride >= e.ss_rows)
@@ -2404,7 +2419,7 @@ int irsde_conv2d_fused(irsde_ctx* ctx, int32_t engine, const float* x, const flo
 
   cudaSetDevice(ctx->cfg.device);
   std::string terr;
-  if (engine != 0 && !tc_init(&terr)) return fail(ctx, IRSDE_ERR_CUDA, "tc_init: " + terr);
+  if (!simt && !tc_init(&terr)) return fail(ctx, IRSDE_ERR_CUDA, "tc_init: " + terr);
   Scratch sc(ctx, (cudaStream_t)stream);
   const int* t_dev = sc.upload(e.t_row);
   if (!t_dev) return sc.oom();
@@ -2417,21 +2432,36 @@ int irsde_conv2d_fused(irsde_ctx* ctx, int32_t engine, const float* x, const flo
   ep.ss_off = e.ss_off;
   if (e.ss) { ep.ss = e.ss; ep.t_ptr = t_dev; ep.ss_img_stride = e.ss_img_stride; }
   ep.res_pitch = e.res_pitch;
-  const WLayout wl = engine == 0 ? WL_SIMT : (s.k3 && up == 2) ? WL_UP : WL_TAPS;
+  const WLayout wl = simt ? WL_SIMT : k7 ? WL_STEM : (s.k3 && up == 2) ? WL_UP : WL_TAPS;
   float* out_nchw = nchw ? y : nullptr;
   int rc;
-  if (engine == 1) {  // bf16 copies of the whole of x, res and y
+  if (bf) {  // bf16 copies of the whole of x, res and y
     const long long npix_out = (long long)B * Ho * Wo;
-    const bf16* xb = sc.in(x, (long long)B * H * W * e.in_pitch);
+    const bf16* xb;
+    int in_pitch = e.in_pitch;
+    if (k7) {  // the stem reads its input view from the zero-bordered [B][H+6][W+8][8] layout, as a plan stages it
+      const long long nin = (long long)B * (H + 6) * (W + 8) * 8 + 64;
+      float* xn = sc.alloc<float>((long long)B * Cin * H * W);
+      bf16* xp = sc.alloc<bf16>(nin);
+      if (!xn || !xp) return sc.oom();
+      cudaMemsetAsync(xp, 0, nin * sizeof(bf16), sc.st);
+      launch_nhwc_to_nchw<float>(x + e.in_off, e.in_pitch, xn, B, Cin, H, W, sc.st);
+      launch_prep_input<bf16>(xn, nullptr, xp, B, Cin, H, W, H, W, 8, 0, sc.st, 3, 3, W + 8, H + 6);
+      xb = xp;
+      in_pitch = 8;
+    } else {
+      xb = sc.in(x, (long long)B * H * W * e.in_pitch);
+      if (xb) xb += e.in_off;
+    }
     const bf16* rb = e.res ? sc.in(e.res, npix_out * e.res_pitch) : nullptr;
     bf16* yb = nchw ? nullptr : sc.inout(y, npix_out * e.out_pitch);
     if (!xb || (e.res && !rb) || (!nchw && !yb)) return sc.oom();
     if (rb) ep.res = rb + e.res_off;
-    rc = run_conv<bf16>(sc, engine, g, xb + e.in_off, e.in_pitch, wl, w, ep, yb ? yb + e.out_off : nullptr, e.out_pitch, out_nchw,
-                        e.crop_h, e.crop_w, qsm ? TC_FLAG_QSOFTMAX : 0, info);
+    rc = run_conv<bf16>(sc, g, xb, in_pitch, wl, w, ep, yb ? yb + e.out_off : nullptr, e.out_pitch, out_nchw, e.crop_h, e.crop_w,
+                        qsm ? TC_FLAG_QSOFTMAX : 0, info);
   } else {
     if (e.res) ep.res = e.res + e.res_off;
-    rc = run_conv<float>(sc, engine, g, x + e.in_off, e.in_pitch, wl, w, ep, nchw ? nullptr : y + e.out_off, e.out_pitch, out_nchw,
+    rc = run_conv<float>(sc, g, x + e.in_off, e.in_pitch, wl, w, ep, nchw ? nullptr : y + e.out_off, e.out_pitch, out_nchw,
                          e.crop_h, e.crop_w, 0, info);
   }
   if (!rc) ctx->launches += 4;

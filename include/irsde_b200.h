@@ -266,14 +266,19 @@ typedef struct {
                               /* top-left crop_h x crop_w pixels; out_pitch / out_off are then ignored */
 } irsde_conv_epilogue;
 
-/* One conv of the launch plan with its fused epilogue, through the same descriptor and launch calls the plan builder uses
- * (engine 0 = fp32 SIMT, 1 = bf16 wgmma, 2 = fp32x3 wgmma; KxK/stride/pad/upsample as in irsde_conv2d, 3x3/1, 1x1 and 4x4/2).
- * y is read and written: the whole buffer is converted to the engine's storage type (bf16 for engine 1), the conv writes its
- * slice, and the whole buffer is converted back, so an element outside the slice comes back unchanged when it is
+/* One conv of the launch plan with its fused epilogue, through the same descriptor and launch calls the plan builder uses.
+ * Engines: 0 = fp32 SIMT, 1 = bf16 wgmma, 2 = fp32x3 wgmma, 3 = the SIMT kernel over bf16 storage (fp32 weights), which a
+ * bf16 plan runs for every conv the tensor cores refuse.  The SIMT engines take any KxK, stride, padding and upsample; the
+ * wgmma engines 3x3/1 (optionally after nearest x2), 1x1, and 4x4/2 pad 1 or 2x2/2 pad 0 over an even H x W, and engine 1
+ * also the 7x7/1 stem (Cin <= 8, staged into its zero-bordered layout as a plan stages it).
+ * y is read and written: the whole buffer is converted to the engine's storage type (bf16 for engines 1 and 3), the conv
+ * writes its slice, and the whole buffer is converted back, so an element outside the slice comes back unchanged when it is
  * representable in that type.  Every view, table row and crop is checked on the host before anything is launched; offsets
- * and pitches must be multiples of 16 bytes of the engine's storage type.
+ * and pitches must be multiples of 16 bytes of the storage type on the wgmma engines, of 4 elements on the SIMT engines.
+ * The cropped fp32 NCHW output is the 3x3/1 head's on the wgmma engines, any conv's on the SIMT engines.
  * info (or NULL) receives {BN, MODE, EKT, number of output tiles} of the conv_tc_persist_kernel instantiation that ran
- * (engines 1 and 2), or zeros (engine 0). */
+ * (engines 1 and 2), or {vecA, vecB, vecO, blocks}: the SIMT kernel's 4-wide input gather, weight load and NHWC store, each
+ * 1 when taken (engines 0 and 3). */
 int irsde_conv2d_fused(irsde_ctx* ctx, int32_t engine, const float* x, const float* w, const irsde_conv_epilogue* ep, float* y,
                        int32_t B, int32_t Cin, int32_t H, int32_t W, int32_t Cout, int32_t KH, int32_t KW, int32_t stride,
                        int32_t pad, int32_t upsample, int32_t* info, void* stream);

@@ -1,12 +1,14 @@
 """Every instantiation of the tap-GEMM conv kernel (conv_tc_persist_kernel<BN, MODE, EKT>) with its fused epilogue, against
 an fp64 reference, through irsde_conv2d_fused: the same descriptor, runtime-table and launch calls the launch plan makes,
 with the views the plan gives a conv (channel-offset input, output and residual views into wider buffers, a cropped fp32
-NCHW head) and the time-modulation table read at a runtime row, shared by the batch or one row per image.
+NCHW head) and the time-modulation table read at a runtime row, shared by the batch or one row per image.  The rows include
+the NAFNet downs (2x2/2 over space-to-depth planes) at the BN the selector picks for each width, and the bf16 7x7 stem.
 
 Each case names the <BN, MODE, EKT> it must land on and checks it through the `info` the call returns.  The reference is
 the conv of the operands rounded as the engine rounds them (bf16 for engine 1) in fp64, then (acc + bias) * (scale + 1) +
 shift (or * mult_vec), SiLU, + residual.  Bounds: bf16 2^-8 |ref| + 1e-3 max|ref| (output rounding and summation order);
-fp32x3 max(2e-5 max|ref|, 8x what plain fp32 gets); fp32 SIMT 2e-5.  Before the kernel's output is compared, every
+fp32x3 max(2e-5 max|ref|, 8x what plain fp32 gets); fp32 SIMT 2e-5.  The SIMT kernel's own matrix is
+test_gpu_conv_simt.py; the three SIMT rows here stay for test_fused_conv_refuses_bad_views, which reuses the pitched one.  Before the kernel's output is compared, every
 time-modulated case shows that references built from a wrong table row, another image's row, scale and shift exchanged,
 or the table shifted by one channel all violate its bound.  Everything outside the conv's output slice (other channels of
 the wide buffer, a guard band after the cropped NCHW head) must come back bit-identical.
@@ -56,6 +58,17 @@ CASES = [
     _case("per-tap BN=256: 3x3 64->256, ragged 60x50 (BW=8, BH=16), bias + shared row", (256, 0, AFF), 1, 3, 64, 60, 50,
           256, 3, bias=True, ss="shared", t_row=1),
     _case("per-tap BN=256: 1x1 128->512 into a concat slice", (256, 0, 0), 1, 9, 128, 32, 32, 512, 1, out_view=(768, 256)),
+    # ---- engine 1 (bf16): the NAFNet downs (2x2/2 over space-to-depth planes, bias) and the 7x7 stem (7 row taps)
+    _case("per-tap BN=128: NAFNet downs.0 2x2/2 64->128, bias", (128, 0, AFF), 1, 3, 64, 128, 128, 128, 2, bias=True),
+    _case("per-tap BN=256: NAFNet downs.1 2x2/2 128->256, bias", (256, 0, AFF), 1, 2, 128, 256, 256, 256, 2, bias=True),
+    _case("per-tap BN halved 256 -> 128: NAFNet downs.2 2x2/2 256->512, bias", (128, 0, AFF), 1, 1, 256, 128, 128, 512, 2,
+          bias=True),
+    _case("per-tap BN halved 256 -> 64: NAFNet downs.3 2x2/2 512->1024, bias", (64, 0, AFF), 1, 2, 512, 32, 32, 1024, 2,
+          bias=True),
+    _case("per-tap BN=64 stem: 7x7 Cin 6 in pitch 8 -> 64, into channels 64.. of a 128-ch buffer", (64, 0, 0), 1, 2, 6, 20,
+          28, 64, 7, in_view=(8, 0), out_view=(128, 64)),
+    _case("per-tap BN=64 stem: 7x7 Cin 3 in pitch 8 -> 64", (64, 0, 0), 1, 2, 3, 32, 24, 64, 7, in_view=(8, 0)),
+    _case("per-tap BN=64 stem: 7x7 Cin 6 -> 64, ragged 37x53", (64, 0, 0), 1, 2, 6, 37, 53, 64, 7, in_view=(8, 0)),
     # ---- engine 1 (bf16), ROWS (MODE 2)
     _case("ROWS BN=32: 3x3 24->16, W < 16 (BW=8), H % 16 != 0, bias + SiLU", (32, 2, GEN), 1, 2, 24, 13, 7, 16, 3,
           bias=True, silu=True),
@@ -81,6 +94,7 @@ CASES = [
           silu=True, ss="image", t_row=3, min_tiles=2 * NUM_SMS),
     _case("fp32x3 BN=128: nearest x2 + 3x3 40->136 (two N tiles), shared row + pitched residual", (128, 3, GEN), 2, 2, 40,
           6, 10, 136, 3, up=True, ss="shared", t_row=5, res_view=(144, 8)),
+    _case("fp32x3 BN=128: NAFNet down 2x2/2 64->128, bias", (128, 3, GEN), 2, 3, 64, 128, 128, 128, 2, bias=True),
     # ---- engine 0 (fp32 SIMT)
     _case("SIMT: 3x3 20->12, per-image rows + SiLU + pitched residual, pitched input and output", None, 0, 3, 20, 9, 11, 12,
           3, silu=True, ss="image", t_row=1, in_view=(24, 4), out_view=(20, 8), res_view=(16, 4)),
@@ -114,7 +128,7 @@ def scratch_ctx(lib):
 
 def _geom(c):
     K = c["K"]
-    s, p = (2, 1) if K == 4 else (1, (K - 1) // 2)
+    s, p = {4: (2, 1), 2: (2, 0)}.get(K, (1, (K - 1) // 2))  # 4x4/2 pad 1, 2x2/2 pad 0, else KxK/1 "same"
     up = 2 if c["up"] else 1
     return s, p, (c["H"] * up + 2 * p - K) // s + 1, (c["W"] * up + 2 * p - K) // s + 1
 

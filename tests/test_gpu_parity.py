@@ -62,29 +62,6 @@ def _conv_ref(x, w, bias, stride, pad, up, silu):
     return F.silu(y) if silu else y
 
 
-CONV_CASES = [
-    # B, Cin, H, W, Cout, K, stride, pad, up, bias, silu
-    (2, 6, 20, 28, 8, 7, 1, 3, False, False, False),    # stem: Cin=6 scalar gather path
-    (2, 16, 12, 20, 24, 3, 1, 1, False, False, True),   # ResBlock conv
-    (1, 32, 9, 7, 16, 1, 1, 0, False, True, False),     # 1x1 with bias, ragged spatial size
-    (2, 8, 16, 24, 16, 4, 2, 1, False, True, False),    # Downsample 4x4 s2 p1
-    (2, 16, 6, 10, 8, 3, 1, 1, True, True, False),      # nearest x2 + 3x3
-    (1, 8, 10, 10, 3, 3, 1, 1, False, True, False),     # head: Cout=3
-    (1, 72, 5, 5, 136, 3, 1, 1, False, False, False),   # several K tiles / two N tiles
-]
-
-
-@pytest.mark.parametrize("case", CONV_CASES)
-def test_conv_simt_fp32(lib, scratch_ctx, case):
-    B, Cin, H, W, Cout, K, s, p, up, hb, silu = case
-    g = torch.Generator().manual_seed(sum(case[:6]))
-    x = torch.randn(B, Cin, H, W, generator=g)
-    w = torch.randn(Cout, Cin, K, K, generator=g) / (Cin * K * K) ** 0.5
-    b = torch.randn(Cout, generator=g) if hb else None
-    y = _conv2d(lib, scratch_ctx, 0, x, w, b, s, p, up, silu)
-    assert _maxdiff(y, _conv_ref(x, w, b, s, p, up, silu)) < 2e-5  # fp32, summation order only
-
-
 def test_sde_steps_bitexact(lib, golden):
     """Fused update kernel vs the reference's own step outputs: same op order, no FMA contraction."""
     dev = _dev()
