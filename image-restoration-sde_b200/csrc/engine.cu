@@ -47,7 +47,7 @@ struct RunCfg {  // per-invocation pointers read by the op closures at launch ti
 };
 
 struct Plan;
-typedef std::function<void(Plan*, cudaStream_t)> Op;
+typedef std::function<int(Plan*, cudaStream_t)> Op;  // enqueues the op's kernels, returns how many it launched
 enum { CAT_TC = 0, CAT_SIMT, CAT_LN, CAT_ATTN, CAT_MISC, CAT_UPDATE, CAT_COUNT };
 struct OpRec {
   int cat;
@@ -381,9 +381,14 @@ std::vector<ResBlockInfo> resblocks(const irsde_config& c, const std::vector<int
   return v;
 }
 
+// How irsde_finalize_weights packs a parameter: RAW stays fp32 as loaded (vectors, Linear matrices, gains, and the NAFBlock's
+// beta / gamma, depthwise and SCA weights, which their kernels read raw); TAPS is a conv weight over its own taps; UP is the
+// 3x3 conv of an Upsample, run as four 2x2 phases over the low-resolution input (nearest x2 + 3x3).
+enum Pack { PACK_RAW, PACK_TAPS, PACK_UP };
 struct ParamSpec {
   std::string name;
   std::vector<int64_t> shape;
+  Pack pack = PACK_RAW;
 };
 
 // NAFBlocks of ConditionalNAFNet in a fixed order (prefix, channels)   DenoisingNAFNet_arch.py:111-141
@@ -415,9 +420,9 @@ std::vector<ParamSpec> naf_param_specs(const NafCfg& n, int variant) {
   v.push_back({"time_mlp.1.bias", {2 * td}});
   v.push_back({"time_mlp.3.weight", {td, td}});
   v.push_back({"time_mlp.3.bias", {td}});
-  v.push_back({"intro.weight", {w, variant == IRSDE_NET_CONDITIONAL ? 2 * ic : ic, 3, 3}});
+  v.push_back({"intro.weight", {w, variant == IRSDE_NET_CONDITIONAL ? 2 * ic : ic, 3, 3}, PACK_TAPS});
   v.push_back({"intro.bias", {w}});
-  v.push_back({"ending.weight", {ic, w, 3, 3}});
+  v.push_back({"ending.weight", {ic, w, 3, 3}, PACK_TAPS});
   v.push_back({"ending.bias", {ic}});
   for (auto& blk : naf_blocks(n)) {
     int64_t c = blk.c;
@@ -426,17 +431,17 @@ std::vector<ParamSpec> naf_param_specs(const NafCfg& n, int variant) {
     v.push_back({p + "gamma", {1, c, 1, 1}});
     v.push_back({p + "mlp.1.weight", {4 * c, td / 2}});
     v.push_back({p + "mlp.1.bias", {4 * c}});
-    v.push_back({p + "conv1.weight", {2 * c, c, 1, 1}});
+    v.push_back({p + "conv1.weight", {2 * c, c, 1, 1}, PACK_TAPS});
     v.push_back({p + "conv1.bias", {2 * c}});
     v.push_back({p + "conv2.weight", {2 * c, 1, 3, 3}});
     v.push_back({p + "conv2.bias", {2 * c}});
-    v.push_back({p + "conv3.weight", {c, c, 1, 1}});
+    v.push_back({p + "conv3.weight", {c, c, 1, 1}, PACK_TAPS});
     v.push_back({p + "conv3.bias", {c}});
     v.push_back({p + "sca.1.weight", {c, c, 1, 1}});
     v.push_back({p + "sca.1.bias", {c}});
-    v.push_back({p + "conv4.weight", {2 * c, c, 1, 1}});
+    v.push_back({p + "conv4.weight", {2 * c, c, 1, 1}, PACK_TAPS});
     v.push_back({p + "conv4.bias", {2 * c}});
-    v.push_back({p + "conv5.weight", {c, c, 1, 1}});
+    v.push_back({p + "conv5.weight", {c, c, 1, 1}, PACK_TAPS});
     v.push_back({p + "conv5.bias", {c}});
     v.push_back({p + "norm1.g", {1, c, 1, 1}});
     v.push_back({p + "norm2.g", {1, c, 1, 1}});
@@ -445,13 +450,13 @@ std::vector<ParamSpec> naf_param_specs(const NafCfg& n, int variant) {
   int64_t chan = w << n.n_enc;
   for (int i = 0; i < n.n_dec; ++i) {
     snprintf(b, sizeof b, "ups.%d.0.weight", i);
-    v.push_back({b, {chan * 2, chan, 1, 1}});
+    v.push_back({b, {chan * 2, chan, 1, 1}, PACK_TAPS});
     chan /= 2;
   }
   chan = w;
   for (int i = 0; i < n.n_enc; ++i) {
     snprintf(b, sizeof b, "downs.%d.", i);
-    v.push_back({std::string(b) + "weight", {chan * 2, chan, 2, 2}});
+    v.push_back({std::string(b) + "weight", {chan * 2, chan, 2, 2}, PACK_TAPS});
     v.push_back({std::string(b) + "bias", {chan * 2}});
     chan *= 2;
   }
@@ -461,7 +466,7 @@ std::vector<ParamSpec> param_specs(const irsde_config& c, const std::vector<int>
   std::vector<ParamSpec> v;
   int64_t nf = c.nf, td = 4 * nf;
   int64_t cin0 = c.variant == IRSDE_NET_CONDITIONAL ? 2 * c.in_nc : c.in_nc;
-  v.push_back({"init_conv.weight", {nf, cin0, 7, 7}});
+  v.push_back({"init_conv.weight", {nf, cin0, 7, 7}, PACK_TAPS});
   v.push_back({"time_mlp.1.weight", {td, nf}});
   v.push_back({"time_mlp.1.bias", {td}});
   v.push_back({"time_mlp.3.weight", {td, td}});
@@ -469,17 +474,17 @@ std::vector<ParamSpec> param_specs(const irsde_config& c, const std::vector<int>
   for (auto& rb : resblocks(c, D)) {
     v.push_back({rb.pre + "mlp.1.weight", {2 * rb.cout, td}});
     v.push_back({rb.pre + "mlp.1.bias", {2 * rb.cout}});
-    v.push_back({rb.pre + "block1.proj.weight", {rb.cout, rb.cin, 3, 3}});
-    v.push_back({rb.pre + "block2.proj.weight", {rb.cout, rb.cout, 3, 3}});
-    if (rb.cin != rb.cout) v.push_back({rb.pre + "res_conv.weight", {rb.cout, rb.cin, 1, 1}});
+    v.push_back({rb.pre + "block1.proj.weight", {rb.cout, rb.cin, 3, 3}, PACK_TAPS});
+    v.push_back({rb.pre + "block2.proj.weight", {rb.cout, rb.cout, 3, 3}, PACK_TAPS});
+    if (rb.cin != rb.cout) v.push_back({rb.pre + "res_conv.weight", {rb.cout, rb.cin, 1, 1}, PACK_TAPS});
   }
   auto attn = [&](const std::string& pre, int64_t C, bool full) {
-    v.push_back({pre + "fn.fn.to_qkv.weight", {384, C, 1, 1}});
+    v.push_back({pre + "fn.fn.to_qkv.weight", {384, C, 1, 1}, PACK_TAPS});
     if (full) {
-      v.push_back({pre + "fn.fn.to_out.weight", {C, 128, 1, 1}});
+      v.push_back({pre + "fn.fn.to_out.weight", {C, 128, 1, 1}, PACK_TAPS});
       v.push_back({pre + "fn.fn.to_out.bias", {C}});
     } else {
-      v.push_back({pre + "fn.fn.to_out.0.weight", {C, 128, 1, 1}});
+      v.push_back({pre + "fn.fn.to_out.0.weight", {C, 128, 1, 1}, PACK_TAPS});
       v.push_back({pre + "fn.fn.to_out.0.bias", {C}});
       v.push_back({pre + "fn.fn.to_out.1.g", {1, C, 1, 1}});
     }
@@ -492,10 +497,10 @@ std::vector<ParamSpec> param_specs(const irsde_config& c, const std::vector<int>
     attn(b, di, false);
     snprintf(b, sizeof b, "downs.%d.3.", i);
     if (i != c.depth - 1) {
-      v.push_back({std::string(b) + "weight", {dout, di, 4, 4}});
+      v.push_back({std::string(b) + "weight", {dout, di, 4, 4}, PACK_TAPS});
       v.push_back({std::string(b) + "bias", {dout}});
     } else {
-      v.push_back({std::string(b) + "weight", {dout, di, 3, 3}});
+      v.push_back({std::string(b) + "weight", {dout, di, 3, 3}, PACK_TAPS});
     }
   }
   attn("mid_attn.", D[c.depth], c.variant == IRSDE_NET_DENOISING);
@@ -506,14 +511,14 @@ std::vector<ParamSpec> param_specs(const irsde_config& c, const std::vector<int>
     attn(b, dout, false);
     if (i != 0) {
       snprintf(b, sizeof b, "ups.%d.3.1.", j);
-      v.push_back({std::string(b) + "weight", {di, dout, 3, 3}});
+      v.push_back({std::string(b) + "weight", {di, dout, 3, 3}, PACK_UP});
       v.push_back({std::string(b) + "bias", {di}});
     } else {
       snprintf(b, sizeof b, "ups.%d.3.", j);
-      v.push_back({std::string(b) + "weight", {di, dout, 3, 3}});
+      v.push_back({std::string(b) + "weight", {di, dout, 3, 3}, PACK_TAPS});
     }
   }
-  v.push_back({"final_conv.weight", {c.out_nc, nf, 3, 3}});
+  v.push_back({"final_conv.weight", {c.out_nc, nf, 3, 3}, PACK_TAPS});
   v.push_back({"final_conv.bias", {c.out_nc}});
   return v;
 }
@@ -521,15 +526,15 @@ std::vector<ParamSpec> param_specs(const irsde_config& c, const std::vector<int>
 std::vector<ParamSpec> lat_param_specs(const LatCfg& L) {
   std::vector<ParamSpec> v;
   char b[64];
-  v.push_back({"init_conv.weight", {L.ch, L.in_ch, 3, 3}});
+  v.push_back({"init_conv.weight", {L.ch, L.in_ch, 3, 3}, PACK_TAPS});
   auto rb = [&](const std::string& pre, int64_t ci, int64_t co) {
-    v.push_back({pre + "block1.proj.weight", {co, ci, 3, 3}});
-    v.push_back({pre + "block2.proj.weight", {co, co, 3, 3}});
-    if (ci != co) v.push_back({pre + "res_conv.weight", {co, ci, 1, 1}});
+    v.push_back({pre + "block1.proj.weight", {co, ci, 3, 3}, PACK_TAPS});
+    v.push_back({pre + "block2.proj.weight", {co, co, 3, 3}, PACK_TAPS});
+    if (ci != co) v.push_back({pre + "res_conv.weight", {co, ci, 1, 1}, PACK_TAPS});
   };
   auto la = [&](const std::string& pre, int64_t C) {
-    v.push_back({pre + "fn.fn.to_qkv.weight", {384, C, 1, 1}});
-    v.push_back({pre + "fn.fn.to_out.0.weight", {C, 128, 1, 1}});
+    v.push_back({pre + "fn.fn.to_qkv.weight", {384, C, 1, 1}, PACK_TAPS});
+    v.push_back({pre + "fn.fn.to_out.0.weight", {C, 128, 1, 1}, PACK_TAPS});
     v.push_back({pre + "fn.fn.to_out.0.bias", {C}});
     v.push_back({pre + "fn.fn.to_out.1.g", {1, C, 1, 1}});
     v.push_back({pre + "fn.norm.g", {1, C, 1, 1}});
@@ -542,10 +547,10 @@ std::vector<ParamSpec> lat_param_specs(const LatCfg& L) {
     rb(pre + "1.", di, di);
     if (i == L.depth - 1) la(pre + "2.", di);
     if (i != L.depth - 1) {
-      v.push_back({pre + "3.weight", {dout, di, 4, 4}});
+      v.push_back({pre + "3.weight", {dout, di, 4, 4}, PACK_TAPS});
       v.push_back({pre + "3.bias", {dout}});
     } else {
-      v.push_back({pre + "3.weight", {dout, di, 3, 3}});
+      v.push_back({pre + "3.weight", {dout, di, 3, 3}, PACK_TAPS});
     }
   }
   for (int j = 0; j < L.depth; ++j) {
@@ -557,18 +562,47 @@ std::vector<ParamSpec> lat_param_specs(const LatCfg& L) {
     rb(pre + "1.", dout + di, dout);
     if (i == L.depth - 1) la(pre + "2.", dout);
     if (i != 0) {
-      v.push_back({pre + "3.1.weight", {di, dout, 3, 3}});
+      v.push_back({pre + "3.1.weight", {di, dout, 3, 3}, PACK_UP});
       v.push_back({pre + "3.1.bias", {di}});
     } else {
-      v.push_back({pre + "3.weight", {di, dout, 3, 3}});
+      v.push_back({pre + "3.weight", {di, dout, 3, 3}, PACK_TAPS});
     }
   }
   int64_t mid = (int64_t)L.ch * L.mult[L.depth];
-  v.push_back({"latent_conv.weight", {L.embed, mid, 1, 1}});
-  v.push_back({"post_latent_conv.weight", {mid, L.embed, 1, 1}});
-  v.push_back({"final_conv.weight", {L.out_ch, L.ch, 3, 3}});
+  v.push_back({"latent_conv.weight", {L.embed, mid, 1, 1}, PACK_TAPS});
+  v.push_back({"post_latent_conv.weight", {mid, L.embed, 1, 1}, PACK_TAPS});
+  v.push_back({"final_conv.weight", {L.out_ch, L.ch, 3, 3}, PACK_TAPS});
   v.push_back({"final_conv.bias", {L.out_ch}});
   return v;
+}
+
+// Which of the tap-GEMM's conv shapes (tap_table) a conv is: 3x3/1 pad 1 (also after nearest x2), 1x1, 4x4/2 pad 1 or 2x2/2
+// pad 0 over an even H x W, or the 7x7/1 pad 3 stem.  The plan builder and each standalone entry apply their own engine
+// rules on top.
+struct ConvShape {
+  bool k3, k1, k4, k2, k7;
+};
+ConvShape conv_shape(int KH, int KW, int stride, int pad, int up, int H, int W) {
+  const bool even = up == 1 && H % 2 == 0 && W % 2 == 0;
+  return ConvShape{KH == 3 && KW == 3 && stride == 1 && pad == 1, KH == 1 && KW == 1 && stride == 1 && pad == 0 && up == 1,
+                   KH == 4 && KW == 4 && stride == 2 && pad == 1 && even, KH == 2 && KW == 2 && stride == 2 && pad == 0 && even,
+                   KH == 7 && KW == 7 && stride == 1 && pad == 3 && up == 1};
+}
+ConvGeom conv_geom(int B, int Cin, int H, int W, int Cout, int KH, int KW, int stride, int pad, int up) {
+  return ConvGeom{B, H, W, Cin, up, KH, KW, stride, pad, (H * up + 2 * pad - KH) / stride + 1, (W * up + 2 * pad - KW) / stride + 1,
+                  Cout};
+}
+
+// The three networks run every level on the image padded to a multiple of 2^levels: level i is (Hp >> i) x (Wp >> i).  The
+// padded size is held in long long so that build_plan can check it against the kernels' limits for any int H, W.
+struct Levels {
+  long long Hp, Wp;
+  int h(int i) const { return (int)(Hp >> i); }
+  int w(int i) const { return (int)(Wp >> i); }
+};
+Levels level_sizes(long long H, long long W, int levels) {
+  const long long s = 1LL << levels;
+  return Levels{(H + s - 1) / s * s, (W + s - 1) / s * s};
 }
 
 // ---- plan builder ----------------------------------------------------------------------------------
@@ -580,9 +614,6 @@ struct Builder {
   std::string err;
   std::multimap<size_t, void*> free_tmp;
   std::map<void*, size_t> tmp_size;
-  const float* pending_mult = nullptr;  // per-output-channel multiplier for the NEXT conv() (NAFBlock beta / gamma)
-  int nchw_H = 0, nchw_W = 0;           // crop size of fp32 NCHW outputs (0 = the image size)
-  bool stem_padded = false;  // X0 lives in the zero-bordered [B][Hp+6][Wp+8][8] layout of the tensor-core stem
 
   T* alloc(long long elems) {
     void* p = dev_alloc(ctx, (size_t)elems * sizeof(T), &plan->allocs);
@@ -611,37 +642,44 @@ struct Builder {
 
   struct V { T* p; int pitch; int C; };  // channel-offset NHWC view
   static V view(T* base, int pitch, int off, int C) { return V{base + off, pitch, C}; }
+  // appends an op to the plan; label and bytes are what IRSDE_PROFILE_DUMP and irsde_profile_end_bytes report
+  void push_op(int cat, double flops, std::string label, double bytes, Op fn) {
+    plan->ops.push_back(OpRec{cat, flops, std::move(fn), std::move(label), bytes});
+  }
   void mark_out(V out, int H, int W) {  // the op just pushed writes this view (irsde_trace_forward)
     OpRec& r = plan->ops.back();
     r.out_p = out.p; r.out_pitch = out.pitch; r.out_C = out.C; r.out_H = H; r.out_W = W;
   }
 
-  // generic conv op. ss_block = ResBlock prefix whose (scale,shift) modulate the output ("" = none)
-  void conv(const std::string& wname, V in, int Hin, int Win, int K, int stride, int pad, int up, const char* bias,
-            const std::string& ss_block, int silu, const V* res, V out, int Cout, float** out_nchw_slot = nullptr,
-            int tc_flags = 0, const bf16* w_override = nullptr) {
-    size_t first = plan->ops.size();
-    conv_impl(wname, in, Hin, Win, K, stride, pad, up, bias, ss_block, silu, res, out, Cout, out_nchw_slot, tc_flags, w_override);
-    if (plan->ops.size() > first) {
-      OpRec& r = plan->ops.back();
-      char b[160];
-      int Ho = (Hin * up + 2 * pad - K) / stride + 1, Wo = (Win * up + 2 * pad - K) / stride + 1;
-      snprintf(b, sizeof b, "%s %dx%d k%d s%d up%d Cin%d Cout%d", wname.c_str(), Hin, Win, K, stride, up, in.C, Cout);
-      r.label = b;
-      if (!out_nchw_slot) { r.out_p = out.p; r.out_pitch = out.pitch; r.out_C = Cout; r.out_H = Ho; r.out_W = Wo; }
-      double esz = sizeof(T);
-      r.bytes = (double)plan->B * Hin * Win * in.C * esz + (double)plan->B * Ho * Wo * Cout * (out_nchw_slot ? 4.0 : esz) +
-                (double)K * K * in.C * Cout * esz + (res ? (double)plan->B * Ho * Wo * Cout * esz : 0.0);
-    }
-  }
-  void conv_impl(const std::string& wname, V in, int Hin, int Win, int K, int stride, int pad, int up, const char* bias,
-                 const std::string& ss_block, int silu, const V* res, V out, int Cout, float** out_nchw_slot, int tc_flags,
-                 const bf16* w_override) {
-    ConvGeom g;
-    g.B = plan->B; g.Hin = Hin; g.Win = Win; g.Cin = in.C; g.up = up; g.KH = K; g.KW = K; g.stride = stride; g.pad = pad;
-    g.Hout = (Hin * up + 2 * pad - K) / stride + 1;
-    g.Wout = (Win * up + 2 * pad - K) / stride + 1;
-    g.Cout = Cout;
+  // One conv of a network.  Every conv here pads to keep the size at stride 1 and to halve it exactly at stride 2, so its
+  // padding is (K - stride) / 2.
+  struct ConvSpec {
+    std::string w;              // weight name
+    V in;
+    int H = 0, W = 0;           // input size (before the nearest x2 upsample)
+    int K = 0, stride = 1, up = 1;
+    std::string bias;           // bias name, "" = none
+    std::string ss;             // ResBlock / NAFBlock prefix whose (scale, shift) modulate the output, "" = none
+    int silu = 0;
+    std::string mult;           // per-output-channel multiplier name (NAFBlock beta / gamma), "" = none
+    V res{};                    // residual added to the output (res.p == nullptr: none)
+    V out{};                    // output view; out.C is Cout
+    bool nchw = false;          // write fp32 NCHW to the run's output pointer instead of `out` (out.p null)
+    int crop_h = 0, crop_w = 0;  // crop of the NCHW output, 0 = the image size
+    bool stem_layout = false;   // `in` is the zero-bordered [B][Hp+6][Wp+8][8] layout of the tensor-core stem
+    int tc_flags = 0;           // TC_FLAG_* epilogues of the tap-GEMM (bf16 only)
+    const bf16* w_override = nullptr;  // tap-GEMM weights other than the packed `w` (per-image weights)
+  };
+  void conv(const ConvSpec& s) {
+    const V in = s.in, out = s.out;
+    const int K = s.K, stride = s.stride, up = s.up, Hin = s.H, Win = s.W, Cout = out.C, pad = (K - stride) / 2;
+    const ConvGeom g = conv_geom(plan->B, in.C, Hin, Win, Cout, K, K, stride, pad, up);
+    char b[160];
+    snprintf(b, sizeof b, "%s %dx%d k%d s%d up%d Cin%d Cout%d", s.w.c_str(), Hin, Win, K, stride, up, in.C, Cout);
+    const std::string label = b;
+    const double esz = sizeof(T);
+    const double bytes = (double)plan->B * Hin * Win * in.C * esz + (double)plan->B * g.Hout * g.Wout * Cout * (s.nchw ? 4.0 : esz) +
+                         (double)K * K * in.C * Cout * esz + (s.res.p ? (double)plan->B * g.Hout * g.Wout * Cout * esz : 0.0);
     double simt_flops = 2.0 * plan->B * g.Hout * g.Wout * (double)Cout * in.C * K * K;
     // the tensor-core engine runs nearest-x2 + 3x3 as four 2x2 phase convolutions (4 taps per output pixel) and the 7x7 stem
     // as 7 row taps of 8 pixels x 8 channels
@@ -650,33 +688,31 @@ struct Builder {
                                           : simt_flops;
     Epilogue ep;
     memset(&ep, 0, sizeof ep);
-    ep.bias = bias ? fw(bias) : nullptr;
-    ep.mult_vec = pending_mult;
-    pending_mult = nullptr;
-    ep.silu = silu;
+    ep.bias = s.bias.empty() ? nullptr : fw(s.bias);
+    ep.mult_vec = s.mult.empty() ? nullptr : fw(s.mult);
+    ep.silu = s.silu;
     ep.ss_S = ctx->S;
-    bool use_ss = !ss_block.empty();
-    if (use_ss && ep.mult_vec) { ok = false; err = "time modulation and mult_vec cannot be combined: " + wname; return; }
-    ep.ss_off = use_ss ? ctx->ss_off[ss_block] : 0;
-    if (res) { ep.res = res->p; ep.res_pitch = res->pitch; }
-    irsde_ctx* c = ctx;
-    bool nchw = out_nchw_slot != nullptr;
-    const int cH = nchw_H ? nchw_H : plan->H, cW = nchw_W ? nchw_W : plan->W;  // crop of the fp32 NCHW output
+    const bool use_ss = !s.ss.empty();
+    if (use_ss && ep.mult_vec) { ok = false; err = "time modulation and mult_vec cannot be combined: " + s.w; return; }
+    ep.ss_off = use_ss ? ctx->ss_off[s.ss] : 0;
+    if (s.res.p) { ep.res = s.res.p; ep.res_pitch = s.res.pitch; }
+    const bool nchw = s.nchw;
+    const int cH = s.crop_h ? s.crop_h : plan->H, cW = s.crop_w ? s.crop_w : plan->W;
     constexpr bool f32 = std::is_same<T, float>::value;  // fp32x3 engine: tf32 hi/lo split operands
     constexpr int al = f32 ? 4 : 8;                       // elements per 16 bytes
-    const bool stem = !f32 && stem_padded && K == 7 && Cout % al == 0 && out.pitch % al == 0;
-    bool shape_ok = (K == 3 && stride == 1 && pad == 1) || (K == 1 && stride == 1 && pad == 0 && up == 1) ||
-                    (K == 4 && stride == 2 && pad == 1 && up == 1 && Hin % 2 == 0 && Win % 2 == 0) ||
-                    (K == 2 && stride == 2 && pad == 0 && up == 1 && Hin % 2 == 0 && Win % 2 == 0);
-    shape_ok = shape_ok && in.C % al == 0 && in.pitch % al == 0 &&
-               (nchw ? (K == 3 && up == 1) : (Cout % al == 0 && out.pitch % al == 0));
+    const ConvShape cs = conv_shape(K, K, stride, pad, up, Hin, Win);
+    const bool out_aligned = Cout % al == 0 && out.pitch % al == 0;
+    const bool stem = !f32 && s.stem_layout && cs.k7 && out_aligned;
+    const bool taps = (cs.k3 || cs.k1 || cs.k4 || cs.k2) && in.C % al == 0 && in.pitch % al == 0 &&
+                      (nchw ? cs.k3 && up == 1 : out_aligned);
     // fused-attention flags and per-image weights are bf16-only epilogues
-    const bool engine_on = f32 ? ctx->use_tc3 && !tc_flags && !w_override && (((uintptr_t)in.p) & 15) == 0 : ctx->use_tc;
-    if (engine_on && (stem || shape_ok)) {
+    const bool engine_on =
+        f32 ? ctx->use_tc3 && !s.tc_flags && !s.w_override && (((uintptr_t)in.p) & 15) == 0 : ctx->use_tc;
+    if (engine_on && (stem || taps)) {
       const T* wt;
-      if constexpr (f32) wt = ctx->w_tc3[wname];
-      else wt = w_override ? w_override : ctx->w_tc[wname];
-      if (!wt) { ok = false; err = (f32 ? "unpacked fp32x3 weight " : "unpacked tc weight ") + wname; return; }
+      if constexpr (f32) wt = ctx->w_tc3[s.w];
+      else wt = s.w_override ? s.w_override : ctx->w_tc[s.w];
+      if (!wt) { ok = false; err = (f32 ? "unpacked fp32x3 weight " : "unpacked tc weight ") + s.w; return; }
       const TapTable t = tap_table(K, up);
       const int Ha = t.s2d() ? Hin / 2 : Hin, Wa = t.s2d() ? Win / 2 : Win;
       const T* a = in.p;
@@ -684,10 +720,10 @@ struct Builder {
       if (t.s2d()) {
         T* s2d = tmp((long long)plan->B * Hin * Win * in.C);
         int Bc = plan->B, Cc = in.C;
-        plan->ops.push_back(OpRec{CAT_MISC, 0.0, [=](Plan*, cudaStream_t st) {
+        push_op(CAT_MISC, 0.0, "", 0.0, [=](Plan*, cudaStream_t st) {
           launch_space_to_depth<T>(in.p, in.pitch, s2d, Bc, Hin, Win, Cc, st);
-          c->launches++;
-        }});
+          return 1;
+        });
         a = s2d; a_pitch = in.C;
         release(s2d);  // safe: stream order; the next tmp user runs after this conv
       }
@@ -696,52 +732,51 @@ struct Builder {
         const long long npix_a = (long long)t.planes * plan->B * Ha * Wa;
         float* split = tmp(2 * npix_a * in.C);
         int Cc = in.C;
-        plan->ops.push_back(OpRec{CAT_MISC, 0.0, [=](Plan*, cudaStream_t st) {
+        push_op(CAT_MISC, 0.0, s.w + " tf32 hi/lo split of the input", 3.0 * npix_a * in.C * 4.0, [=](Plan*, cudaStream_t st) {
           launch_split_tf32(a, a_pitch, split, npix_a, Cc, st);
-          c->launches++;
-        }});
-        plan->ops.back().label = wname + " tf32 hi/lo split of the input";
-        plan->ops.back().bytes = 3.0 * npix_a * in.C * 4.0;
+          return 1;
+        });
         a = split; a_pitch = in.C;
         release(split);  // safe: stream order, as for s2d
       }
       std::string terr;
       TcConvDesc* d = tc_conv_create(a, a_pitch, plan->B, Ha, Wa, in.C, t.planes, wt, Cout, t.ntaps, t.taps, t.nph, ep, out.p,
-                                     out.pitch, g.Hout, g.Wout, &terr, tc_flags);
-      if (!d) { ok = false; err = "tc_conv_create(" + wname + "): " + terr; return; }
+                                     out.pitch, g.Hout, g.Wout, &terr, s.tc_flags);
+      if (!d) { ok = false; err = "tc_conv_create(" + s.w + "): " + terr; return; }
       plan->tc_descs.push_back(d);
-      plan->ops.push_back(OpRec{CAT_TC, tc_flops, [=](Plan* p, cudaStream_t st) {
+      push_op(CAT_TC, tc_flops, label, bytes, [=](Plan* p, cudaStream_t st) {
         if (use_ss) tc_conv_set_runtime(d, p->cur.ss, p->cur.t_ptr, p->cur.ss_img_stride);
         if (nchw) tc_conv_set_out_nchw(d, p->cur.out, cH, cW);
         tc_conv_launch(d, st);
-        c->launches++;
-      }});
-      return;
+        return 1;
+      });
+    } else {
+      if (s.tc_flags || s.w_override) { ok = false; err = "fused attention conv needs the tensor-core engine: " + s.w; return; }
+      const float* w = ctx->w_simt[s.w];
+      if (!w) { ok = false; err = "unpacked weight " + s.w; return; }
+      push_op(CAT_SIMT, simt_flops, label, bytes, [=](Plan* p, cudaStream_t st) {
+        Epilogue e = ep;
+        if (use_ss) { e.ss = p->cur.ss; e.t_ptr = p->cur.t_ptr; e.ss_img_stride = p->cur.ss_img_stride; }
+        launch_conv_simt<T>(g, in.p, in.pitch, w, e, out.p, out.pitch, nchw ? p->cur.out : nullptr, cH, cW, st);
+        return 1;
+      });
     }
-    if (tc_flags || w_override) { ok = false; err = "fused attention conv needs the tensor-core engine: " + wname; return; }
-    const float* w = ctx->w_simt[wname];
-    if (!w) { ok = false; err = "unpacked weight " + wname; return; }
-    plan->ops.push_back(OpRec{CAT_SIMT, simt_flops, [=](Plan* p, cudaStream_t st) {
-      Epilogue e = ep;
-      if (use_ss) { e.ss = p->cur.ss; e.t_ptr = p->cur.t_ptr; e.ss_img_stride = p->cur.ss_img_stride; }
-      launch_conv_simt<T>(g, in.p, in.pitch, w, e, out.p, out.pitch, nchw ? p->cur.out : nullptr, cH, cW, st);
-      c->launches++;
-    }});
+    if (!nchw) mark_out(out, g.Hout, g.Wout);
   }
 
   void resblock(const std::string& pre, V in, int Cout, V out, int H, int W, bool time_mod = true) {
     long long npix = (long long)plan->B * H * W;
     T* h1 = tmp(npix * Cout);
     V vh1{h1, Cout, Cout};
-    conv(pre + "block1.proj.weight", in, H, W, 3, 1, 1, 1, nullptr, time_mod ? pre : std::string(), 1, nullptr, vh1, Cout);
+    conv({.w = pre + "block1.proj.weight", .in = in, .H = H, .W = W, .K = 3, .ss = time_mod ? pre : "", .silu = 1, .out = vh1});
     V res = in;
     T* r = nullptr;
     if (in.C != Cout) {
       r = tmp(npix * Cout);
       res = V{r, Cout, Cout};
-      conv(pre + "res_conv.weight", in, H, W, 1, 1, 0, 1, nullptr, "", 0, nullptr, res, Cout);
+      conv({.w = pre + "res_conv.weight", .in = in, .H = H, .W = W, .K = 1, .out = res});
     }
-    conv(pre + "block2.proj.weight", vh1, H, W, 3, 1, 1, 1, nullptr, "", 1, &res, out, Cout);
+    conv({.w = pre + "block2.proj.weight", .in = vh1, .H = H, .W = W, .K = 3, .silu = 1, .res = res, .out = out});
     release(h1);
     if (r) release(r);
   }
@@ -758,13 +793,10 @@ struct Builder {
     }
     T* xn = tmp(npix * C);
     float* g1 = fw(pre + "fn.norm.g");
-    irsde_ctx* c = ctx;
-    plan->ops.push_back(OpRec{CAT_LN, 0.0, [=](Plan*, cudaStream_t st) {
+    push_op(CAT_LN, 0.0, pre + "norm", 2.0 * npix * C * sizeof(T), [=](Plan*, cudaStream_t st) {
       launch_layernorm<T>(in.p, in.pitch, g1, nullptr, 0, xn, C, npix, C, st);
-      c->launches++;
-    }});
-    plan->ops.back().label = pre + "norm";
-    plan->ops.back().bytes = 2.0 * npix * C * sizeof(T);
+      return 1;
+    });
     mark_out(V{xn, C, C}, H, W);
     T* qkv = tmp(npix * 384);
     if constexpr (std::is_same<T, bf16>::value) {
@@ -772,35 +804,29 @@ struct Builder {
         // Fused LinearAttention: (1) the to_qkv GEMM epilogue applies softmax_d(q)*32^-.5 per head, (2) k,v -> ctx,
         // (3) ctx is folded into the to_out weights per image, (4) ONE per-image-weight 1x1 GEMM on q gives to_out's
         // output (module_util.py:163-178 with the two einsums + to_out conv re-associated), (5) LayerNorm + residual.
-        conv(pre + "fn.fn.to_qkv.weight", V{xn, C, C}, H, W, 1, 1, 0, 1, nullptr, "", 0, nullptr, V{qkv, 384, 384}, 384, nullptr,
-             TC_FLAG_QSOFTMAX);
+        conv({.w = pre + "fn.fn.to_qkv.weight", .in = V{xn, C, C}, .H = H, .W = W, .K = 1, .out = V{qkv, 384, 384},
+              .tc_flags = TC_FLAG_QSOFTMAX});
         release(xn);
         if (!linattn_views_ok(qkv, 384, nullptr, 0, sizeof(T))) { ok = false; err = "linear attention: qkv view not 16-byte aligned"; }
-        plan->ops.push_back(OpRec{CAT_ATTN, 0.0, [=](Plan*, cudaStream_t st) {
+        push_op(CAT_ATTN, 0.0, pre + "linattn kv->ctx (2 kernels)", (double)npix * 256 * sizeof(T), [=](Plan*, cudaStream_t st) {
           launch_linattn_ctx<T>(qkv, 384, la_partial, la_ctx, B, N, st);
-          c->launches += 2;
-        }});
-        plan->ops.back().label = pre + "linattn kv->ctx (2 kernels)";
-        plan->ops.back().bytes = (double)npix * 256 * sizeof(T);
+          return 2;
+        });
         bf16* Mb = tmp((long long)B * C * 128);
         float* wout = fw(pre + "fn.fn.to_out.0.weight");
         // (combine + fold in ONE kernel gives 8-64 blocks of latency-bound work instead of 32 + 256..4096: kept as two launches)
-        plan->ops.push_back(OpRec{CAT_ATTN, 0.0, [=](Plan*, cudaStream_t st) {
+        push_op(CAT_ATTN, 0.0, pre + "fold ctx into to_out", 0.0, [=](Plan*, cudaStream_t st) {
           launch_la_fold(la_ctx, wout, Mb, B, C, st);
-          c->launches++;
-        }});
-        plan->ops.back().label = pre + "fold ctx into to_out";
+          return 1;
+        });
         T* y = tmp(npix * C);
-        std::string bn = pre + "fn.fn.to_out.0.bias";
-        conv(pre + "fn.fn.to_out.0.weight", V{qkv, 384, 128}, H, W, 1, 1, 0, 1, bn.c_str(), "", 0, nullptr, V{y, C, C}, C, nullptr,
-             TC_FLAG_W_PER_IMAGE, Mb);
+        conv({.w = pre + "fn.fn.to_out.0.weight", .in = V{qkv, 384, 128}, .H = H, .W = W, .K = 1, .bias = pre + "fn.fn.to_out.0.bias",
+              .out = V{y, C, C}, .tc_flags = TC_FLAG_W_PER_IMAGE, .w_override = Mb});
         float* g2 = fw(pre + "fn.fn.to_out.1.g");
-        plan->ops.push_back(OpRec{CAT_LN, 0.0, [=](Plan*, cudaStream_t st) {
+        push_op(CAT_LN, 0.0, pre + "to_out.norm+res", 3.0 * npix * C * sizeof(T), [=](Plan*, cudaStream_t st) {
           launch_layernorm<T>(y, C, g2, in.p, in.pitch, out.p, out.pitch, npix, C, st);
-          c->launches++;
-        }});
-        plan->ops.back().label = pre + "to_out.norm+res";
-        plan->ops.back().bytes = 3.0 * npix * C * sizeof(T);
+          return 1;
+        });
         mark_out(out, H, W);
         release(y);
         release(Mb);
@@ -808,36 +834,31 @@ struct Builder {
         return;
       }
     }
-    conv(pre + "fn.fn.to_qkv.weight", V{xn, C, C}, H, W, 1, 1, 0, 1, nullptr, "", 0, nullptr, V{qkv, 384, 384}, 384);
+    conv({.w = pre + "fn.fn.to_qkv.weight", .in = V{xn, C, C}, .H = H, .W = W, .K = 1, .out = V{qkv, 384, 384}});
     release(xn);
     T* hid = tmp(npix * 128);
     if (full) {
-      plan->ops.push_back(OpRec{CAT_ATTN, 0.0, [=](Plan*, cudaStream_t st) {
+      push_op(CAT_ATTN, 0.0, pre + "full attention", 0.0, [=](Plan*, cudaStream_t st) {
         launch_fullattn<T>(qkv, 384, hid, 128, B, N, st);
-        c->launches++;
-      }});
-      plan->ops.back().label = pre + "full attention";
+        return 1;
+      });
       mark_out(V{hid, 128, 128}, H, W);
-      std::string bn = pre + "fn.fn.to_out.bias";
-      conv(pre + "fn.fn.to_out.weight", V{hid, 128, 128}, H, W, 1, 1, 0, 1, bn.c_str(), "", 0, &in, out, C);
+      conv({.w = pre + "fn.fn.to_out.weight", .in = V{hid, 128, 128}, .H = H, .W = W, .K = 1, .bias = pre + "fn.fn.to_out.bias",
+            .res = in, .out = out});
     } else {
       if (!linattn_views_ok(qkv, 384, hid, 128, sizeof(T))) { ok = false; err = "linear attention: views not 16-byte aligned"; }
-      plan->ops.push_back(OpRec{CAT_ATTN, 0.0, [=](Plan*, cudaStream_t st) {
+      push_op(CAT_ATTN, 0.0, pre + "linattn(3 kernels)", (double)npix * (384 + 128) * sizeof(T), [=](Plan*, cudaStream_t st) {
         launch_linattn<T>(qkv, 384, la_partial, la_ctx, hid, 128, B, N, st);
-        c->launches += 3;
-      }});
-      plan->ops.back().label = pre + "linattn(3 kernels)";
-      plan->ops.back().bytes = (double)npix * (384 + 128) * sizeof(T);
+        return 3;
+      });
       T* y = tmp(npix * C);
-      std::string bn = pre + "fn.fn.to_out.0.bias";
-      conv(pre + "fn.fn.to_out.0.weight", V{hid, 128, 128}, H, W, 1, 1, 0, 1, bn.c_str(), "", 0, nullptr, V{y, C, C}, C);
+      conv({.w = pre + "fn.fn.to_out.0.weight", .in = V{hid, 128, 128}, .H = H, .W = W, .K = 1, .bias = pre + "fn.fn.to_out.0.bias",
+            .out = V{y, C, C}});
       float* g2 = fw(pre + "fn.fn.to_out.1.g");
-      plan->ops.push_back(OpRec{CAT_LN, 0.0, [=](Plan*, cudaStream_t st) {
+      push_op(CAT_LN, 0.0, pre + "to_out.norm+res", 3.0 * npix * C * sizeof(T), [=](Plan*, cudaStream_t st) {
         launch_layernorm<T>(y, C, g2, in.p, in.pitch, out.p, out.pitch, npix, C, st);
-        c->launches++;
-      }});
-      plan->ops.back().label = pre + "to_out.norm+res";
-      plan->ops.back().bytes = 3.0 * npix * C * sizeof(T);
+        return 1;
+      });
       mark_out(out, H, W);
       release(y);
     }
@@ -851,36 +872,29 @@ struct Builder {
   void linattn_fused(const std::string& pre, V in, V out, int H, int W, float* la_partial, float* la_ctx) {
     const int C = in.C, B = plan->B, N = H * W;
     const long long npix = (long long)B * N;
-    irsde_ctx* c = ctx;
     const bf16* wqkv = ctx->w_tc[pre + "fn.fn.to_qkv.weight"];
     if (!wqkv) { ok = false; err = "unpacked tc weight " + pre + "fn.fn.to_qkv.weight"; return; }
     float* g1 = fw(pre + "fn.norm.g");
-    plan->ops.push_back(OpRec{CAT_ATTN, 0.0, [=](Plan*, cudaStream_t st) {
+    push_op(CAT_ATTN, 0.0, pre + "norm+to_qkv k,v+linattn kv (fused)", (double)npix * C * sizeof(T), [=](Plan*, cudaStream_t st) {
       launch_la_kv_ln(in.p, in.pitch, g1, wqkv + 128 * C, la_partial, B, N, C, nullptr, st);
-      c->launches++;
-    }});
-    plan->ops.back().label = pre + "norm+to_qkv k,v+linattn kv (fused)";
-    plan->ops.back().bytes = (double)npix * C * sizeof(T);
-    plan->ops.push_back(OpRec{CAT_ATTN, 0.0, [=](Plan*, cudaStream_t st) {
+      return 1;
+    });
+    push_op(CAT_ATTN, 0.0, pre + "linattn combine", 0.0, [=](Plan*, cudaStream_t st) {
       launch_la_combine(la_partial, la_ctx, B, N, st);
-      c->launches++;
-    }});
-    plan->ops.back().label = pre + "linattn combine";
+      return 1;
+    });
     bf16* Mb = tmp((long long)B * C * 128);
     float* wout = fw(pre + "fn.fn.to_out.0.weight");
-    plan->ops.push_back(OpRec{CAT_ATTN, 0.0, [=](Plan*, cudaStream_t st) {
+    push_op(CAT_ATTN, 0.0, pre + "fold ctx into to_out", 0.0, [=](Plan*, cudaStream_t st) {
       launch_la_fold(la_ctx, wout, Mb, B, C, st);
-      c->launches++;
-    }});
-    plan->ops.back().label = pre + "fold ctx into to_out";
+      return 1;
+    });
     float* bout = fw(pre + "fn.fn.to_out.0.bias");
     float* g2 = fw(pre + "fn.fn.to_out.1.g");
-    plan->ops.push_back(OpRec{CAT_ATTN, 0.0, [=](Plan*, cudaStream_t st) {
+    push_op(CAT_ATTN, 0.0, pre + "to_out.norm+res", 2.0 * npix * C * sizeof(T), [=](Plan*, cudaStream_t st) {
       launch_la_out_ln(in.p, in.pitch, g1, wqkv, Mb, bout, g2, out.p, out.pitch, B, N, C, st);
-      c->launches++;
-    }});
-    plan->ops.back().label = pre + "to_out.norm+res";
-    plan->ops.back().bytes = 2.0 * npix * C * sizeof(T);
+      return 1;
+    });
     mark_out(out, H, W);
     release(Mb);
   }
@@ -890,32 +904,28 @@ struct Builder {
   void build_latent() {
     const LatCfg& L = ctx->lat;
     const int B = plan->B, depth = L.depth;
-    const int s = 1 << depth;
-    plan->Hp = plan->H + (s - plan->H % s) % s;
-    plan->Wp = plan->W + (s - plan->W % s) % s;
-    std::vector<int> hs(depth), ws(depth);
-    hs[0] = plan->Hp; ws[0] = plan->Wp;
-    for (int i = 1; i < depth; ++i) { hs[i] = hs[i - 1] / 2; ws[i] = ws[i - 1] / 2; }
-    plan->lat_h = hs[depth - 1]; plan->lat_w = ws[depth - 1];
-    float* la_partial = (float*)dev_alloc(ctx, linattn_partial_floats(B, hs[depth - 1] * ws[depth - 1]) * sizeof(float), &plan->allocs);
+    const Levels lv = level_sizes(plan->H, plan->W, depth);
+    plan->Hp = lv.h(0);
+    plan->Wp = lv.w(0);
+    plan->lat_h = lv.h(depth - 1); plan->lat_w = lv.w(depth - 1);
+    float* la_partial = (float*)dev_alloc(ctx, linattn_partial_floats(B, plan->lat_h * plan->lat_w) * sizeof(float), &plan->allocs);
     float* la_ctx = (float*)dev_alloc(ctx, (size_t)B * 4096 * sizeof(float), &plan->allocs);
     if (!la_partial || !la_ctx) { ok = false; err = "cudaMalloc failed"; return; }
     const int C0 = L.in_ch, pitch0 = (C0 + 7) / 8 * 8;
-    const long long np0 = (long long)B * hs[0] * ws[0];
+    const long long np0 = (long long)B * plan->Hp * plan->Wp;
     T* X0 = alloc(np0 * pitch0);
     T* H0 = alloc(np0 * L.ch);  // h[0] = init_conv output, added back before final_conv
     int in_ch = L.in_ch, Hh = plan->H, Ww = plan->W, Hp = plan->Hp, Wp = plan->Wp;
-    irsde_ctx* cx = ctx;
-    plan->ops.push_back(OpRec{CAT_MISC, 0.0, [=](Plan* p, cudaStream_t st) {
+    push_op(CAT_MISC, 0.0, "", 0.0, [=](Plan* p, cudaStream_t st) {
       launch_prep_input<T>(p->cur.x, nullptr, X0, B, in_ch, Hh, Ww, Hp, Wp, pitch0, 0, st);  // reflect pad, no condition
-      cx->launches++;
-    }});
-    conv("init_conv.weight", V{X0, pitch0, C0}, hs[0], ws[0], 3, 1, 1, 1, nullptr, "", 0, nullptr, V{H0, L.ch, L.ch}, L.ch);
+      return 1;
+    });
+    conv({.w = "init_conv.weight", .in = V{X0, pitch0, C0}, .H = Hp, .W = Wp, .K = 3, .out = V{H0, L.ch, L.ch}});
     V cur{H0, L.ch, L.ch};
     std::vector<T*> U1(depth), U2(depth);
     char nb[64];
     for (int i = 0; i < depth; ++i) {
-      const int di = L.ch * L.mult[i], dout = L.ch * L.mult[i + 1], H = hs[i], W = ws[i];
+      const int di = L.ch * L.mult[i], dout = L.ch * L.mult[i + 1], H = lv.h(i), W = lv.w(i);
       const long long npix = (long long)B * H * W;
       U1[i] = alloc(npix * (dout + di));
       U2[i] = alloc(npix * (dout + di));
@@ -929,22 +939,18 @@ struct Builder {
         attention(pre + "2.", V{ta, di, di}, s1, H, W, false, la_partial, la_ctx);
         release(ta);
         T* xm = alloc(npix * dout);
-        conv(pre + "3.weight", s1, H, W, 3, 1, 1, 1, nullptr, "", 0, nullptr, V{xm, dout, dout}, dout);
+        conv({.w = pre + "3.weight", .in = s1, .H = H, .W = W, .K = 3, .out = V{xm, dout, dout}});
         cur = V{xm, dout, dout};
       } else {
         resblock(pre + "1.", s2, di, s1, H, W, false);  // Identity attention: the skip is b2's output
-        T* xn = alloc((long long)B * hs[i + 1] * ws[i + 1] * dout);
-        std::string bn = pre + "3.bias";
-        conv(pre + "3.weight", s1, H, W, 4, 2, 1, 1, bn.c_str(), "", 0, nullptr, V{xn, dout, dout}, dout);
+        T* xn = alloc((long long)B * lv.h(i + 1) * lv.w(i + 1) * dout);
+        conv({.w = pre + "3.weight", .in = s1, .H = H, .W = W, .K = 4, .stride = 2, .bias = pre + "3.bias", .out = V{xn, dout, dout}});
         cur = V{xn, dout, dout};
       }
     }
-    {  // z = latent_conv(x): fp32 NCHW [B, embed, lat_h, lat_w] straight from the epilogue
-      float* dummy = nullptr;
-      nchw_H = plan->lat_h; nchw_W = plan->lat_w;
-      conv("latent_conv.weight", cur, plan->lat_h, plan->lat_w, 1, 1, 0, 1, nullptr, "", 0, nullptr, V{nullptr, 0, 0}, L.embed, &dummy);
-      nchw_H = nchw_W = 0;
-    }
+    // z = latent_conv(x): fp32 NCHW [B, embed, lat_h, lat_w] straight from the epilogue
+    conv({.w = "latent_conv.weight", .in = cur, .H = plan->lat_h, .W = plan->lat_w, .K = 1, .out = V{nullptr, 0, L.embed},
+          .nchw = true, .crop_h = plan->lat_h, .crop_w = plan->lat_w});
     // ----- decode half
     std::vector<OpRec> enc_ops;
     enc_ops.swap(plan->ops);
@@ -953,16 +959,16 @@ struct Builder {
     const int zp = (L.embed + 7) / 8 * 8;
     T* Z = alloc(npl * zp);
     int embed = L.embed, lh = plan->lat_h, lw = plan->lat_w;
-    plan->ops.push_back(OpRec{CAT_MISC, 0.0, [=](Plan* p, cudaStream_t st) {
+    push_op(CAT_MISC, 0.0, "", 0.0, [=](Plan* p, cudaStream_t st) {
       launch_nchw_to_nhwc<T>(p->cur.x, Z, B, embed, lh, lw, zp, st);
-      cx->launches++;
-    }});
+      return 1;
+    });
     {
       const int i = depth - 1, di = L.ch * L.mult[i];
-      conv("post_latent_conv.weight", V{Z, zp, L.embed}, lh, lw, 1, 1, 0, 1, nullptr, "", 0, nullptr, view(U1[i], mid + di, 0, mid), mid);
+      conv({.w = "post_latent_conv.weight", .in = V{Z, zp, L.embed}, .H = lh, .W = lw, .K = 1, .out = view(U1[i], mid + di, 0, mid)});
     }
     for (int j = 0; j < depth; ++j) {
-      const int i = depth - 1 - j, di = L.ch * L.mult[i], dout = L.ch * L.mult[i + 1], H = hs[i], W = ws[i];
+      const int i = depth - 1 - j, di = L.ch * L.mult[i], dout = L.ch * L.mult[i + 1], H = lv.h(i), W = lv.w(i);
       const long long npix = (long long)B * H * W;
       snprintf(nb, sizeof nb, "decoder.%d.", j);
       std::string pre = nb;
@@ -978,20 +984,19 @@ struct Builder {
       }
       if (i != 0) {
         const int dprev_total = L.ch * L.mult[i] + L.ch * L.mult[i - 1];  // concat width of level i-1: dout_{i-1} + di_{i-1}
-        std::string bn = pre + "3.1.bias";
-        conv(pre + "3.1.weight", xo, H, W, 3, 1, 1, 2, bn.c_str(), "", 0, nullptr, view(U1[i - 1], dprev_total, 0, di), di);
+        conv({.w = pre + "3.1.weight", .in = xo, .H = H, .W = W, .K = 3, .up = 2, .bias = pre + "3.1.bias",
+              .out = view(U1[i - 1], dprev_total, 0, di)});
       } else {
         T* xf = tmp(np0 * L.ch);
-        conv(pre + "3.weight", xo, H, W, 3, 1, 1, 1, nullptr, "", 0, nullptr, V{xf, L.ch, L.ch}, L.ch);
+        conv({.w = pre + "3.weight", .in = xo, .H = H, .W = W, .K = 3, .out = V{xf, L.ch, L.ch}});
         T* xs = tmp(np0 * L.ch);
         int chn = L.ch;
-        plan->ops.push_back(OpRec{CAT_MISC, 0.0, [=](Plan*, cudaStream_t st) {
+        push_op(CAT_MISC, 0.0, "", 0.0, [=](Plan*, cudaStream_t st) {
           launch_add<T>(xf, chn, H0, chn, xs, chn, np0, chn, st);   // x + h[0]
-          cx->launches++;
-        }});
-        float* dummy = nullptr;
-        conv("final_conv.weight", V{xs, L.ch, L.ch}, hs[0], ws[0], 3, 1, 1, 1, "final_conv.bias", "", 0, nullptr, V{nullptr, 0, 0},
-             L.out_ch, &dummy);
+          return 1;
+        });
+        conv({.w = "final_conv.weight", .in = V{xs, L.ch, L.ch}, .H = Hp, .W = Wp, .K = 3, .bias = "final_conv.bias",
+              .out = V{nullptr, 0, L.out_ch}, .nchw = true});
         release(xf);
         release(xs);
       }
@@ -1011,27 +1016,22 @@ struct Builder {
     long long npix = (long long)B * H * W;
     float* g = fw(gname);
     int base = ctx->ss_off[blk], S = ctx->S, ppi = H * W;
-    irsde_ctx* c = ctx;
-    plan->ops.push_back(OpRec{CAT_LN, 0.0, [=](Plan* p, cudaStream_t st) {
+    push_op(CAT_LN, 0.0, gname + " (LN+mod)", 2.0 * npix * C * sizeof(T), [=](Plan* p, cudaStream_t st) {
       LnMod m;
       m.ss = p->cur.ss; m.t_ptr = p->cur.t_ptr; m.S = S; m.off_scale = base + off_scale; m.off_shift = base + off_shift;
       m.img_stride = p->cur.ss_img_stride; m.pix_per_img = ppi;
       launch_layernorm<T>(in.p, in.pitch, g, nullptr, 0, out.p, out.pitch, npix, C, st, &m);
-      c->launches++;
-    }});
-    plan->ops.back().label = gname + " (LN+mod)";
-    plan->ops.back().bytes = 2.0 * npix * C * sizeof(T);
+      return 1;
+    });
   }
 
   void nafblock(const std::string& pre, V x, V out, int H, int W) {
     const int c = x.C, B = plan->B, N = H * W;
     const long long npix = (long long)B * N;
-    irsde_ctx* cx = ctx;
     T* t1 = tmp(npix * c);
     ln_mod(pre + "norm1.g", pre, c, 0, x, V{t1, c, c}, H, W);            // x * (scale_att + 1) + shift_att
     T* t2 = tmp(npix * 2 * c);
-    std::string b1 = pre + "conv1.bias";
-    conv(pre + "conv1.weight", V{t1, c, c}, H, W, 1, 1, 0, 1, b1.c_str(), "", 0, nullptr, V{t2, 2 * c, 2 * c}, 2 * c);
+    conv({.w = pre + "conv1.weight", .in = V{t1, c, c}, .H = H, .W = W, .K = 1, .bias = pre + "conv1.bias", .out = V{t2, 2 * c, 2 * c}});
     release(t1);
     T* g = tmp(npix * c);
     {
@@ -1039,38 +1039,31 @@ struct Builder {
       float* ws = fw(pre + "sca.1.weight"); float* bs = fw(pre + "sca.1.bias");
       float* partial = naf_partial; float* sca = naf_sca;
       const int nch = dwgate_chunks(H, W);
-      plan->ops.push_back(OpRec{CAT_MISC, 0.0, [=](Plan*, cudaStream_t st) {
+      push_op(CAT_MISC, 0.0, pre + "dw3x3+gate+sca", (double)npix * (2 * c + c + 2 * c) * sizeof(T), [=](Plan*, cudaStream_t st) {
         launch_dwgate<T>(t2, 2 * c, w2, bb2, g, c, partial, B, H, W, c, st);
         int nl = 0;
         launch_sca_scale<T>(partial, ws, bs, sca, g, c, B, c, nch, N, &nl, st);
-        cx->launches += 1 + nl;
-      }});
-      plan->ops.back().label = pre + "dw3x3+gate+sca";
-      plan->ops.back().bytes = (double)npix * (2 * c + c + 2 * c) * sizeof(T);
+        return 1 + nl;
+      });
     }
     release(t2);
     T* y = tmp(npix * c);
-    std::string b3 = pre + "conv3.bias";
-    pending_mult = fw(pre + "beta");
-    conv(pre + "conv3.weight", V{g, c, c}, H, W, 1, 1, 0, 1, b3.c_str(), "", 0, &x, V{y, c, c}, c);     // y = inp + conv3(.)*beta
+    conv({.w = pre + "conv3.weight", .in = V{g, c, c}, .H = H, .W = W, .K = 1, .bias = pre + "conv3.bias", .mult = pre + "beta",
+          .res = x, .out = V{y, c, c}});                                     // y = inp + conv3(.)*beta
     release(g);
     t1 = tmp(npix * c);
-    ln_mod(pre + "norm2.g", pre, 3 * c, 2 * c, V{y, c, c}, V{t1, c, c}, H, W);                          // * (scale_ffn+1) + shift_ffn
+    ln_mod(pre + "norm2.g", pre, 3 * c, 2 * c, V{y, c, c}, V{t1, c, c}, H, W);  // * (scale_ffn+1) + shift_ffn
     t2 = tmp(npix * 2 * c);
-    std::string b4 = pre + "conv4.bias";
-    conv(pre + "conv4.weight", V{t1, c, c}, H, W, 1, 1, 0, 1, b4.c_str(), "", 0, nullptr, V{t2, 2 * c, 2 * c}, 2 * c);
+    conv({.w = pre + "conv4.weight", .in = V{t1, c, c}, .H = H, .W = W, .K = 1, .bias = pre + "conv4.bias", .out = V{t2, 2 * c, 2 * c}});
     release(t1);
     g = tmp(npix * c);
-    plan->ops.push_back(OpRec{CAT_MISC, 0.0, [=](Plan*, cudaStream_t st) {
+    push_op(CAT_MISC, 0.0, pre + "simple_gate", 0.0, [=](Plan*, cudaStream_t st) {
       launch_simple_gate<T>(t2, 2 * c, g, c, npix, c, st);
-      cx->launches++;
-    }});
-    plan->ops.back().label = pre + "simple_gate";
+      return 1;
+    });
     release(t2);
-    std::string b5 = pre + "conv5.bias";
-    pending_mult = fw(pre + "gamma");
-    V vy{y, c, c};
-    conv(pre + "conv5.weight", V{g, c, c}, H, W, 1, 1, 0, 1, b5.c_str(), "", 0, &vy, out, c);           // out = y + conv5(.)*gamma
+    conv({.w = pre + "conv5.weight", .in = V{g, c, c}, .H = H, .W = W, .K = 1, .bias = pre + "conv5.bias", .mult = pre + "gamma",
+          .res = V{y, c, c}, .out = out});                                   // out = y + conv5(.)*gamma
     release(g);
     release(y);
   }
@@ -1078,16 +1071,13 @@ struct Builder {
   void build_naf() {
     const NafCfg& n = ctx->naf;
     const int B = plan->B, w = n.width, ic = n.img_channel;
-    const int s = 1 << n.n_enc;
-    plan->Hp = plan->H + (s - plan->H % s) % s;
-    plan->Wp = plan->W + (s - plan->W % s) % s;
-    std::vector<int> hs(n.n_enc + 1), ws(n.n_enc + 1);
-    hs[0] = plan->Hp; ws[0] = plan->Wp;
-    for (int i = 1; i <= n.n_enc; ++i) { hs[i] = hs[i - 1] / 2; ws[i] = ws[i - 1] / 2; }
+    const Levels lv = level_sizes(plan->H, plan->W, n.n_enc);
+    plan->Hp = lv.h(0);
+    plan->Wp = lv.w(0);
     size_t pmax = 0, cmax = 0;
     for (int i = 0; i <= n.n_enc; ++i) {
       size_t cc = (size_t)w << i;
-      pmax = std::max(pmax, (size_t)B * dwgate_chunks(hs[i], ws[i]) * cc);
+      pmax = std::max(pmax, (size_t)B * dwgate_chunks(lv.h(i), lv.w(i)) * cc);
       cmax = std::max(cmax, cc);
     }
     naf_partial = (float*)dev_alloc(ctx, pmax * sizeof(float), &plan->allocs);
@@ -1096,120 +1086,114 @@ struct Builder {
     // conditional: intro reads cat(x - cond, cond); denoising-sde: x alone (DenoisingNAFNet_arch.py:103,147-150)
     const int cond = ctx->cfg.variant == IRSDE_NET_CONDITIONAL ? 1 : 0;
     const int C0 = cond ? 2 * ic : ic, pitch0 = (C0 + 7) / 8 * 8;
-    const long long np0 = (long long)B * hs[0] * ws[0];
+    const long long np0 = (long long)B * plan->Hp * plan->Wp;
     T* X0 = alloc(np0 * pitch0);
     int Hh = plan->H, Ww = plan->W, Hp = plan->Hp, Wp = plan->Wp;
-    irsde_ctx* cx = ctx;
-    plan->ops.push_back(OpRec{CAT_MISC, 0.0, [=](Plan* p, cudaStream_t st) {
+    push_op(CAT_MISC, 0.0, "", 0.0, [=](Plan* p, cudaStream_t st) {
       launch_prep_input<T>(p->cur.x, p->cur.mu, X0, B, ic, Hh, Ww, Hp, Wp, pitch0, cond, st, 0, 0, 0, 0, 1);  // zero pad
-      cx->launches++;
-    }});
+      return 1;
+    });
     T* xin = alloc(np0 * w);
-    conv("intro.weight", V{X0, pitch0, C0}, hs[0], ws[0], 3, 1, 1, 1, "intro.bias", "", 0, nullptr, V{xin, w, w}, w);
+    conv({.w = "intro.weight", .in = V{X0, pitch0, C0}, .H = Hp, .W = Wp, .K = 3, .bias = "intro.bias", .out = V{xin, w, w}});
     V cur{xin, w, w};
     std::vector<V> encs;
     char nb[64];
     for (int i = 0; i < n.n_enc; ++i) {
       const int c = w << i;
-      const long long npix = (long long)B * hs[i] * ws[i];
+      const long long npix = (long long)B * lv.h(i) * lv.w(i);
       for (int j = 0; j < n.enc[i]; ++j) {
         T* o = alloc(npix * c);
         snprintf(nb, sizeof nb, "encoders.%d.%d.", i, j);
-        nafblock(nb, cur, V{o, c, c}, hs[i], ws[i]);
+        nafblock(nb, cur, V{o, c, c}, lv.h(i), lv.w(i));
         cur = V{o, c, c};
       }
       encs.push_back(cur);
-      T* d = alloc((long long)B * hs[i + 1] * ws[i + 1] * 2 * c);
+      T* d = alloc((long long)B * lv.h(i + 1) * lv.w(i + 1) * 2 * c);
       snprintf(nb, sizeof nb, "downs.%d.", i);
-      std::string wn = std::string(nb) + "weight", bn = std::string(nb) + "bias";
-      conv(wn, cur, hs[i], ws[i], 2, 2, 0, 1, bn.c_str(), "", 0, nullptr, V{d, 2 * c, 2 * c}, 2 * c);
+      conv({.w = std::string(nb) + "weight", .in = cur, .H = lv.h(i), .W = lv.w(i), .K = 2, .stride = 2,
+            .bias = std::string(nb) + "bias", .out = V{d, 2 * c, 2 * c}});
       cur = V{d, 2 * c, 2 * c};
     }
     {
       const int c = w << n.n_enc;
-      const long long npix = (long long)B * hs[n.n_enc] * ws[n.n_enc];
+      const long long npix = (long long)B * lv.h(n.n_enc) * lv.w(n.n_enc);
       for (int j = 0; j < n.middle; ++j) {
         T* o = alloc(npix * c);
         snprintf(nb, sizeof nb, "middle_blks.%d.", j);
-        nafblock(nb, cur, V{o, c, c}, hs[n.n_enc], ws[n.n_enc]);
+        nafblock(nb, cur, V{o, c, c}, lv.h(n.n_enc), lv.w(n.n_enc));
         cur = V{o, c, c};
       }
     }
     for (int i = 0; i < n.n_dec; ++i) {
       const int l = n.n_enc - 1 - i;           // level after upsampling
       const int chan = w << (l + 1), q = chan / 2;
-      const int hl = hs[l + 1], wl = ws[l + 1];
-      const long long np_lo = (long long)B * hl * wl, np_hi = (long long)B * hs[l] * ws[l];
+      const int hl = lv.h(l + 1), wl = lv.w(l + 1);
+      const long long np_lo = (long long)B * hl * wl, np_hi = (long long)B * lv.h(l) * lv.w(l);
       T* u = tmp(np_lo * 2 * chan);
       snprintf(nb, sizeof nb, "ups.%d.0.weight", i);
-      conv(nb, cur, hl, wl, 1, 1, 0, 1, nullptr, "", 0, nullptr, V{u, 2 * chan, 2 * chan}, 2 * chan);
+      conv({.w = nb, .in = cur, .H = hl, .W = wl, .K = 1, .out = V{u, 2 * chan, 2 * chan}});
       T* v = alloc(np_hi * q);
       V skip = encs[l];
-      plan->ops.push_back(OpRec{CAT_MISC, 0.0, [=](Plan*, cudaStream_t st) {
+      push_op(CAT_MISC, 0.0, std::string(nb) + " pixel_shuffle+skip", 0.0, [=](Plan*, cudaStream_t st) {
         launch_pixel_shuffle_add<T>(u, 2 * chan, skip.p, skip.pitch, v, q, B, hl, wl, q, st);
-        cx->launches++;
-      }});
-      plan->ops.back().label = std::string(nb) + " pixel_shuffle+skip";
+        return 1;
+      });
       release(u);
       cur = V{v, q, q};
       for (int j = 0; j < n.dec[i]; ++j) {
         T* o = alloc(np_hi * q);
         snprintf(nb, sizeof nb, "decoders.%d.%d.", i, j);
-        nafblock(nb, cur, V{o, q, q}, hs[l], ws[l]);
+        nafblock(nb, cur, V{o, q, q}, lv.h(l), lv.w(l));
         cur = V{o, q, q};
       }
     }
     if (n.latent) {  // latent variant: ending(x + encs[0]) with encs[0] = intro output
       T* e = alloc(np0 * w);
       V a = cur;
-      plan->ops.push_back(OpRec{CAT_MISC, 0.0, [=](Plan*, cudaStream_t st) {
+      push_op(CAT_MISC, 0.0, "", 0.0, [=](Plan*, cudaStream_t st) {
         launch_add<T>(a.p, a.pitch, xin, w, e, w, np0, w, st);
-        cx->launches++;
-      }});
+        return 1;
+      });
       cur = V{e, w, w};
     }
-    float* dummy = nullptr;
-    conv("ending.weight", cur, hs[0], ws[0], 3, 1, 1, 1, "ending.bias", "", 0, nullptr, V{nullptr, 0, 0}, ic, &dummy);
+    conv({.w = "ending.weight", .in = cur, .H = Hp, .W = Wp, .K = 3, .bias = "ending.bias", .out = V{nullptr, 0, ic}, .nchw = true});
   }
 
   void build() {
     const irsde_config& c = ctx->cfg;
     int B = plan->B, nf = c.nf, depth = c.depth;
     const std::vector<int>& D = ctx->udim;
-    int s = 1 << depth;
-    plan->Hp = plan->H + (s - plan->H % s) % s;
-    plan->Wp = plan->W + (s - plan->W % s) % s;
-    std::vector<int> hs(depth), ws(depth);
-    hs[0] = plan->Hp; ws[0] = plan->Wp;
-    for (int i = 1; i < depth; ++i) { hs[i] = hs[i - 1] / 2; ws[i] = ws[i - 1] / 2; }
+    const Levels lv = level_sizes(plan->H, plan->W, depth);
+    plan->Hp = lv.h(0);
+    plan->Wp = lv.w(0);
     bool cond = c.variant == IRSDE_NET_CONDITIONAL;
     int C0 = cond ? 2 * c.in_nc : c.in_nc;
     int pitch0 = (C0 + 7) / 8 * 8;
-    long long np0 = (long long)B * hs[0] * ws[0];
+    long long np0 = (long long)B * plan->Hp * plan->Wp;
     // linear-attention scratch sized for the largest level
-    float* la_partial = (float*)dev_alloc(ctx, linattn_partial_floats(B, hs[0] * ws[0]) * sizeof(float), &plan->allocs);
+    float* la_partial = (float*)dev_alloc(ctx, linattn_partial_floats(B, plan->Hp * plan->Wp) * sizeof(float), &plan->allocs);
     float* la_ctx = (float*)dev_alloc(ctx, (size_t)B * 4096 * sizeof(float), &plan->allocs);
     if (!la_partial || !la_ctx) { ok = false; err = "cudaMalloc failed"; return; }
 
     int in_nc = c.in_nc, Hh = plan->H, Ww = plan->W, Hp = plan->Hp, Wp = plan->Wp;
-    stem_padded = std::is_same<T, bf16>::value && ctx->use_tc && pitch0 == 8 && nf % 8 == 0;
-    long long x0_elems = stem_padded ? (long long)B * (Hp + 6) * (Wp + 8) * 8 + 64 : np0 * pitch0;
+    // X0 lives in the zero-bordered [B][Hp+6][Wp+8][8] layout of the tensor-core stem
+    const bool sp = std::is_same<T, bf16>::value && ctx->use_tc && pitch0 == 8 && nf % 8 == 0;
+    long long x0_elems = sp ? (long long)B * (Hp + 6) * (Wp + 8) * 8 + 64 : np0 * pitch0;
     T* X0 = alloc(x0_elems);
-    if (X0 && stem_padded) cudaMemset(X0, 0, (size_t)x0_elems * sizeof(T));  // borders stay zero forever
+    if (X0 && sp) cudaMemset(X0, 0, (size_t)x0_elems * sizeof(T));  // borders stay zero forever
     T* F = alloc(np0 * 2 * nf);
-    irsde_ctx* cx = ctx;
-    bool sp = stem_padded;
-    plan->ops.push_back(OpRec{CAT_MISC, 0.0, [=](Plan* p, cudaStream_t st) {
+    push_op(CAT_MISC, 0.0, "", 0.0, [=](Plan* p, cudaStream_t st) {
       if (sp) launch_prep_input<T>(p->cur.x, p->cur.mu, X0, B, in_nc, Hh, Ww, Hp, Wp, pitch0, cond ? 1 : 0, st, 3, 3, Wp + 8, Hp + 6);
       else launch_prep_input<T>(p->cur.x, p->cur.mu, X0, B, in_nc, Hh, Ww, Hp, Wp, pitch0, cond ? 1 : 0, st);
-      cx->launches++;
-    }});
-    conv("init_conv.weight", V{X0, pitch0, C0}, hs[0], ws[0], 7, 1, 3, 1, nullptr, "", 0, nullptr, view(F, 2 * nf, nf, nf), nf);
+      return 1;
+    });
+    conv({.w = "init_conv.weight", .in = V{X0, pitch0, C0}, .H = Hp, .W = Wp, .K = 7, .out = view(F, 2 * nf, nf, nf),
+          .stem_layout = sp});
     V cur = view(F, 2 * nf, nf, nf);
     std::vector<T*> U1(depth), U2(depth);
     char nb[64];
     for (int i = 0; i < depth; ++i) {
-      int di = D[i], dout = D[i + 1], H = hs[i], W = ws[i];
+      int di = D[i], dout = D[i + 1], H = lv.h(i), W = lv.w(i);
       long long npix = (long long)B * H * W;
       U1[i] = alloc(npix * (dout + di));
       U2[i] = alloc(npix * (dout + di));
@@ -1222,18 +1206,17 @@ struct Builder {
       attention(pre + "2.", V{ta, di, di}, s1, H, W, false, la_partial, la_ctx);
       release(ta);
       if (i != depth - 1) {
-        T* xn = alloc((long long)B * hs[i + 1] * ws[i + 1] * dout);
-        std::string bn = pre + "3.bias";
-        conv(pre + "3.weight", s1, H, W, 4, 2, 1, 1, bn.c_str(), "", 0, nullptr, V{xn, dout, dout}, dout);
+        T* xn = alloc((long long)B * lv.h(i + 1) * lv.w(i + 1) * dout);
+        conv({.w = pre + "3.weight", .in = s1, .H = H, .W = W, .K = 4, .stride = 2, .bias = pre + "3.bias", .out = V{xn, dout, dout}});
         cur = V{xn, dout, dout};
       } else {
         T* xn = alloc(npix * dout);
-        conv(pre + "3.weight", s1, H, W, 3, 1, 1, 1, nullptr, "", 0, nullptr, V{xn, dout, dout}, dout);
+        conv({.w = pre + "3.weight", .in = s1, .H = H, .W = W, .K = 3, .out = V{xn, dout, dout}});
         cur = V{xn, dout, dout};
       }
     }
     {
-      int i = depth - 1, di = D[i], mid = D[depth], H = hs[i], W = ws[i];
+      int i = depth - 1, di = D[i], mid = D[depth], H = lv.h(i), W = lv.w(i);
       long long npix = (long long)B * H * W;
       T* m1 = tmp(npix * mid);
       T* m2 = tmp(npix * mid);
@@ -1244,7 +1227,7 @@ struct Builder {
       release(m2);
     }
     for (int j = 0; j < depth; ++j) {
-      int i = depth - 1 - j, di = D[i], dout = D[i + 1], H = hs[i], W = ws[i];
+      int i = depth - 1 - j, di = D[i], dout = D[i + 1], H = lv.h(i), W = lv.w(i);
       long long npix = (long long)B * H * W;
       snprintf(nb, sizeof nb, "ups.%d.", j);
       std::string pre = nb;
@@ -1256,19 +1239,17 @@ struct Builder {
       release(tb);
       if (i != 0) {
         int dprev = D[i];  // == dout of level i-1
-        std::string bn = pre + "3.1.bias";
-        conv(pre + "3.1.weight", V{tc, dout, dout}, H, W, 3, 1, 1, 2, bn.c_str(), "", 0, nullptr,
-             view(U1[i - 1], dprev + D[i - 1], 0, dprev), di);
+        conv({.w = pre + "3.1.weight", .in = V{tc, dout, dout}, .H = H, .W = W, .K = 3, .up = 2, .bias = pre + "3.1.bias",
+              .out = view(U1[i - 1], dprev + D[i - 1], 0, dprev)});
       } else {
-        conv(pre + "3.weight", V{tc, dout, dout}, H, W, 3, 1, 1, 1, nullptr, "", 0, nullptr, view(F, 2 * nf, 0, nf), di);
+        conv({.w = pre + "3.weight", .in = V{tc, dout, dout}, .H = H, .W = W, .K = 3, .out = view(F, 2 * nf, 0, nf)});
       }
       release(tc);
     }
     T* G = tmp(np0 * nf);
-    resblock("final_res_block.", V{F, 2 * nf, 2 * nf}, nf, V{G, nf, nf}, hs[0], ws[0]);
-    float* dummy = nullptr;
-    conv("final_conv.weight", V{G, nf, nf}, hs[0], ws[0], 3, 1, 1, 1, "final_conv.bias", "", 0, nullptr, V{nullptr, 0, 0},
-         c.out_nc, &dummy);
+    resblock("final_res_block.", V{F, 2 * nf, 2 * nf}, nf, V{G, nf, nf}, Hp, Wp);
+    conv({.w = "final_conv.weight", .in = V{G, nf, nf}, .H = Hp, .W = Wp, .K = 3, .bias = "final_conv.bias",
+          .out = V{nullptr, 0, c.out_nc}, .nchw = true});
   }
 };
 
@@ -1311,19 +1292,13 @@ int build_plan(irsde_ctx* ctx, int B, int H, int W, Plan** out) {
   auto it = ctx->plans.find(key);
   if (it != ctx->plans.end()) { it->second->last_use = ++ctx->use_clock; *out = it->second; return IRSDE_OK; }
   if (B <= 0 || H <= 0 || W <= 0) return fail(ctx, IRSDE_ERR_INVALID, "bad image shape");
-  {
-    // every level runs on the image padded to a multiple of 2^levels; the denoising UNet's mid_attn is full attention
-    const long long sp = 1LL << (ctx->lat.on ? ctx->lat.depth : ctx->naf.on ? ctx->naf.n_enc : ctx->cfg.depth);
-    const bool full = !ctx->lat.on && !ctx->naf.on && ctx->cfg.variant == IRSDE_NET_DENOISING;
-    if (int rc = check_shape_limits(ctx, full ? 4LL * B : B, full ? "4 B (full-attention grid rows)" : "B",
-                                    (H + sp - 1) / sp * sp, (W + sp - 1) / sp * sp))
-      return rc;
-  }
+  // the denoising UNet's mid_attn is full attention
+  const Levels lv = level_sizes(H, W, ctx->lat.on ? ctx->lat.depth : ctx->naf.on ? ctx->naf.n_enc : ctx->cfg.depth);
+  const bool full = !ctx->lat.on && !ctx->naf.on && ctx->cfg.variant == IRSDE_NET_DENOISING;
+  if (int rc = check_shape_limits(ctx, full ? 4LL * B : B, full ? "4 B (full-attention grid rows)" : "B", lv.Hp, lv.Wp)) return rc;
   const long long bytes_before = ctx->dev_bytes;
-  int s = 1 << ctx->cfg.depth;
   // reflect pad needs pad < size (F.pad 'reflect' raises otherwise, DenoisingUNet_arch.py:82)
-  if (!ctx->naf.on && ((s - H % s) % s >= H || (s - W % s) % s >= W))
-    return fail(ctx, IRSDE_ERR_INVALID, "image too small for reflect padding");
+  if (!ctx->naf.on && (lv.Hp - H >= H || lv.Wp - W >= W)) return fail(ctx, IRSDE_ERR_INVALID, "image too small for reflect padding");
   Plan* p = new Plan();
   p->B = B; p->H = H; p->W = W;
   std::string err;
@@ -1373,7 +1348,7 @@ int build_plan(irsde_ctx* ctx, int B, int H, int W, Plan** out) {
 
 void run_ops(irsde_ctx* ctx, Plan* p, std::vector<OpRec>& ops, cudaStream_t st) {
   if (!ctx->prof) {
-    for (auto& op : ops) op.fn(p, st);
+    for (auto& op : ops) ctx->launches += op.fn(p, st);
     return;
   }
   for (auto& op : ops) {
@@ -1381,7 +1356,7 @@ void run_ops(irsde_ctx* ctx, Plan* p, std::vector<OpRec>& ops, cudaStream_t st) 
     cudaEventCreate(&e0);
     cudaEventCreate(&e1);
     cudaEventRecord(e0, st);
-    op.fn(p, st);
+    ctx->launches += op.fn(p, st);
     cudaEventRecord(e1, st);
     ctx->prof_events.push_back({op.cat, op.flops, e0, e1, &op});
   }
@@ -1563,22 +1538,6 @@ int32_t* zeroed_info(int32_t* info, int32_t* local) {
   return info;
 }
 
-// Which of the tap-GEMM's conv shapes (tap_table) a standalone conv is: 3x3/1 pad 1 (also after nearest x2), 1x1, 4x4/2
-// pad 1 or 2x2/2 pad 0 over an even H x W, or the 7x7/1 pad 3 stem.  Each entry applies its own engine rules on top.
-struct ConvShape {
-  bool k3, k1, k4, k2, k7;
-};
-ConvShape conv_shape(int KH, int KW, int stride, int pad, int up, int H, int W) {
-  const bool even = up == 1 && H % 2 == 0 && W % 2 == 0;
-  return ConvShape{KH == 3 && KW == 3 && stride == 1 && pad == 1, KH == 1 && KW == 1 && stride == 1 && pad == 0 && up == 1,
-                   KH == 4 && KW == 4 && stride == 2 && pad == 1 && even, KH == 2 && KW == 2 && stride == 2 && pad == 0 && even,
-                   KH == 7 && KW == 7 && stride == 1 && pad == 3 && up == 1};
-}
-ConvGeom conv_geom(int B, int Cin, int H, int W, int Cout, int KH, int KW, int stride, int pad, int up) {
-  return ConvGeom{B, H, W, Cin, up, KH, KW, stride, pad, (H * up + 2 * pad - KH) / stride + 1, (W * up + 2 * pad - KW) / stride + 1,
-                  Cout};
-}
-
 // Runs the conv the plan builder would make of this shape on the tap-GEMM (S = bf16, or fp32 for the fp32x3 engine), with
 // the operands of run_conv.  As in a plan, the time table of `ep` (ss, t_ptr, ss_img_stride) is attached after the
 // descriptor is created.
@@ -1743,10 +1702,9 @@ int irsde_latent_decode(irsde_ctx* ctx, const float* z, float* out, int32_t B, i
 }
 int irsde_latent_shape(irsde_ctx* ctx, int32_t H, int32_t W, int32_t* lat_h, int32_t* lat_w) {
   if (!ctx || !ctx->lat.on || !lat_h || !lat_w) return fail(ctx, IRSDE_ERR_INVALID, "bad argument");
-  const int s = 1 << ctx->lat.depth;
-  const int Hp = H + (s - H % s) % s, Wp = W + (s - W % s) % s;
-  *lat_h = Hp >> (ctx->lat.depth - 1);
-  *lat_w = Wp >> (ctx->lat.depth - 1);
+  const Levels lv = level_sizes(H, W, ctx->lat.depth);
+  *lat_h = lv.h(ctx->lat.depth - 1);
+  *lat_w = lv.w(ctx->lat.depth - 1);
   return IRSDE_OK;
 }
 
@@ -1949,11 +1907,7 @@ int irsde_finalize_weights(irsde_ctx* ctx) {
   if (ctx->raw.size() != specs.size()) return fail(ctx, IRSDE_ERR_INVALID, "unexpected extra state-dict entries");
   // conv weights -> engine layouts (buffers are allocated once; reload keeps pointers stable)
   for (auto& s : specs) {
-    if (s.shape.size() != 4) continue;  // vectors / Linear matrices stay fp32 as loaded
-    if (s.name.size() > 2 && s.name.substr(s.name.size() - 2) == ".g") continue;
-    if (ctx->naf.on && (s.shape[0] == 1 || s.name.find("conv2.weight") != std::string::npos ||
-                        s.name.find("sca.1.weight") != std::string::npos))
-      continue;  // beta/gamma vectors, depthwise and SCA weights are consumed raw
+    if (s.pack == PACK_RAW) continue;
     const int Cout = (int)s.shape[0], Cin = (int)s.shape[1], KH = (int)s.shape[2], KW = (int)s.shape[3];
     const float* raw = ctx->raw[s.name].dev;
     auto pack_into = [&](auto*& buf, WLayout l) {
@@ -1963,11 +1917,10 @@ int irsde_finalize_weights(irsde_ctx* ctx) {
       return buf != nullptr;
     };
     if (!pack_into(ctx->w_simt[s.name], WL_SIMT)) return fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
-    // the tap-GEMM runs a 7x7 conv only as the bf16 stem over at most 8 input channels; the Upsample convs (".3.1.") are
-    // nearest x2 + 3x3
+    // the tap-GEMM runs a 7x7 conv only as the bf16 stem over at most 8 input channels
     const bool bf = ctx->cfg.precision == IRSDE_PREC_BF16;
     if (ctx->cfg.precision == IRSDE_PREC_FP32 || (KH == 7 && !(bf && Cin <= 8))) continue;
-    const WLayout l = KH == 7 ? WL_STEM : (KH == 3 && s.name.find(".3.1.weight") != std::string::npos ? WL_UP : WL_TAPS);
+    const WLayout l = KH == 7 ? WL_STEM : s.pack == PACK_UP ? WL_UP : WL_TAPS;
     if (!(bf ? pack_into(ctx->w_tc[s.name], l) : pack_into(ctx->w_tc3[s.name], l))) return fail(ctx, IRSDE_ERR_CUDA, "cudaMalloc failed");
   }
   // time-modulation: concatenate every block's mlp.1 into one [S][td_in] matrix
@@ -2279,7 +2232,7 @@ int irsde_trace_forward(irsde_ctx* ctx, const float* x, const float* mu, const f
   time_rows(ctx, p->fwd_times, n_times, p->fwd_temb, p->fwd_table, st);
   p->cur.x = x; p->cur.mu = mu; p->cur.out = p->eps_buf;
   p->cur.ss = p->fwd_table; p->cur.t_ptr = p->d_zero; p->cur.ss_img_stride = (n_times > 1) ? 1 : 0;
-  for (int i = 0; i <= op; ++i) p->ops[i].fn(p, st);
+  for (int i = 0; i <= op; ++i) ctx->launches += p->ops[i].fn(p, st);
   if (ctx->cfg.precision != IRSDE_PREC_BF16)
     launch_nhwc_to_nchw<float>((const float*)r.out_p, r.out_pitch, dump, B, r.out_C, r.out_H, r.out_W, st);
   else
